@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- rays/sec of the NeO-360 ray-marching hot path on B200 (BASELINE.json metric).
+"""bench.py -- rays/sec of the NeO-360 ray-marching hot path on H100 (BASELINE.json metric).
 
 Workload (BASELINE.json configs[1]): NeO-360 tri-planar render, 3 source views, 640x480 target frame,
 128 coarse + 64 fine samples per ray and branch (129 + 193 points, fg and bg => 644 field evaluations per ray,
@@ -8,6 +8,7 @@ One "step" = one full frame (307 200 rays) through the hot path.  N GPUs: every 
 turntable (weak scaling, no data-path collective), value = all rays of all ranks / max-over-ranks device time.
 
   python bench.py [--gpus N] [--steps K] [--warmup W]            our CUDA path
+  python bench.py ... --dump-outputs DIR                         + the last timed step's outputs as DIR/<name>.npy (float32)
   python bench.py --impl reference [...]                         the reference algorithm (CPU oracle port) on host cores
 
 Prints ONE JSON line (rank 0).  See the prompt contract for the keys; `roofline` is for the dominant kernel (the
@@ -30,8 +31,8 @@ FLOP_PER_POINT = {0: 2 * 770688, 1: 2 * 786816}          # fg, bg
 POINTS_PER_RAY = (N_COARSE + 1) + (N_COARSE + 1 + N_FINE)  # per branch
 FLOP_PER_RAY = POINTS_PER_RAY * (FLOP_PER_POINT[0] + FLOP_PER_POINT[1])   # 1.003 GFLOP
 # MACs the TC path actually needs per point (mean of fg/bg): per view the re-associated trunk 128*(KE+128+128+128+KE), the bilinear
-# blend of the 4 maps (16 taps x 256 projected channels, on the tensor pipe since round 2) and the folded head 80*128; once per
-# point the direction / colour head 80*32 + 64*64 + 16*64.  Padding of the tcgen05 tiles (window slots without a tap, K 63->64) is
+# blend of the 4 maps (16 taps x 256 projected channels) and the folded head 80*128; once per
+# point the direction / colour head 80*32 + 64*64 + 16*64.  Padding of the wgmma tiles (K 63->64, N 65->80) is
 # NOT counted: this is the useful work the tensor pipe has to do, the denominator of the honest roofline fraction.
 ISSUED_MAC_PER_POINT = 0.5 * sum(3 * (128 * (2 * ke + 384) + 16 * 256 + 80 * 128) + 80 * 32 + 64 * 64 + 16 * 64 for ke in (64, 96))
 
@@ -51,7 +52,7 @@ def parse():
                     help="frames: BASELINE configs[1], one frame per rank (the headline, default); strong: ONE 640x480 frame split over the ranks "
                          "+ NCCL all-gather of the pixels (models/interface.py:30-50); turntable: BASELINE configs[4], views sharded first; "
                          "train: BASELINE configs[3], 4096-ray batches with an NCCL gradient all-reduce; mip360: BASELINE configs[2], "
-                         "Mip-NeRF 360 at 640x480 with 64+64+64 samples, every dense layer on tcgen05")
+                         "Mip-NeRF 360 at 640x480 with 64+64+64 samples, every dense layer on the tensor cores")
     ap.add_argument("--views", type=int, default=100, help="turntable mode: number of target views")
     ap.add_argument("--batch-rays", type=int, default=4096, help="train mode: rays per optimisation step over all ranks")
     ap.add_argument("--train-matmul", choices=("fp32", "tf32"), default="fp32",
@@ -61,6 +62,9 @@ def parse():
                     help="train mode: projected = map columns of layers 0/3 applied to the feature maps once per step (exact re-association, default); "
                          "reference = the reference's row-by-row K=703/831 input layers")
     ap.add_argument("--freeze-encoder", action="store_true", help="train mode: MLPs only (finetune mode); default trains GridEncoder inside the step")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="frames mode: after the timed steps write the outputs of the last timed step (rgb, fg_rgb, bg_rgb, depth, fg_acc of "
+                         "every ray of the frame) as DIR/<name>.npy in float32, to compare two builds output for output")
     return ap.parse_args()
 
 
@@ -69,7 +73,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return {"bf16_tflops": d["bf16_tflops_sustained"], "burst": d["bf16_tflops"], "hbm_gbs": d["hbm_gbs"], "src": "measured (MEASURED_PEAKS.json, sustained)"}
-    return {"bf16_tflops": 1400.0, "burst": 1590.0, "hbm_gbs": 6650.0, "src": "fallback (B200_PROFILING.md)"}
+    # NVIDIA H100 SXM data sheet (700 W card), dense fp16/bf16 tensor rate and HBM3 bandwidth: bounds, never reached figures
+    return {"bf16_tflops": 989.0, "burst": 989.0, "hbm_gbs": 3350.0, "src": "NVIDIA H100 SXM data sheet (dense fp16/bf16, 700 W)"}
 
 
 class ClockSampler(threading.Thread):
@@ -207,6 +212,14 @@ def eager_gpu_rates(sc, P, dev, steps=2, warmup=1, n_chunks=8):
     return res
 
 
+def dump_outputs(path, out):
+    """The arrays the timed path returned in its last step, as float32 .npy files (a 640x480 frame: 11 MB in all)."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    for k, v in out.items():
+        np.save(os.path.join(path, f"{k}.npy"), v.detach().float().cpu().numpy())
+
+
 def main():
     args = parse()
     rank = int(os.environ.get("RANK", "0"))
@@ -300,8 +313,11 @@ def main():
 
     wh = (IMG_W, IMG_H) if (n == IMG_W * IMG_H and not os.environ.get("NEO360_NO_BLOCK_ORDER")) else None
 
+    last = {}
+
     def step_resident(s):
-        return net.render_rays_test(devrays[s % len(devrays)], chunk=CHUNK, img_wh=wh)
+        last["out"] = net.render_rays_test(devrays[s % len(devrays)], chunk=CHUNK, img_wh=wh)
+        return last["out"]
 
     in_o, in_d = torch.empty(n, 3, device=dev), torch.empty(n, 3, device=dev)        # device staging of the per-step inputs
     out_rgb, out_depth = torch.empty(n, 3).pin_memory(), torch.empty(n).pin_memory()   # contiguous pinned outputs (one DMA each)
@@ -338,6 +354,8 @@ def main():
     sampler = ClockSampler(local) if rank == 0 else None
     lib.neo_profile(0)
     ms_res = timed(step_resident, sampler)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last["out"])
     launches = C.c_ulonglong()
     lib.neo_profile_read(None, None, C.byref(launches), None)
     net.check()
@@ -406,11 +424,11 @@ def main():
         "metric": "rays/sec at 640x480, 192 samples/ray", "value": value, "unit": "rays/s", "n_gpus": world,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_res / args.steps, "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None,
-        "dtype": "f16 operands, f32 accumulate (tcgen05)" if args.precision == "tc" else "f32",
+        "dtype": "f16 operands, f32 accumulate (wgmma)" if args.precision == "tc" else "f32",
         "data": "synthetic",
         "config": {"workload": workload, "rays_per_step_per_gpu": n, "chunk": CHUNK, "precision": args.precision,
                    "parallelism": f"ray-sharded x{world} (one frame per rank, no collective)",
-                   "l2": "inputs larger than L2 (feature maps + per-sample workspace >> 126 MB)",
+                   "l2": "inputs larger than L2 (feature maps + per-sample workspace >> 50 MB)",
                    "valid_headline": n == IMG_W * IMG_H},
         "roofline": {"bound": "tensor", "achieved": ach, "peak": pk["bf16_tflops"], "unit": "TFLOP/s",
                      "frac": ach / pk["bf16_tflops"], "traffic": traffic, "peak_source": pk["src"],

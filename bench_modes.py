@@ -83,7 +83,7 @@ def run(args, rank, world, local, dev, dist, pk):
             ref = net.render_rays_test({"rays_o": o, "rays_d": d, "viewdirs": d}, chunk=B.CHUNK)
         diff = float((full["px"][:, :3] - ref["rgb"]).abs().max())
         line = dict(base, metric="rays/sec at 640x480, 192 samples/ray", value=n * args.steps / (ms * 1e-3), ms_per_step=ms / args.steps,
-                    scaling="strong", dtype="f16 operands, f32 accumulate (tcgen05)" if args.precision == "tc" else "f32",
+                    scaling="strong", dtype="f16 operands, f32 accumulate (wgmma)" if args.precision == "tc" else "f32",
                     config={"workload": "ONE neo360 640x480 frame (128+64 samples, 3 src views) split over the ranks on 1024-ray chunk boundaries, "
                                         "pixels (rgb+depth) all-gathered over NCCL inside the timed region", "rays_per_step": n,
                             "rays_per_rank": b - a, "chunk": B.CHUNK, "precision": args.precision,
@@ -121,7 +121,7 @@ def run(args, rank, world, local, dev, dist, pk):
             sampler.stop_flag = True
         rays = args.views * W * H * args.steps
         return dict(base, metric="rays/sec, 360-degree turntable at 1280x960, 256 samples/ray", value=rays / (ms * 1e-3), ms_per_step=ms / args.steps,
-                    scaling="strong", warmup=1, dtype="f16 operands, f32 accumulate (tcgen05)" if args.precision == "tc" else "f32",
+                    scaling="strong", warmup=1, dtype="f16 operands, f32 accumulate (wgmma)" if args.precision == "tc" else "f32",
                     config={"workload": f"full 360-degree turntable, {args.views} novel views at 1280x960, 128+128 samples (BASELINE configs[4]), "
                                         "rays generated on the device from the pose, rgb+depth copied back to pinned host memory per view",
                             "views_per_rank": len(views), "chunk": B.CHUNK, "precision": args.precision,
@@ -161,7 +161,7 @@ def run(args, rank, world, local, dev, dist, pk):
         flop_ray = 2.0 * (2 * npp * prop + nn_ * nerf)
         ach = rays * flop_ray / (ms * 1e-3) / 1e12
         return dict(base, metric="rays/sec at 640x480, 192 samples/ray (mipnerf360)", value=rays / (ms * 1e-3), ms_per_step=ms / args.steps,
-                    scaling="weak", dtype="f16 operands, f32 accumulate (tcgen05)" if args.precision == "tc" else "f32",
+                    scaling="weak", dtype="f16 operands, f32 accumulate (wgmma)" if args.precision == "tc" else "f32",
                     config={"workload": "mipnerf360 unbounded-contraction render, 640x480, 64+64 proposal + 64 NeRF samples (BASELINE configs[2]), "
                                         "rays generated on the device, rgb copied back to pinned host memory",
                             "rays_per_step_per_gpu": n, "rays_per_call": sub, "precision": args.precision,
@@ -203,7 +203,7 @@ def run(args, rank, world, local, dev, dist, pk):
         flop_ray = 2.0 * 593408 * ((nc + 1) + (nc + 1 + nf))               # SURVEY.md 8(d): 593 408 MAC per point
         ach = rays * flop_ray / (ms * 1e-3) / 1e12
         return dict(base, metric="rays/sec at 640x480, vanilla NeRF 64+128 samples", value=rays / (ms * 1e-3), ms_per_step=ms / args.steps,
-                    scaling="weak", dtype="f16 operands, f32 accumulate (tcgen05)" if args.precision == "tc" else "f32",
+                    scaling="weak", dtype="f16 operands, f32 accumulate (wgmma)" if args.precision == "tc" else "f32",
                     config={"workload": "vanilla NeRF two-level render, 640x480, 64 + 128 samples (65 + 193 points per ray), rays generated on the device",
                             "rays_per_step_per_gpu": n, "rays_per_call": sub, "precision": args.precision,
                             "parallelism": f"one frame per rank x{world}, no collective", "valid_headline": n == W * H},
@@ -226,21 +226,21 @@ def run(args, rank, world, local, dev, dist, pk):
         res = {}
         with torch.no_grad():
             lat = enc.spatial_encoder(imgs)
-            for name, fn in (("dense_cuda_tcgen05", lambda: enc.dense_cuda(lat, poses, focal, c, B.IMG_W, B.IMG_H)),
+            for name, fn in (("dense_cuda_tc", lambda: enc.dense_cuda(lat, poses, focal, c, B.IMG_W, B.IMG_H)),
                              ("dense_framework_fp32", lambda: enc.dense_torch(lat, poses, focal, c, B.IMG_W, B.IMG_H)),
                              ("whole_forward", lambda: enc(imgs, poses, focal, c))):
                 res[name] = _timed(lambda s: fn(), args.steps, args.warmup, dev, dist) / args.steps
         rows = B.NV * 64 ** 3
         flop = 2.0 * rows * (518 * 512 + 2 * 512 * 512 + 3 * (513 * 512 + 512))
         return dict(base, metric="GridEncoder scenes/sec (3 source views, 640x480)", unit="scenes/s", value=1e3 / res["whole_forward"],
-                    ms_per_step=res["whole_forward"], scaling="weak", dtype="f16 operands, f32 accumulate (tcgen05) for the dense part",
+                    ms_per_step=res["whole_forward"], scaling="weak", dtype="f16 operands, f32 accumulate (wgmma) for the dense part",
                     config={"workload": "GridEncoder.forward: ResNet-34 trunk (framework) + dense part (hand-written CUDA) + 3 conv stacks (framework)",
                             "rows": rows, "parallelism": "one scene per rank"},
-                    dense_part_ms=res, roofline={"bound": "tensor", "achieved": flop / (res["dense_cuda_tcgen05"] * 1e-3) / 1e12, "peak": pk["bf16_tflops"],
-                                                 "unit": "TFLOP/s", "frac": flop / (res["dense_cuda_tcgen05"] * 1e-3) / 1e12 / pk["bf16_tflops"],
+                    dense_part_ms=res, roofline={"bound": "tensor", "achieved": flop / (res["dense_cuda_tc"] * 1e-3) / 1e12, "peak": pk["bf16_tflops"],
+                                                 "unit": "TFLOP/s", "frac": flop / (res["dense_cuda_tc"] * 1e-3) / 1e12 / pk["bf16_tflops"],
                                                  "traffic": None, "peak_source": pk["src"],
                                                  "flops": f"{flop / 1e12:.2f} TFLOP of dense layers per scene over the dense part's time (gather, softmax sums included)"},
-                    speedup_dense_vs_framework_fp32=res["dense_framework_fp32"] / res["dense_cuda_tcgen05"])
+                    speedup_dense_vs_framework_fp32=res["dense_framework_fp32"] / res["dense_cuda_tc"])
 
     if args.mode == "train":
         from neo360_b200 import training

@@ -308,23 +308,8 @@ int neo_grid_encoder_dense(const NeoGridEncoderParams* params, const float* late
 int neo_profile(int enable);
 int neo_profile_read(float* field_ms, int* n_field, unsigned long long* launches, double* points);
 
-/* Self-test of the tcgen05 building blocks of the NEO_PREC_TC path (TMEM-resident A operand, 128B-swizzled K-major
- * operand tiles in K-major and MN-major form, TMEM loads): X (128,128), W (128,128), Wn (80,128) fp32 device ->
- * out1 = out3 (128,128) = W X^T (B operand K-major / MN-major), out2 = out4 (128,80) = X Wn^T (A operand K-major / MN-major),
- * computed with fp16 operands / fp32 accumulation. */
-int neo_tc_selftest(const float* X, const float* W, const float* Wn, float* out1, float* out2, float* out3, float* out4,
-                    void* stream);
-/* Self-test of the no-swizzle K-major operand descriptor (identity A operand): outa / outb (128,128) = X^T under the two readings
- * of the descriptor's LBO/SBO fields (outa is the one the library uses). */
-int neo_tc_selftest_transpose(const float* X, float* outa, float* outb, void* stream);
-/* Self-test of the texel-window MMA of the NEO_PREC_TC field kernel (the bilinear lookups on the tensor pipe): `texels` (H*W,256)
- * fp32 texel-major stands for one projected map, (ox,oy) is the top-left texel of a 4x4 window (may lie partly or wholly outside
- * the map: zero fill), wt (64,16) the tap weights of 64 points over the window's 16 texels (y-major).  The window is staged by one
- * TMA box load (cp.async.bulk.tensor, 128B swizzle) and multiplied on tcgen05:
- * out0[c][p] = sum_k texel(oy + k/4, ox + k%4)[c] * wt[p][k],  out3 the same for channels 128..255; both (128,64) fp32. */
-int neo_tc_selftest_window(const float* texels, int H, int W, int ox, int oy, const float* wt, float* out0, float* out3, void* stream);
-/* Stage-level entry point of the tensor-core dense layer used by the wide MLPs (csrc/gemm_tc.cu: 2-D TMA tile loads, tcgen05 MMAs,
- * double-buffered TMEM accumulators): A (M,K), W (N,K) fp32 device, bias (N) or NULL -> out (M,N) fp32 = act(fp16(A) . fp16(W)^T + bias)
+/* Stage-level entry point of the tensor-core dense layer used by the wide MLPs (csrc/gemm_tc.cu: 2-D TMA tile loads, wgmma with
+ * register accumulators): A (M,K), W (N,K) fp32 device, bias (N) or NULL -> out (M,N) fp32 = act(fp16(A) . fp16(W)^T + bias)
  * rounded to fp16.  K % 64 == 0, N % 64 == 0.  Synchronises the stream (allocates its fp16 staging buffers). */
 int neo_tc_dense(const float* A, const float* W, const float* bias, long long M, int N, int K, int relu, float* out, void* stream);
 /* Host-side view of the TC kernel's encoding-column layout (csrc/field_tc.cu enc_col<>): for in_ch = 3|4 and operand column
@@ -332,17 +317,11 @@ int neo_tc_dense(const float* A, const float* W, const float* bias, long long M,
  * -1 for the constant-one (bias) column, -2 for a zero padding column, -3 for invalid arguments.  Pure host code (no GPU). */
 int neo_tc_enc_column(int in_ch, int col);
 
-/* Diagnostics only, NOT for production callers: per-CTA cycle accounting of the NEO_PREC_TC field kernel into a caller-zeroed
- * device array of (#SMs x 64) int64 that must outlive every render issued while it is set; NULL disables (a separate
- * instantiation of the kernel carries the timers; production launches have none).  neo_scene_create resets it to NULL.
- * Slots: tools/tc_debug.py. */
-int neo_tc_debug(long long* buf);
-
-/* "" or a description of the mbarrier wait that timed out inside the NEO_PREC_TC field kernel (the kernel bounds every wait and
- * traps instead of hanging; the waiter's identity is recorded in host-mapped memory, which survives the failed context). */
+/* "" or a description of the mbarrier wait that timed out inside the NEO_PREC_TC field kernel (the kernel bounds its wait for the
+ * weight copies and traps instead of hanging; the waiter's identity is recorded in host-mapped memory, which survives the failed context). */
 const char* neo_tc_trap_info(void);
 const char* neo_last_error(void);
-/* "neo360_b200 <version> sm_100a" */
+/* "neo360_b200 <version> sm_90a" */
 const char* neo_version(void);
 
 #ifdef __cplusplus

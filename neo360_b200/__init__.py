@@ -1,4 +1,4 @@
-"""neo360_b200 -- B200-native (sm_100a) implementation of NeO-360's ray-marching hot path behind the reference's
+"""neo360_b200 -- H100-native (sm_90a) implementation of NeO-360's ray-marching hot path behind the reference's
 `model(rays, randomized, white_bkgd, near, far, out_depth)` call surface.  See DESIGN.md / INTEGRATION.md."""
 from . import synth  # noqa: F401
 

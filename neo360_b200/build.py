@@ -1,4 +1,4 @@
-"""Builds libneo360_b200.so in-tree with nvcc for sm_100a (no torch headers: the library is a plain C ABI)."""
+"""Builds libneo360_b200.so in-tree with nvcc for sm_90a (no torch headers: the library is a plain C ABI)."""
 import os
 import shutil
 import subprocess
@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libneo360_b200.so")
 SOURCES = ["scene.cu", "sampling.cu", "field_fp32.cu", "field_tc.cu", "render.cu", "vanilla.cu", "mip.cu", "gemm_tc.cu", "encoder.cu"]
-FLAGS = ["-shared", "-Xcompiler", "-fPIC", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3",
+FLAGS = ["-shared", "-Xcompiler", "-fPIC", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
          "-std=c++17", "--threads", "4"]
 
 

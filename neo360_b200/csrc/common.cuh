@@ -1,4 +1,4 @@
-// Shared device helpers for the NeO-360 hot path (sm_100a).  All math is fp32 and follows the order of
+// Shared device helpers for the NeO-360 hot path (sm_90a).  All math is fp32 and follows the order of
 // operations of the reference's eager PyTorch ops (separate mul / add kernels => no FMA contraction) wherever
 // a value feeds a discrete decision (sample positions, CDF brackets); see SURVEY.md Appendix A.
 #pragma once

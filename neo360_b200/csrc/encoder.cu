@@ -3,7 +3,7 @@
 //   world grid 64^3 -> per source view: camera transform, projection, bilinear lookup of the 512-channel latent image (zeros padding),
 //   [latent | camera xyz | unit direction to the camera * (z_cam < 1e-3)] -> DepthPillarEncoder 518 -> 512 -> 512 -> 512,
 //   three pillar aggregators (Linear 513 -> 512, ReLU, Linear 512 -> 1, softmax along one grid axis) -> weighted pillar sums.
-// 786 432 rows per scene at NV = 3: every dense layer runs on tcgen05 through gemm_f16 (csrc/gemm_tc.cu); the gather, the logit
+// 786 432 rows per scene at NV = 3: every dense layer runs on the tensor cores through gemm_f16 (csrc/gemm_tc.cu); the gather, the logit
 // reduction and the softmax-weighted pillar sum are the kernels below.  fp16 weights / activations, fp32 accumulation and softmax.
 #include "common.cuh"
 #include <cuda_fp16.h>

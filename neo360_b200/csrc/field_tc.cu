@@ -1,32 +1,24 @@
-// NEO_PREC_TC: the radiance field of NeO-360 on tcgen05 tensor cores (sm_100a), weight-stationary in TMEM.
+// NEO_PREC_TC: the radiance field of NeO-360 on Hopper tensor cores (sm_90a wgmma), weights resident in shared memory.
 //
 // Formulation (exact re-association of models/neo360/model.py:110-158, see DESIGN.md "TC path"):
 //   * bilinear lookups are linear, so the latent columns of layers 0 and 3 are applied to the feature maps once per
 //     scene:  P0 = W0[:, enc:] . F,  P3 = W3[:, 128+enc:] . F  (F = pixel-aligned latent or a tri-plane).  Per sample
-//     the kernel gathers 4 taps of [P0|P3] (256 fp16 channels) from 4 maps instead of 4 taps of 512+3*128 raw channels.
+//     the kernel blends 4 taps of [P0|P3] (256 fp16 channels) from 4 maps instead of 4 taps of 512+3*128 raw channels.
 //   * bottleneck_layer -> views_linear.0 has no nonlinearity in between and the view mean is linear, so
 //       q = (Wv0[:, :128] Wb / NV) . sum_v h3_v + Wv0[:, 128:] . mean_v(dir_enc_v) + (Wv0[:, :128] bb + bv0)
 //       sigma_raw = (w_sigma / NV) . sum_v h3_v + b_sigma
-//     i.e. the cross-view means become accumulation over the views in one TMEM accumulator.
-//   * trunk layers run transposed, D^T[neuron][point] = W[neuron][k] . X[point][k]:  the weights are the A operand and
-//     live in TMEM for the whole kernel (tcgen05.mma with A from TMEM), the activations X (fp16, 128B swizzle) are the
-//     B operand in shared memory.
-//   * everything additive rides on the tensor pipe: biases through a K=16 "bias MMA" (b1, b2) or a constant-one encoding
-//     column (b0, b3); the layer-3 skip input is accumulated into a second accumulator at layer-0 time.  The
-//     epilogue is tcgen05.ld -> cvt.f16x2 -> max.f16x2 -> 16-byte shared stores.
-//   * the bilinear lookups themselves run on the tensor pipe: the projected maps are stored as 64-channel groups
-//     [view*4 + group][y][x][64] so that ONE TMA box load (cp.async.bulk.tensor.4d, 128B swizzle) stages a 4x4 texel
-//     window of all 256 channels as an MN-major A operand; the producers only compute the 2x2 tap weights of each point
-//     and scatter them into a sparse [64 points x 16 texels] B tile.  D[channel][point] += WINDOW^T . TAPW^T is then
-//     the exact zero-padded bilinear blend, accumulated in fp32 (no per-lane gathers, no fp16 blend arithmetic).
-//     A 64-point job touches ~4 windows (quads of neighbouring pixels/samples share texels); windows live in an
-//     8-deep shared-memory ring filled by TMA and released by tcgen05.commit.
+//     i.e. the cross-view means become one register accumulator summed over the views.
+//   * b0 and b3 ride on a constant-one column of the positional encoding; b1, b2 and the head biases seed the accumulators.
 //
-// One CTA per SM, persistent over tiles of 128 points (32 rays x 4 consecutive samples); per tile the NV source views
-// are processed in turn, each as two half-jobs of 64 points.  Warp roles: 0-3 epilogue (TMEM lane quarters), 4 MMA issue,
-// 5-15 producers (geometry, positional encoding, tap weights, window enumeration + TMA issue).  Hand-offs are
-// mbarriers; tcgen05.commit signals MMA completion and releases producer slots.  DESIGN.md section 5 has the full story.
+// Layout: one persistent CTA per SM, two warpgroups, each working on its own tiles of 64 points (16 rays x 4 consecutive samples).
+// Every weight matrix of the branch's MLP (trunk, folded head, colour head: up to 200 KB fp16, 128-byte-swizzled K-major tiles) is
+// copied into shared memory once per CTA by TMA bulk copies.  Per (tile, view) a warpgroup runs the whole MLP as wgmma.mma_async
+// m64nNk16 with the activations as REGISTER A fragments: the fp32 accumulator of one layer is rectified, packed to fp16 and fed to
+// the next layer without touching shared memory.  The projected-map blends are added straight into the accumulators of layers 0 and
+// 3: the projected maps are stored with their channels in the accumulator-fragment order (pmap_logical), so the 32 channels a thread
+// owns for a point are 64 contiguous bytes of each texel (four 16-byte loads per tap, a quad of lanes reads whole 256-byte rows).
 #include "common.cuh"
+#include "hopper.cuh"
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cstdio>
@@ -34,72 +26,48 @@
 
 namespace neo {
 namespace tc {
+using namespace hopper;
 
-// 18 warps: 0-3 epilogue set A (block 0 + colour head), 4-7 epilogue set B (block 1), 8 MMA issue, 9-12 geometry, 13-16 texel windows
-// (one map each: latent, xz, xy, yz), 17 points + direction encoding.  Every hand-off is an mbarrier: the roles run decoupled, as far
-// ahead as their double-buffered slots and the window ring allow.  (5 warps on two of the four schedulers => 96 registers/thread.)
-#ifndef NEO_TRUNK_N64
-#define NEO_TRUNK_N64 1
-#endif
-#ifndef NEO_WIN_WARPS
-#define NEO_WIN_WARPS 4
-#endif
-constexpr int kMmaWarp = 8;
-constexpr int kGeomWarp0 = 9, kGeomWarps = 4;
-constexpr int kWinWarp0 = 13, kWinWarps = NEO_WIN_WARPS, kMapsPerWin = 4 / kWinWarps;
-constexpr int kMiscWarp = kWinWarp0 + kWinWarps;
-constexpr int kThreads = (kMiscWarp + 1) * 32;
-constexpr int kProducerWarp0 = 9;         // first non-consumer warp (set-up duties)
-constexpr int kProducerWarps = kMiscWarp + 1 - kProducerWarp0;
-constexpr int kTileRays = 32;
+constexpr int kTileRays = 16;
 constexpr int kTileSamples = 4;
-constexpr int kHalfPts = 64;          // producer->consumer unit: half a tile (32 rays x 2 samples) x 1 view
+constexpr int kTilePts = kTileRays * kTileSamples;  // = the M of one wgmma
+constexpr int kWarpgroups = 2;
+constexpr int kThreads = 128 * kWarpgroups;
 
-// ---- shared memory map (bytes; UMMA tiles 1024-aligned) ----
-constexpr uint32_t SM_ENC = 0;            // 2 slots x (64 x KE fp16, SW128 K-major, up to 2 slabs of 8 KB)
-constexpr uint32_t SM_H = 32768;          // 128 x 128 fp16, 2 slabs
-constexpr uint32_t SM_DIR = 65536;        // 128 x 64 fp16 (32 used), 1 slab
-constexpr uint32_t SM_WHEAD = 81920;      // head weights, B operands
+// head weights image (B operands, 128-byte swizzle): Whead_h 80 x 128 | Whead_dir 80 x 64 | Wv1 64 x 64 | Wrgb 16 x 64
 constexpr uint32_t WH_H = 0, WH_DIR = 20480, WH_V1 = 30720, WH_RGB = 38912, WH_BYTES = 40960;
-constexpr int kRing = 8;                  // texel-window ring depth
-constexpr uint32_t WIN_BYTES = 8192;      // one window: 4 channel groups x (16 texels x 128 B), SW128 MN-major A operand (TMA box 64 x 4 x 4 x 4)
-constexpr uint32_t WT_BYTES = 2048;       // its tap-weight tile: 64 points x 16 texels fp16, no-swizzle K-major B operand
-constexpr uint32_t SM_WIN = 122880;       // kRing x WIN_BYTES
-constexpr uint32_t SM_WT = SM_WIN + kRing * WIN_BYTES;       // 188416: kRing x WT_BYTES
-constexpr uint32_t SM_BIAS = SM_WT + kRing * WT_BYTES;       // 204800: fp32: b0..b3 (512) | bq (64) | bv1 (64) | brgb (4) | bsig (1)
-constexpr uint32_t SM_PTS = 207872;       // per-tile cache: 128 rows x 48 B (world points are view independent)
-constexpr uint32_t SM_VIEWS = 214016;     // kMaxViews x 64 B source-camera transforms
-constexpr uint32_t SM_BAR = 214528;       // mbarriers (8 B each) + TMEM base slot
-constexpr uint32_t SM_SEL = 215040;       // 32 x 128 B one-hot selector tile (SW128): B operand of the bias MMA, k-step l selects layer l
-constexpr uint32_t SM_ROWINFO = 219136;   // 2 slots x 4 maps x 64 rows x 16 B: (x0, y0 | dead, w_nw w_ne, w_sw w_se)
-constexpr uint32_t SM_CNT = 227328;       // 2 slots x 4 window counts | ring tail
-constexpr uint32_t SM_TOTAL = 227392;
-constexpr uint32_t SLOT_ENC = 16384, SLAB_ENC = 8192, SLOT_INFO = 4096;
-constexpr int BIAS_FLOATS = 512 + 64 + 64 + 4 + 4;
-constexpr uint32_t kDeadRow = 0x7fffffffu;
+constexpr int BIAS_FLOATS = 512 + 64 + 64 + 4 + 4;   // fp32: b0..b3 (512) | bq (64) | bv1 (64) | brgb (4) | bsig (1)
+constexpr uint32_t BIAS_BYTES = 2624;                // BIAS_FLOATS * 4 rounded up to 64
+constexpr uint32_t SLAB = 128 * 128;                 // one 64-column slab of a 128-row weight tile
 
-// TMEM column map (512 columns allocated)
-constexpr uint32_t TM_D = 0;        // trunk accumulator of layers 0-2 (2 blocks x 32 points)
-constexpr uint32_t TM_D3 = 64;      // layer-3 accumulator (2 x 32): seeded with W3enc.ENC + b3 + G3 at layer-0 time so the ENC / G slots free early
-constexpr uint32_t TM_DH = 128;     // head accumulator (80: 64 q + sigma + pad); afterwards the colour head's accumulators (64 | 16)
-constexpr uint32_t TM_BIAS = 208;   // A tile (K = 16) of the bias MMA: k = l holds the bias of trunk layer l (fp16)
-constexpr uint32_t TM_W = 224;      // weights: W0enc | W1 | W2 | W3h | W3enc   (fp16 pairs per column)
+// trunk weights image: W0enc | W1 | W2 | W3h | W3enc, each 128 rows (neurons) x K, K-major in 64-column slabs
+__host__ __device__ constexpr int enc_slabs(int KE) { return (KE + 63) / 64; }
+__host__ __device__ constexpr uint32_t trunk_off(int KE, int seg) { return seg == 0 ? 0u : (uint32_t)(enc_slabs(KE) + 2 * (seg - 1)) * SLAB; }
+__host__ __device__ constexpr uint32_t trunk_bytes(int KE) { return trunk_off(KE, 4) + (uint32_t)enc_slabs(KE) * SLAB; }
 
-// slot-indexed barriers come in pairs (slot 0, slot 1)
-// ACC_READY / H_READY are indexed by the 32-point block (0/1) of the half-job: the two blocks ping-pong between the
-// tensor core and the epilogue warps, so MMA latency hides behind the other block's epilogue.
-enum Bar { ENC_READY = 0, ENC_FREE = 2, CNT_READY = 4, ACC_READY = 6, H_READY = 8, INFO_READY = 10, INFO_FREE = 12, PTS_READY = 14, PTS_FREE = 16,
-           DIR_READY = 18, HEAD_READY, DIR_FREE,
-           Q_READY, CH_READY, HEAD_DONE,                  // colour head: q / v1 tile written, its MMA done, accumulator drained
-           WIN_FULL, WIN_EMPTY = WIN_FULL + kRing, NUM_BARS = WIN_EMPTY + kRing };
+// channel order of the projected maps: physical channel p of a texel holds logical channel pmap_logical(p) of [P0 | P3], so that
+// thread t (lane % 4) of an accumulator fragment finds its channels 8 j + 2 t + e (j < 16, e < 2) at p = 32 t + 2 j + e
+__host__ __device__ inline int pmap_logical(int p) {
+    const int q = p & 127, t = q >> 5, j = (q & 31) >> 1, e = q & 1;
+    return (p & 128) + 8 * j + 2 * t + e;
+}
+
+struct PtsRow {        // 48 bytes: view-independent data of one point of a tile
+    float xe[3];       // point fed to the positional encoding (fg: sample point, bg: unit-sphere point)
+    float tv;          // t (fg) or inverse radius s (bg)
+    float xl[3];       // lookup point (fg: same point, bg: far(1-s)+3s along the ray, quirk Q2)
+    int rid, sidx;     // ray and sample index
+    int src;           // ray whose view direction conditions this point (quirk Q1)
+    int valid;         // 0: padding row of the tile, its outputs are not stored
+    int pad;
+};
 
 struct MlpTc {
     int in_ch, enc_dim, KE;          // 3|4, 63|84, 64|96
-    const uint32_t* wimg;            // [KW/2][128] TMEM image words
+    const unsigned char* trunkimg;   // trunk_bytes(KE), pre-swizzled
+    const unsigned char* headimg;    // WH_BYTES, pre-swizzled
     const float* bias;               // BIAS_FLOATS
-    const uint4* headimg;            // WH_BYTES pre-swizzled
-    const __half* pmap[4];           // projected maps [P0|P3]: latent, xz, xy, yz; layout [nv*4 + channel group][H][W][64]
-    alignas(64) CUtensorMap tmap[4]; // their 4-D TMA descriptors (64 ch, W, H, nv*4), box 64 x 4 x 4 x 4, 128B swizzle
+    const __half* pmap[4];           // projected maps [P0|P3] of latent, xz, xy, yz: [nv][H][W][256] fp16 in pmap_logical order
 };
 
 struct State {
@@ -115,297 +83,15 @@ struct Params {
     MlpTc mlp;
     float* rgb_out;
     float* sigma_out;
-    int* err;
-    int* trap;          // host-mapped int[8]: who timed out on which mbarrier (mbar_timeout)
-    long long* dbg;     // optional [gridDim.x][kDbgStride] cycle counters (neo_tc_debug), null in production
+    int* trap;          // host-mapped int[8]: who timed out on the weight-load mbarrier
 };
-
-// back-off of the producers' slot waits (they run ahead of the tensor pipeline; see mbar_wait)
-#ifndef NEO_PROD_SLEEP_NS
-#define NEO_PROD_SLEEP_NS 0
-#endif
-constexpr int kProdSleep = NEO_PROD_SLEEP_NS;
-// consumer-side waits (MMA issue, epilogue): poll NEO_SPIN_POLLS times at full rate (the latency-critical hand-offs complete within
-// that), then back off so that a long wait does not flood the shared-memory / mbarrier pipe the producers' loads and stores need
-// suspend-time hint of mbarrier.try_wait (ns): the hardware parks a waiting thread for up to this long between checks of the phase;
-// with a long hint a waiter that has been parked for a while is woken late (measured: ~2 us after the phase flipped)
-#ifndef NEO_TRYWAIT_HINT_NS
-#define NEO_TRYWAIT_HINT_NS 2000
-#endif
-#ifndef NEO_SPIN_POLLS
-#define NEO_SPIN_POLLS 16
-#endif
-#ifndef NEO_SPIN_SLEEP_NS
-#define NEO_SPIN_SLEEP_NS 0
-#endif
-constexpr int kDbgStride = 64;
-// cycle accounting (neo_tc_debug): compiled only into the DBG instantiation of the kernel
-// event trace (DBG instantiation, CTA 0, first kTraceJobs half-jobs): int64 stamps at dbg[gridDim.x * kDbgStride + role * 1024 + job * 8 + k]
-constexpr int kTraceJobs = 120;
-#define TRACE(role, job, k, dep) do { if (DBG && P.dbg && blockIdx.x == 0 && (job) < kTraceJobs) { long long _ts; \
-    asm volatile("mov.u64 %0, %%clock64;" : "=l"(_ts) : "r"((uint32_t)(dep)) : "memory"); \
-    P.dbg[(size_t)gridDim.x * kDbgStride + (role) * 1024 + (job) * 8 + (k)] = _ts; } } while (0)
-#define TSTART() long long _t0 = DBG ? clock64() : 0
-#define TLAP(acc) do { if (DBG) { long long _t1 = clock64(); acc += _t1 - _t0; _t0 = _t1; } } while (0)
-
-// ------------------------------------------------------------------------------------------------
-// PTX wrappers
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-// whole-warp arrival: every lane has finished (and fenced) its writes, one lane signals
-__device__ __forceinline__ void mbar_arrive_warp(uint32_t bar, int lane) {
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar);
-}
-__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"      // %3: suspend-time hint (ns); wakes on completion
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok) : "r"(bar), "r"(parity), "r"((uint32_t)NEO_TRYWAIT_HINT_NS) : "memory");
-    return ok != 0;
-}
-// Wait on an mbarrier phase: asm loop with an in-register spin bound, so a protocol bug traps (launch failure reported by
-// neo_check_async / the next CUDA call) instead of hanging the GPU.  Before trapping, the waiter records (tag, CTA, thread, barrier,
-// parity) in a host-mapped buffer, which survives the dead context: neo_tc_trap_info() / neo_check_async print it.
-// SLEEP_NS > 0 backs off between polls: used by the producer warps, which run ahead of the tensor pipeline and must not steal
-// issue slots from the epilogue warps sharing their schedulers.
-__device__ __noinline__ void mbar_timeout(int* trapinfo, int tag, uint32_t bar, uint32_t parity) {
-    if (trapinfo) {
-        volatile int* t = trapinfo;
-        if (t[0] == 0) {
-            t[1] = (int)blockIdx.x; t[2] = (int)threadIdx.x; t[3] = (int)bar; t[4] = (int)parity; t[5] = (int)gridDim.x;
-            t[0] = tag + 1000;
-        }
-        __threadfence_system();
-    }
-    asm volatile("trap;");
-}
-template <int SLEEP_NS = 0>
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int* trapinfo, int tag) {
-    uint32_t ok;
-    if (SLEEP_NS > 0) {
-        asm volatile(
-            "{\n\t.reg .pred p, q;\n\t.reg .u32 c;\n\t"
-            "mov.u32 c, 0;\n\t"
-            "mov.u32 %0, 1;\n\t"
-            "NEO_WAIT_%=:\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-            "@p bra NEO_DONE_%=;\n\t"
-            "nanosleep.u32 %4;\n\t"
-            "add.u32 c, c, 1;\n\t"
-            "setp.lt.u32 q, c, 0x800000;\n\t"
-            "@q bra NEO_WAIT_%=;\n\t"
-            "mov.u32 %0, 0;\n\t"
-            "NEO_DONE_%=:\n\t}"
-            : "=r"(ok) : "r"(bar), "r"(parity), "r"((uint32_t)NEO_TRYWAIT_HINT_NS), "r"((uint32_t)SLEEP_NS) : "memory");
-    } else {
-        asm volatile(
-            "{\n\t.reg .pred p, q;\n\t.reg .u32 c;\n\t"
-            "mov.u32 c, 0;\n\t"
-            "mov.u32 %0, 1;\n\t"
-            "NEO_WAIT_%=:\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-            "@p bra NEO_DONE_%=;\n\t"
-            "add.u32 c, c, 1;\n\t"
-            "setp.gt.u32 q, c, %4;\n\t"
-            "@q nanosleep.u32 %5;\n\t"
-            "setp.lt.u32 q, c, 0x4000000;\n\t"
-            "@q bra NEO_WAIT_%=;\n\t"
-            "mov.u32 %0, 0;\n\t"
-            "NEO_DONE_%=:\n\t}"
-            : "=r"(ok) : "r"(bar), "r"(parity), "r"((uint32_t)NEO_TRYWAIT_HINT_NS), "r"((uint32_t)NEO_SPIN_POLLS), "r"((uint32_t)NEO_SPIN_SLEEP_NS) : "memory");
-    }
-    if (!ok) mbar_timeout(trapinfo, tag, bar, parity);
-}
-// one lane of a fully converged warp (the MMA warp keeps warp-uniform control flow so descriptors stay in uniform registers)
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-// TMA: one 4-D box (64 channels x 4 x 4 texels x 4 channel groups) of a projected map -> shared memory (128B swizzle);
-// out-of-range texels are zero-filled, which is exactly grid_sample's zeros padding
-__device__ __forceinline__ void tma_load_window(uint32_t dst, const CUtensorMap* tmap, int x, int y, int g, uint32_t bar) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-        ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(0), "r"(x), "r"(y), "r"(g), "r"(bar) : "memory");
-}
-
-// K-major, 128-byte-swizzled operand descriptor: rows of 128 B (64 fp16), 8-row groups 1024 B apart.
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);     // start address, 16-byte units
-    d |= (uint64_t)1 << 16;                       // leading byte offset (ignored for swizzled K-major; CUTLASS writes 1)
-    d |= (uint64_t)(1024u >> 4) << 32;            // stride byte offset between 8-row groups
-    d |= (uint64_t)1 << 46;                       // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;                       // SWIZZLE_128B
-    return d;
-}
-// K-major operand WITHOUT swizzle: core matrices of 8 rows x 16 B stored as 128 contiguous bytes; LBO = byte stride between the
-// core matrices of one 8-row group along K, SBO = byte stride between 8-row groups.
-__device__ __forceinline__ uint64_t desc_nosw(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)(lbo_bytes >> 4) << 16;
-    d |= (uint64_t)(sbo_bytes >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    return d;
-}
-// Shifted-identity tile (A operand of the "transpose-accumulate" MMA that adds the gathered features G[point][channel] into the
-// accumulator D[channel][point]): 240 rows x 16 k, zero except a 16x16 identity at rows 112..127.  The A operand of k-step s is
-// the 128-row window starting at row 112 - 16 s, whose identity block then sits at rows 16 s .. 16 s + 15.
-constexpr uint32_t IDENT_LBO = 128, IDENT_SBO = 256, IDENT_BYTES = 30 * 256;
-__device__ __forceinline__ void ident_fill(unsigned char* tile, int tid, int nthreads) {
-    for (int i = tid; i < (int)IDENT_BYTES / 16; i += nthreads) reinterpret_cast<uint4*>(tile)[i] = make_uint4(0u, 0u, 0u, 0u);
-}
-__device__ __forceinline__ void ident_ones(unsigned char* tile, int tid) {     // call after ident_fill + barrier, tid 0..15
-    if (tid < 16) {
-        const int r = 112 + tid, k = tid;
-        *reinterpret_cast<__half*>(tile + (r >> 3) * IDENT_SBO + (k >> 3) * IDENT_LBO + (r & 7) * 16 + (k & 7) * 2) = __float2half_rn(1.0f);
-    }
-}
-__device__ __forceinline__ uint64_t desc_ident(uint32_t tile_saddr, int ks, bool swap = false) {
-    const uint32_t a = tile_saddr + (uint32_t)(14 - 2 * ks) * IDENT_SBO;
-    return swap ? desc_nosw(a, IDENT_SBO, IDENT_LBO) : desc_nosw(a, IDENT_LBO, IDENT_SBO);
-}
-// MN-major, 128-byte-swizzled operand: 64 consecutive M/N elements (128 B) per K row, 8 K rows per 1024-B atom;
-// SBO = byte stride between 8-K-row atoms, LBO = byte stride between 64-element groups along M/N.
-__device__ __forceinline__ uint64_t desc_mn_sw128(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-// byte offset of element (mn, k) in an MN-major SW128 tile of 64 M/N elements (atoms of 8 K rows, contiguous)
-__host__ __device__ inline uint32_t mn128_off(int mn, int k) {
-    return (uint32_t)((k >> 3) * 1024 + (k & 7) * 128 + ((((mn & 63) >> 3) ^ (k & 7)) << 4) + (mn & 7) * 2);
-}
-// kind::f16 instruction descriptor: fp16 A/B, fp32 accumulate, K-major A and B
-__host__ __device__ constexpr uint32_t idesc_f16(int M, int N, int a_mn_major = 0, int b_mn_major = 0) {
-    return (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// D[tmem] (+)= A[tmem] . B[smem]^T     (A: M x 16 from TMEM, B: N x 16 K-major from smem)
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, {%5, %5, %5, %5}, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accum), "r"(0u) : "memory");
-}
-// D[tmem] (+)= A[smem] . B[smem]^T
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accum), "r"(0u) : "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-          "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]) : "memory");
-}
-
-__device__ __forceinline__ void sts128(uint32_t addr, uint4 v) {
-    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ void sts64(uint32_t addr, uint2 v) {
-    asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(v.x), "r"(v.y) : "memory");
-}
-__device__ __forceinline__ void sts16(uint32_t addr, unsigned short v) {
-    asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"(v) : "memory");
-}
-__device__ __forceinline__ uint4 lds128(uint32_t addr) {
-    uint4 v;
-    asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-    return v;
-}
-__device__ __forceinline__ unsigned short lds16(uint32_t addr) {
-    unsigned short v;
-    asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(addr));
-    return v;
-}
-__device__ __forceinline__ float lds_f32(uint32_t addr) {
-    float v;
-    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
-    return v;
-}
-__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
-// byte offset of element (row, k) inside a SW128 K-major tile whose slabs hold `rows` rows
-__host__ __device__ inline uint32_t sw128_off(int row, int k, int rows) {
-    int slab = k >> 6, kk = k & 63;
-    return (uint32_t)slab * (uint32_t)rows * 128u + (uint32_t)row * 128u + (uint32_t)((((kk >> 3) ^ (row & 7)) << 4) + (kk & 7) * 2);
-}
 
 // ------------------------------------------------------------------------------------------------
 // per-scene preparation kernels
 // ------------------------------------------------------------------------------------------------
 // Per scene and MLP the latent columns of layers 0 and 3 are applied to the raw feature maps once (linearity of the lookups):
-// P[(v*4 + n'/64)][p][n'%64] = sum_c Wsel[n'][c] * F[v][c][p],  n' in [0,256) = [P0 | P3] -- a plain contraction, run on tcgen05 by
-// gemm_f16 (csrc/gemm_tc.cu) from the two operands prepared below.
+// P[v][pixel][p] = sum_c Wsel[p][c] * F[v][c][pixel],  p in [0,256) = [P0 | P3] in pmap_logical order -- a plain contraction, run on
+// the tensor cores by gemm_f16 (csrc/gemm_tc.cu) from the two operands prepared below.
 // (n, C, HW) fp32 -> (n, HW, C) fp16: the A operand (pixels x channels, K-major) of the tensor-core pre-projection
 __global__ void nchw_to_nhwc_f16_kernel(const float* __restrict__ in, __half* __restrict__ out, int C, int HW) {
     __shared__ float tile[32][33];
@@ -422,20 +108,19 @@ __global__ void nchw_to_nhwc_f16_kernel(const float* __restrict__ in, __half* __
         if (c < C && p < HW) dst[(size_t)p * C + c] = __float2half_rn(tile[threadIdx.x][i]);
     }
 }
-// Wsel[r][c] fp16, r in [0,256): rows 0..127 = W0[r][col0 + c], rows 128..255 = W3[r - 128][col3 + c]   (the latent columns of layers 0 and 3)
+// Wsel[p][c] fp16, p in [0,256): logical row r = pmap_logical(p); rows 0..127 = W0[r][col0 + c], rows 128..255 = W3[r - 128][col3 + c]
+// (the latent columns of layers 0 and 3)
 __global__ void wsel_kernel(const float* __restrict__ w0, int ld0, int col0, const float* __restrict__ w3, int ld3, int col3, int C, __half* __restrict__ out) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= 256 * C) return;
-    const int r = idx / C, c = idx % C;
+    const int r = pmap_logical(idx / C), c = idx % C;
     out[idx] = __float2half_rn(r < 128 ? w0[(size_t)r * ld0 + col0 + c] : w3[(size_t)(r - 128) * ld3 + col3 + c]);
 }
 
 // ---- positional encoding of the camera-frame point (helper.py:121-125), tensor-core operand layout ----
-// The MMA does not care about the ORDER of the K columns as long as W0enc / W3enc use the same one (wimg_kernel), so the columns
-// are grouped per coordinate: [x, sin(2^0 x) .. sin(2^9 x), cos(2^0 x) .. cos(2^9 x)] -- 21 columns per coordinate, stride 21
+// The MMA does not care about the ORDER of the K columns as long as W0enc / W3enc use the same one (trunk_img_kernel), so the
+// columns are grouped per coordinate: [x, sin(2^0 x) .. sin(2^9 x), cos(2^0 x) .. cos(2^9 x)] -- 21 columns per coordinate, stride 21
 // (3 coordinates + the constant-one column 63 = 64 = KE) or stride 24 (4 coordinates, column 21 = constant one, KE = 96).
-// One thread produces KE/4 consecutive columns and needs at most two coordinates, whose 20 sines/cosines come from ONE
-// sin/cos evaluation and the double-angle recurrence instead of 20 range-reduced evaluations.
 struct EncCol { int kind, cc, lvl; };          // kind 0: zero, 1: constant one, 2: x, 3: sin level, 4: cos level
 template <int ICH>
 __host__ __device__ constexpr EncCol enc_col(int col) {
@@ -457,34 +142,35 @@ __host__ __device__ constexpr int enc_col_ref_index(int col) {
     if (e.kind == 4) return ICH + kPosDeg * ICH + e.lvl * ICH + e.cc;
     return -1;
 }
-// TMEM weight image: word j of neuron n = fp16(Wcat[n][2j]) | fp16(Wcat[n][2j+1]) << 16,
-// Wcat = [W0enc (KE) | W1 (128) | W2 (128) | W3h (128) | W3enc (KE)]
-__global__ void wimg_kernel(NeoMLPParams p, int enc_dim, int KE, uint32_t* __restrict__ out) {
-    const int KW = 2 * KE + 384;
-    int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= (KW / 2) * 128) return;
-    int j = idx / 128, n = idx % 128;
+__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
+    __half2 h = __floats2half2_rn(a, b);
+    return *reinterpret_cast<uint32_t*>(&h);
+}
+// trunk weights image (shared-memory bytes, 128-byte swizzle): element (neuron n, k) of segment s at trunk_off(KE, s) +
+// sw128_off(n, k, 128); segments W0enc (KE) | W1 | W2 | W3h (128 each) | W3enc (KE), encoding segments zero-padded to whole slabs
+__global__ void trunk_img_kernel(NeoMLPParams p, int enc_dim, int KE, unsigned char* __restrict__ img) {
+    const int es = enc_slabs(KE) * 64, KW = 2 * es + 384;
+    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= KW * 128) return;
+    const int n = idx / KW, kk = idx % KW;
     const int in_dim = enc_dim + kLocalCh + kWorldCh;
     const bool bg = (KE == 96);
     // encoding column `col` of the kernel's operand layout (enc_col<>): reference column, bias (constant-one column) or zero
     auto enc_w = [&](const float* w, size_t stride, size_t off0, const float* bias, int col) -> float {
+        if (col >= KE) return 0.f;
         const EncCol e = bg ? enc_col<4>(col) : enc_col<3>(col);
         if (e.kind == 1) return bias[n];
         const int ref = bg ? enc_col_ref_index<4>(col) : enc_col_ref_index<3>(col);
         return ref >= 0 ? w[(size_t)n * stride + off0 + ref] : 0.f;
     };
-    float v[2];
-    for (int h = 0; h < 2; ++h) {
-        int k = 2 * j + h;
-        float x;
-        if (k < KE) x = enc_w(p.w0, in_dim, 0, p.b0, k);
-        else if (k < KE + 128) x = p.w1[n * 128 + (k - KE)];
-        else if (k < KE + 256) x = p.w2[n * 128 + (k - KE - 128)];
-        else if (k < KE + 384) x = p.w3[(size_t)n * (128 + in_dim) + (k - KE - 256)];
-        else x = enc_w(p.w3, 128 + in_dim, 128, p.b3, k - KE - 384);
-        v[h] = x;
-    }
-    out[idx] = pack_h2(v[0], v[1]);
+    int seg, k;
+    float x;
+    if (kk < es) { seg = 0; k = kk; x = enc_w(p.w0, in_dim, 0, p.b0, k); }
+    else if (kk < es + 128) { seg = 1; k = kk - es; x = p.w1[n * 128 + k]; }
+    else if (kk < es + 256) { seg = 2; k = kk - es - 128; x = p.w2[n * 128 + k]; }
+    else if (kk < es + 384) { seg = 3; k = kk - es - 256; x = p.w3[(size_t)n * (128 + in_dim) + k]; }
+    else { seg = 4; k = kk - es - 384; x = enc_w(p.w3, 128 + in_dim, 128, p.b3, k); }
+    *reinterpret_cast<__half*>(img + trunk_off(KE, seg) + sw128_off(n, k, 128)) = __float2half_rn(x);
 }
 
 // head weights (pre-swizzled smem image) + folded biases
@@ -522,10 +208,6 @@ __global__ void head_kernel(NeoMLPParams p, int nv, unsigned char* __restrict__ 
         bias[idx] = x;
     }
 }
-
-// ------------------------------------------------------------------------------------------------
-// the field kernel
-// ------------------------------------------------------------------------------------------------
 
 // Fast-math restatement of ray_geom / fg_point / bg_point (common.cuh) for the TC path: the results only feed fp16
 // operands and bilinear coordinates, so FMA contraction, rsqrt and approximate division are fine here.
@@ -584,1011 +266,335 @@ __device__ __forceinline__ void tap_quad(float gx, float gy, int W, int H, TapQu
     t.w[3] = (inr & vx1 & vy1) ? fx * fy : 0.f;
 }
 
-struct PtsRow {        // 48 bytes: view-independent per-row data, computed once per tile
-    float xe[3];       // point fed to the positional encoding (fg: sample point, bg: unit-sphere point)
-    float tv;          // t (fg) or inverse radius s (bg)
-    float xl[3];       // lookup point (fg: same point, bg: far(1-s)+3s along the ray, quirk Q2)
-    int pad[5];
-};
-
-// one positional-encoding chunk (8 consecutive K elements) of row `x`
-template <int ICH, int SUB>
-__device__ __forceinline__ void enc_cols(const float* x, uint32_t encb, int row, bool zero) {
-    constexpr int KE = (ICH == 3) ? 64 : 96, CP = KE / 4, C0 = SUB * CP;
-    constexpr int STRIDE = (ICH == 3) ? 21 : 24;
-    constexpr int cA = (C0 / STRIDE < ICH) ? C0 / STRIDE : ICH - 1;
-    constexpr int cB = ((C0 + CP - 1) / STRIDE < ICH) ? (C0 + CP - 1) / STRIDE : ICH - 1;
-    float sn[2][kPosDeg], cs[2][kPosDeg];
-#pragma unroll
-    for (int w = 0; w < 2; ++w) {
-        if (w == 1 && cB == cA) break;
-        const float xv = x[w == 0 ? cA : cB];
-        float s = __sinf(xv), c = __cosf(xv);
-#pragma unroll
-        for (int k = 0; k < kPosDeg; ++k) {
-            sn[w][k] = s; cs[w][k] = c;
-            const float s2 = 2.f * s * c, c2 = fmaf(c, c, -s * s);
-            s = s2; c = c2;
+// ------------------------------------------------------------------------------------------------
+// the field kernel
+// ------------------------------------------------------------------------------------------------
+__device__ __noinline__ void load_timeout(int* trapinfo, uint32_t bar) {
+    if (trapinfo) {
+        volatile int* t = trapinfo;
+        if (t[0] == 0) {
+            t[1] = (int)blockIdx.x; t[2] = (int)threadIdx.x; t[3] = (int)bar; t[4] = 0; t[5] = (int)gridDim.x;
+            t[0] = 1000;
         }
+        __threadfence_system();
     }
-    float v[CP];
+    asm volatile("trap;");
+}
+
+__device__ __forceinline__ float sel4(const float* x, int i) { return i == 0 ? x[0] : i == 1 ? x[1] : i == 2 ? x[2] : x[3]; }
+
+// encoding column `col` (enc_col<> order) of the point x (3 coordinates, + t for the background MLP)
+template <int ICH>
+__device__ __forceinline__ float enc_value(const float* x, int col) {
+    const EncCol e = enc_col<ICH>(col);
+    if (e.kind == 0) return 0.f;
+    if (e.kind == 1) return 1.f;
+    const float xc = sel4(x, e.cc);
+    if (e.kind == 2) return xc;
+    const float a = xc * (float)(1 << e.lvl);            // exact: power-of-two scaling
+    return e.kind == 3 ? sinf(a) : cosf(a);
+}
+
+// column e of the direction encoding of the conditioning ray in one source camera's frame (model.py:357-360): [d, sin(2^k d),
+// sin(2^k d + pi/2)], 27 columns, zero beyond
+__device__ __forceinline__ float dir_value(const float* dc, int e) {
+    if (e >= kDirEnc) return 0.f;
+    if (e < 3) return sel4(dc, e);
+    const int q0 = e - 3;
+    const bool shifted = q0 >= 12;
+    const int qq = shifted ? q0 - 12 : q0;
+    const float xb = sel4(dc, qq % 3) * (float)(1 << (qq / 3));
+    return sinf(shifted ? xb + 1.57079637f : xb);
+}
+
+// rectified accumulator (NC columns) -> fp16 A fragments of the next layer (K = NC, NC / 16 k-steps)
+template <int NC>
+__device__ __forceinline__ void relu_to_frags(const float (&d)[NC / 2], uint32_t (&a)[NC / 16][4]) {
 #pragma unroll
-    for (int i = 0; i < CP; ++i) {
-        const EncCol e = enc_col<ICH>(C0 + i);
-        const int w = (e.cc == cA) ? 0 : 1;
-        v[i] = (e.kind == 1) ? 1.0f : (e.kind == 2) ? x[e.cc] : (e.kind == 3) ? sn[w][e.lvl] : (e.kind == 4) ? cs[w][e.lvl] : 0.f;
-        if (zero) v[i] = 0.f;
-    }
+    for (int ks = 0; ks < NC / 16; ++ks)
 #pragma unroll
-    for (int j = 0; j < CP / 8; ++j) {
-        const int c = C0 / 8 + j;
-        sts128(encb + (c >> 3) * SLAB_ENC + row * 128 + (((c & 7) ^ (row & 7)) << 4),
-               make_uint4(pack_h2(v[8 * j], v[8 * j + 1]), pack_h2(v[8 * j + 2], v[8 * j + 3]),
-                          pack_h2(v[8 * j + 4], v[8 * j + 5]), pack_h2(v[8 * j + 6], v[8 * j + 7])));
+        for (int r = 0; r < 4; ++r) a[ks][r] = pack_h2(fmaxf(d[8 * ks + 2 * r], 0.f), fmaxf(d[8 * ks + 2 * r + 1], 0.f));
+}
+// accumulator (NC columns) seeded with a bias vector (shared memory)
+template <int NC>
+__device__ __forceinline__ void seed_bias(float (&d)[NC / 2], const float* b, int t) {
+#pragma unroll
+    for (int j = 0; j < NC / 8; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) { d[4 * j + 2 * i] = b[8 * j + 2 * t]; d[4 * j + 2 * i + 1] = b[8 * j + 2 * t + 1]; }
+}
+// descriptor of k-step ks of a 128-byte-swizzled K-major weight tile whose 64-column slabs are `slab` bytes apart
+__device__ __forceinline__ uint64_t wdesc(uint32_t base, int ks, uint32_t slab) { return desc_sw128(base + (uint32_t)(ks >> 2) * slab + (uint32_t)(ks & 3) * 32u); }
+
+// acc[4 j + 2 i + e] += bilinear blend (grid_sample, align_corners=True, zeros) of channel 8 j + 2 t + e of half HALF of [P0 | P3]
+// over the four maps, at this thread's two points (camera-frame lookup points cl[i]) in source view v; fp32 blend of fp16 texels
+template <int HALF>
+__device__ __forceinline__ void blend_maps(float (&acc)[64], const Params& P, const float (&cl)[2][3], int v, int t) {
+    const SceneDev& sc = P.sc;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+#pragma unroll 1
+        for (int m = 0; m < 4; ++m) {
+            float gx, gy;
+            int mw, mh;
+            if (m == 0) {
+                local_grid_coords(sc, cl[i], gx, gy);
+                mw = sc.lat_w; mh = sc.lat_h;
+            } else {
+                gx = (m == 3) ? cl[i][1] : cl[i][0];
+                gy = (m == 2) ? cl[i][1] : cl[i][2];          // xz, xy, yz
+                mw = sc.plane_w; mh = sc.plane_h;
+            }
+            TapQuad tq;
+            tap_quad(gx, gy, mw, mh, tq);
+            const __half* base = P.mlp.pmap[m] + (size_t)v * mh * mw * 256 + HALF * 128 + t * 32;
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const float w = tq.w[k];
+                if (w == 0.f) continue;                        // out-of-range tap (zeros padding): its texel index may be invalid
+                const int x = tq.x0 + (k & 1), y = tq.y0 + (k >> 1);
+                const uint4* p = reinterpret_cast<const uint4*>(base + ((size_t)y * mw + x) * 256);
+                uint4 q[4];
+#pragma unroll
+                for (int u = 0; u < 4; ++u) q[u] = __ldg(p + u);
+#pragma unroll
+                for (int u = 0; u < 4; ++u) {
+                    const uint32_t wd[4] = {q[u].x, q[u].y, q[u].z, q[u].w};
+#pragma unroll
+                    for (int jj = 0; jj < 4; ++jj) {
+                        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&wd[jj]));
+                        const int j = 4 * u + jj;
+                        acc[4 * j + 2 * i] = fmaf(w, f.x, acc[4 * j + 2 * i]);
+                        acc[4 * j + 2 * i + 1] = fmaf(w, f.y, acc[4 * j + 2 * i + 1]);
+                    }
+                }
+            }
+        }
     }
 }
 
-template <int ICH, bool DBG>
+template <int KE>
+struct SmemMap {
+    static constexpr uint32_t HEAD = trunk_bytes(KE), BIAS = HEAD + WH_BYTES, VIEWS = BIAS + BIAS_BYTES,
+                              PTS = VIEWS + kMaxViews * 64, BAR = PTS + kWarpgroups * kTilePts * (uint32_t)sizeof(PtsRow), TOTAL = BAR + 16;
+};
+
+template <int ICH>
 __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_constant__ Params P) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
     unsigned char* sgen = smem_raw + (sbase - smem_u32(smem_raw));
-    constexpr int KE = (ICH == 3) ? 64 : 96;
+    constexpr int KE = (ICH == 3) ? 64 : 96, KS = KE / 16;
     constexpr bool IS_BG = (ICH == 4);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t bar0 = sbase + SM_BAR;
-    auto BAR = [&](int i) { return bar0 + 8u * i; };
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(sgen + SM_BAR + 8 * NUM_BARS);     // [NUM_BARS]: TMEM base, [NUM_BARS+1]: TMA barrier
+    using SM = SmemMap<KE>;
+    const uint32_t bar = sbase + SM::BAR;
 
-    // ---- one-time setup ----
+    // ---- one-time setup: every weight of the MLP -> shared memory (TMA bulk copies), source-camera transforms ----
     if (threadIdx.x == 0) {
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(BAR(ENC_READY + s), kGeomWarps);            // one elected arrival per geometry warp
-            mbar_init(BAR(ENC_FREE + s), 1);                      // tcgen05.commit after the layer-0 / skip MMAs that read the slot
-            mbar_init(BAR(CNT_READY + s), kWinWarps);             // the window warps posted their maps' window counts
-            mbar_init(BAR(INFO_READY + s), kGeomWarps);           // ROWINFO[s] written
-            mbar_init(BAR(INFO_FREE + s), kWinWarps);             // ... and read by the window warps
-            mbar_init(BAR(PTS_READY + s), 1);                     // world points of tile half s written by the point warp
-            mbar_init(BAR(PTS_FREE + s), kGeomWarps);             // ... and no longer needed (last view done)
-        }
-        mbar_init(BAR(DIR_READY), 1);
-        for (int r = 0; r < kRing; ++r) {
-            mbar_init(BAR(WIN_FULL + r), 2);                      // expect_tx arrival (+ 8 KB of TMA bytes) and the tap-weight tile
-            mbar_init(BAR(WIN_EMPTY + r), 1);                     // tcgen05.commit after the window's MMAs
-        }
-        *reinterpret_cast<volatile uint32_t*>(sgen + SM_CNT + 36) = 0u;     // issue turn: windows acquire their ring slots in sequence order
-        mbar_init(BAR(ACC_READY), 1);
-        mbar_init(BAR(ACC_READY + 1), 1);
-        mbar_init(BAR(H_READY), 4);
-        mbar_init(BAR(H_READY + 1), 4);
-        mbar_init(BAR(HEAD_READY), 1);
-        mbar_init(BAR(DIR_FREE), 1);
-        mbar_init(BAR(Q_READY), 4);
-        mbar_init(BAR(CH_READY), 1);
-        mbar_init(BAR(HEAD_DONE), 4);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init(bar, 1);
+        mbar_init_fence();
+        constexpr uint32_t TB = trunk_bytes(KE);
+        mbar_expect_tx(bar, TB + WH_BYTES + BIAS_FLOATS * 4);
+        for (uint32_t off = 0; off < TB; off += 32768u) bulk_load(sbase + off, P.mlp.trunkimg + off, min(32768u, TB - off), bar);
+        bulk_load(sbase + SM::HEAD, P.mlp.headimg, WH_BYTES, bar);
+        bulk_load(sbase + SM::BIAS, P.mlp.bias, BIAS_FLOATS * 4, bar);
     }
-    if (warp == kMmaWarp) tmem_alloc(sbase + SM_BAR + 8 * NUM_BARS, 512);
-    {   // head weights (pre-swizzled UMMA tiles) + biases -> smem with one TMA bulk copy each (cp.async.bulk, mbarrier tx-count)
-        const uint32_t tbar = BAR(NUM_BARS + 1);
-        if (threadIdx.x == 0) {
-            mbar_init(tbar, 1);
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-            const uint32_t bytes = WH_BYTES + BIAS_FLOATS * 4;
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(tbar), "r"(bytes) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(sbase + SM_WHEAD), "l"(P.mlp.headimg), "r"((uint32_t)WH_BYTES), "r"(tbar) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(sbase + SM_BIAS), "l"(P.mlp.bias), "r"((uint32_t)(BIAS_FLOATS * 4)), "r"(tbar) : "memory");
-        }
-        __syncthreads();
-        mbar_wait(tbar, 0, P.trap, 90);
-        float* vsm = reinterpret_cast<float*>(sgen + SM_VIEWS);
+    {
+        float* vsm = reinterpret_cast<float*>(sgen + SM::VIEWS);
         const float* vsrc = reinterpret_cast<const float*>(P.sc.views);
         for (int i = threadIdx.x; i < P.nv * 16; i += kThreads) vsm[i] = __ldg(vsrc + i);
-        fence_proxy_async();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    if (warp < 4) {   // trunk weights -> TMEM (thread = neuron = TMEM lane)
-        constexpr int NW = (2 * KE + 384) / 2;
-        const uint32_t tw = tmem + ((uint32_t)(warp * 32) << 16) + TM_W;
-        const int n = warp * 32 + lane;
-        for (int j0 = 0; j0 < NW; j0 += 16) {
-            uint32_t r[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) r[i] = __ldg(P.mlp.wimg + (size_t)(j0 + i) * 128 + n);
-            tmem_st16(tw + j0, r);
-        }
-        // trunk biases enter the accumulators through one extra K=16 MMA per block-layer (A = this tile, B = one-hot selector),
-        // which removes 32 FADDs per block-layer from the issue-bound epilogue warps
-        {
-            const float* bs = reinterpret_cast<const float*>(sgen + SM_BIAS);
-            uint32_t r[16];
-#pragma unroll
-            for (int i = 0; i < 16; ++i) r[i] = 0u;
-            r[0] = pack_h2(bs[n], bs[128 + n]);
-            r[1] = pack_h2(bs[256 + n], bs[384 + n]);
-            tmem_st16(tmem + ((uint32_t)(warp * 32) << 16) + TM_BIAS, r);
-        }
-        tc_wait_st();
-    } else if (warp >= kProducerWarp0) {
-        for (int e = threadIdx.x - kProducerWarp0 * 32; e < 256; e += kProducerWarps * 32) {   // selector tile: row n (point), logical k = 17 l  <->  k-step l, element l   is 1.0
-            const int row = e >> 3, chunk = e & 7;
-            uint4 z = make_uint4(0u, 0u, 0u, 0u);
-            if ((chunk & 1) == 0) {
-                const int l = chunk >> 1;                         // logical byte 34 l: chunk 2l, half-word l
-                const uint32_t one = 0x3C00u << (16 * (l & 1));
-                if ((l >> 1) == 0) z.x = one; else z.y = one;
-            }
-            *reinterpret_cast<uint4*>(sgen + SM_SEL + row * 128 + ((chunk ^ (row & 7)) << 4)) = z;
-        }
-        fence_proxy_async();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
+    if (!mbar_wait_bounded(bar, 0)) load_timeout(P.trap, bar);
 
+    const int wg = threadIdx.x >> 7, wt = threadIdx.x & 127, warp = wt >> 5, lane = threadIdx.x & 31, t = lane & 3;
+    PtsRow* pts = reinterpret_cast<PtsRow*>(sgen + SM::PTS) + wg * kTilePts;
+    const ViewXform* vxs = reinterpret_cast<const ViewXform*>(sgen + SM::VIEWS);
+    const float* sb = reinterpret_cast<const float*>(sgen + SM::BIAS);
+    const uint32_t sW = sbase, sH = sbase + SM::HEAD;
     const int nv = P.nv, N = P.N;
+    const int r0 = warp * 16 + (lane >> 2);          // this thread's accumulator rows (points) r0, r0 + 8
 
-    if (warp == kMiscWarp) {
-        // =====================================================================================
-        // POINT / DIRECTION WARP.  Per tile: the view-independent world points of its two 64-row halves (two dependent global
-        // round trips: ray order -> ray, far, t) and the view-mean direction encoding of the quirk-Q1 conditioning rays.
-        // =====================================================================================
-        PtsRow* pts = reinterpret_cast<PtsRow*>(sgen + SM_PTS);
-        const ViewXform* vxs = reinterpret_cast<const ViewXform*>(sgen + SM_VIEWS);
-        uint32_t tcount = 0;
-        for (int t = blockIdx.x; t < P.n_tiles; t += gridDim.x, ++tcount) {
-            const int g = t / P.sg, q = t % P.sg;
-            const uint32_t tpar = tcount & 1u;
-            for (int hh = 0; hh < 2; ++hh) {
-                mbar_wait<kProdSleep>(BAR(PTS_FREE + hh), tpar ^ 1u, P.trap, 6);       // the geometry warps are done with the previous tile's half
-                for (int th = lane; th < kHalfPts; th += 32) {
-                    const int n = hh * kHalfPts + th, rl = n & 31, sl = n >> 5;
-                    const int slot_r = min(g * kTileRays + rl, P.n_rays - 1);
-                    const int rid = P.ray_order ? P.ray_order[slot_r] : slot_r;
-                    const int sidx = min(q * kTileSamples + sl, N - 1);
-                    const float fr = P.far[rid];
-                    const float tv = P.tvals[(long long)rid * N + sidx];
-                    RayFast rg;
-                    ray_fast(P.rays_o + 3 * rid, P.rays_d + 3 * rid, fr, rg, IS_BG);
-                    PtsRow pr;
-                    pr.tv = tv;
-                    if (IS_BG) bg_point_fast(rg, tv, P.far_unc, pr.xe, pr.xl);
-                    else {
-                        for (int i = 0; i < 3; ++i) { pr.xe[i] = rg.o[i] + tv * rg.d[i]; pr.xl[i] = pr.xe[i]; }
-                    }
-                    pts[n] = pr;
-                }
-                mbar_arrive_warp(BAR(PTS_READY + hh), lane);
-            }
-            // ---- mean over views of the direction encoding of the quirk-Q1 conditioning ray (model.py:357-360) ----
-            mbar_wait<kProdSleep>(BAR(DIR_FREE), tpar ^ 1u, P.trap, 2);               // the previous tile's head MMA has read the DIR tile
-            for (int n = lane; n < 2 * kHalfPts; n += 32) {
-                const int rl = n & 31, sl = n >> 5;
-                const int slot_r = min(g * kTileRays + rl, P.n_rays - 1);
-                const int rid = P.ray_order ? P.ray_order[slot_r] : slot_r;
-                const int sidx = min(q * kTileSamples + sl, N - 1);
-                const int ch = P.chunk > 0 ? P.chunk : P.n_rays;
-                const int c0 = (rid / ch) * ch;
-                const int Bc = min(ch, P.n_rays - c0);
-                const long long jl = (long long)(rid - c0) * N + sidx;
-                const int src = c0 + ((jl < 0x7fffffffLL) ? (int)((unsigned)jl % (unsigned)Bc) : (int)(jl % Bc));
-                const float wd[3] = {P.viewdirs[3 * src], P.viewdirs[3 * src + 1], P.viewdirs[3 * src + 2]};
-                float acc[32];
+    for (int tile = blockIdx.x * kWarpgroups + wg; tile < P.n_tiles; tile += gridDim.x * kWarpgroups) {
+        const int g = tile / P.sg, q = tile % P.sg;
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");       // the previous tile's rows have been read
+        if (wt < kTilePts) {
+            const int n = wt, rl = n % kTileRays, sl = n / kTileRays;
+            const int slot = g * kTileRays + rl, s = q * kTileSamples + sl;
+            const int slot_c = min(slot, P.n_rays - 1), s_c = min(s, N - 1);
+            const int rid = P.ray_order ? P.ray_order[slot_c] : slot_c;
+            PtsRow pr;
+            pr.rid = rid; pr.sidx = s_c; pr.valid = (slot < P.n_rays) && (s < N);
+            pr.tv = P.tvals[(long long)rid * N + s_c];
+            RayFast rg;
+            ray_fast(P.rays_o + 3 * rid, P.rays_d + 3 * rid, P.far[rid], rg, IS_BG);
+            if (IS_BG) bg_point_fast(rg, pr.tv, P.far_unc, pr.xe, pr.xl);
+            else for (int i = 0; i < 3; ++i) { pr.xe[i] = rg.o[i] + pr.tv * rg.d[i]; pr.xl[i] = pr.xe[i]; }
+            // quirk Q1: the direction of ray (j mod B) of the ray's chunk, j = flat (ray, sample) index inside the chunk
+            const int ch = P.chunk > 0 ? P.chunk : P.n_rays;
+            const int c0 = (rid / ch) * ch;
+            const int Bc = min(ch, P.n_rays - c0);
+            const long long jl = (long long)(rid - c0) * N + s_c;
+            pr.src = c0 + (int)(jl % Bc);
+            pr.pad = 0;
+            pts[n] = pr;
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+
+        float hacc[40];                                 // folded head: [q (64) | sigma | pad], summed over the views
 #pragma unroll
-                for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+        for (int i = 0; i < 40; ++i) hacc[i] = 0.f;
+#pragma unroll 1
+        for (int v = 0; v < nv; ++v) {
+            float ce[2][4], cl[2][3];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const PtsRow& pr = pts[r0 + 8 * i];
+                to_camera(vxs[v], pr.xe, ce[i]);
+                if (IS_BG) to_camera(vxs[v], pr.xl, cl[i]);
+                else { cl[i][0] = ce[i][0]; cl[i][1] = ce[i][1]; cl[i][2] = ce[i][2]; }      // foreground: the lookup point IS the encoded point
+                ce[i][3] = pr.tv;
+            }
+            uint32_t enc[KS][4];
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        const int c = 16 * ks + 8 * h + 2 * t;
+                        enc[ks][2 * h + i] = pack_h2(enc_value<ICH>(ce[i], c), enc_value<ICH>(ce[i], c + 1));
+                    }
+            float acc[64];
+            uint32_t a[8][4];
+            // layer 0: blend of P0 + W0enc . enc (b0 on the constant-one column)
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+            blend_maps<0>(acc, P, cl, v, t);
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks) wgmma_rs_n128(acc, enc[ks], wdesc(sW + trunk_off(KE, 0), ks, SLAB));
+            wgmma_commit();
+            wgmma_wait<0>();
+            relu_to_frags<128>(acc, a);
+            // layers 1, 2
+#pragma unroll 1
+            for (int l = 1; l <= 2; ++l) {
+                seed_bias<128>(acc, sb + 128 * l, t);
+                wgmma_fence();
+#pragma unroll
+                for (int ks = 0; ks < 8; ++ks) wgmma_rs_n128(acc, a[ks], wdesc(sW + trunk_off(KE, l), ks, SLAB));
+                wgmma_commit();
+                wgmma_wait<0>();
+                relu_to_frags<128>(acc, a);
+            }
+            // layer 3: blend of P3 + W3h . h2 + W3enc . enc (b3 on the constant-one column)
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+            blend_maps<1>(acc, P, cl, v, t);
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < 8; ++ks) wgmma_rs_n128(acc, a[ks], wdesc(sW + trunk_off(KE, 3), ks, SLAB));
+#pragma unroll
+            for (int ks = 0; ks < KS; ++ks) wgmma_rs_n128(acc, enc[ks], wdesc(sW + trunk_off(KE, 4), ks, SLAB));
+            wgmma_commit();
+            wgmma_wait<0>();
+            relu_to_frags<128>(acc, a);
+            // folded head: hacc += h3 . Whead_h^T
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < 8; ++ks) wgmma_rs_n80(hacc, a[ks], wdesc(sH + WH_H, ks, 80 * 128));
+            wgmma_commit();
+            wgmma_wait<0>();
+        }
+        // direction term: hacc += mean_v(dir_enc_v) . Whead_dir^T   (K = 32: 27 columns + zero padding)
+        {
+            uint32_t dfr[2][4];
+            float dsum[2][8];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const int src = pts[r0 + 8 * i].src;
+                const float wd[3] = {P.viewdirs[3 * src], P.viewdirs[3 * src + 1], P.viewdirs[3 * src + 2]};
+#pragma unroll
+                for (int c = 0; c < 8; ++c) dsum[i][c] = 0.f;
                 for (int vv = 0; vv < nv; ++vv) {
                     float dc[3];
                     rotate_to_camera(vxs[vv], wd, dc);
 #pragma unroll
-                    for (int e = 0; e < kDirEnc; ++e) {
-                        float val;
-                        if (e < 3) val = dc[e];
-                        else {
-                            const int q0 = e - 3;
-                            const bool shifted = q0 >= 12;
-                            const int qq = shifted ? q0 - 12 : q0;
-                            const float xb = dc[qq % 3] * (float)(1 << (qq / 3));
-                            val = __sinf(shifted ? xb + 1.57079637f : xb);
-                        }
-                        acc[e] += val;
-                    }
+                    for (int c = 0; c < 8; ++c) dsum[i][c] += dir_value(dc, 16 * (c >> 2) + 8 * ((c >> 1) & 1) + 2 * t + (c & 1));
                 }
-                const float inv = 1.0f / (float)nv;
-#pragma unroll
-                for (int chunk = 0; chunk < 4; ++chunk)
-                    sts128(sbase + SM_DIR + n * 128 + ((chunk ^ (n & 7)) << 4),
-                           make_uint4(pack_h2(acc[8 * chunk] * inv, acc[8 * chunk + 1] * inv), pack_h2(acc[8 * chunk + 2] * inv, acc[8 * chunk + 3] * inv),
-                                      pack_h2(acc[8 * chunk + 4] * inv, acc[8 * chunk + 5] * inv), pack_h2(acc[8 * chunk + 6] * inv, acc[8 * chunk + 7] * inv)));
             }
-            fence_proxy_async();
-            mbar_arrive_warp(BAR(DIR_READY), lane);
-        }
-    } else if (warp >= kGeomWarp0 && warp < kGeomWarp0 + kGeomWarps) {
-        // =====================================================================================
-        // GEOMETRY WARPS.  Unit of work: half-job (tile, view, half) = 64 points of one view; thread = (row, map pair): camera
-        // transform, the 2x2 tap quads of two maps (-> ROWINFO) and two quarters of the row's positional encoding (-> ENC).
-        // =====================================================================================
-        const int gt = threadIdx.x - kGeomWarp0 * 32, row = gt & (kHalfPts - 1), pair = gt >> 6;      // pair is warp-uniform
-        const PtsRow* pts = reinterpret_cast<const PtsRow*>(sgen + SM_PTS);
-        const ViewXform* vxs = reinterpret_cast<const ViewXform*>(sgen + SM_VIEWS);
-        uint32_t kcount = 0, tcount = 0;
-        long long tp_encwait = 0, tp_geom = 0;
-        TSTART();
-        for (int t = blockIdx.x; t < P.n_tiles; t += gridDim.x, ++tcount) {
-            const int g = t / P.sg, q = t % P.sg;
-            for (int v = 0; v < nv; ++v) {
-                for (int h = 0; h < 2; ++h, ++kcount) {
-                    const uint32_t slot = kcount & 1, use = (kcount >> 1) & 1;
-                    const uint32_t encb = sbase + SM_ENC + slot * SLOT_ENC;
-                    const uint32_t rowinfo = sbase + SM_ROWINFO + slot * SLOT_INFO;
-                    if (v == 0) mbar_wait<kProdSleep>(BAR(PTS_READY + h), tcount & 1u, P.trap, 7);
-                    mbar_wait<kProdSleep>(BAR(ENC_FREE + slot), use ^ 1, P.trap, 1);
-                    mbar_wait<kProdSleep>(BAR(INFO_FREE + slot), use ^ 1, P.trap, 8);
-                    TLAP(tp_encwait);
-                    if (warp == kGeomWarp0 && lane == 0) TRACE(0, kcount, 0, 0);
-                    const PtsRow pr = pts[h * kHalfPts + row];
-                    const ViewXform vx = vxs[v];
-                    float ce[4], cl[3];
-                    to_camera(vx, pr.xe, ce);
-                    if (IS_BG) to_camera(vx, pr.xl, cl);
-                    else { cl[0] = ce[0]; cl[1] = ce[1]; cl[2] = ce[2]; }      // foreground: the lookup point IS the encoded point
-                    ce[3] = pr.tv;
-                    // a padding row of the tile (sample index past N / ray past the batch: its outputs are never stored) joins no window
-                    const bool pad = (q * kTileSamples + ((h * kHalfPts + row) >> 5) >= N) | (g * kTileRays + (row & 31) >= P.n_rays);
+            const float inv = 1.0f / (float)nv;
 #pragma unroll
-                    for (int j = 0; j < 2; ++j) {
-                        const int sub = pair * 2 + j;
-                        float gx, gy;
-                        int mw, mh;
-                        if (sub == 0) {
-                            local_grid_coords(P.sc, cl, gx, gy);
-                            mw = P.sc.lat_w; mh = P.sc.lat_h;
-                        } else {
-                            gx = (sub == 3) ? cl[1] : cl[0];
-                            gy = (sub == 2) ? cl[1] : cl[2];          // xz, xy, yz
-                            mw = P.sc.plane_w; mh = P.sc.plane_h;
-                        }
-                        // 2x2 tap quad of grid_sample(align_corners=True, zeros): base texel (x0, y0) in [-1, W-1] x [-1, H-1] and the four
-                        // weights (0 for an out-of-range tap); a row whose taps all fall outside is dead: it joins no window
-                        TapQuad tq;
-                        tap_quad(gx, gy, mw, mh, tq);
-                        const bool dead = ((tq.w[0] == 0.f) & (tq.w[1] == 0.f) & (tq.w[2] == 0.f) & (tq.w[3] == 0.f)) | pad;
-                        sts128(rowinfo + sub * 1024 + row * 16,
-                               make_uint4((uint32_t)tq.x0, dead ? kDeadRow : (uint32_t)tq.y0, pack_h2(tq.w[0], tq.w[1]), pack_h2(tq.w[2], tq.w[3])));
+            for (int ks = 0; ks < 2; ++ks)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        const int c = 4 * ks + 2 * h;
+                        dfr[ks][2 * h + i] = pack_h2(dsum[i][c] * inv, dsum[i][c + 1] * inv);
                     }
-                    if (pair == 0) { enc_cols<ICH, 0>(ce, encb, row, false); enc_cols<ICH, 1>(ce, encb, row, false); }
-                    else { enc_cols<ICH, 2>(ce, encb, row, false); enc_cols<ICH, 3>(ce, encb, row, false); }
-                    fence_proxy_async();                       // ENC is read by the tensor core (async proxy)
-                    __syncwarp();
-                    if (lane == 0) {
-                        mbar_arrive(BAR(ENC_READY + slot));
-                        mbar_arrive(BAR(INFO_READY + slot));
-                        if (v == nv - 1) mbar_arrive(BAR(PTS_FREE + h));
-                    }
-                    TLAP(tp_geom);
-                    if (warp == kGeomWarp0 && lane == 0) TRACE(0, kcount, 1, 0);
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < 2; ++ks) wgmma_rs_n80(hacc, dfr[ks], wdesc(sH + WH_DIR, ks, 80 * 128));
+            wgmma_commit();
+            wgmma_wait<0>();
+        }
+        // sigma (column 64: thread t = 0 of each quad), q = relu(hacc + bq) -> colour head 64 x 64 -> relu -> 64 x 3 -> sigmoid
+        const PtsRow pr0 = pts[r0], pr1 = pts[r0 + 8];
+        if (t == 0) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const PtsRow& pr = i ? pr1 : pr0;
+                const float xs = (hacc[32 + 2 * i] + sb[644]) - 1.0f;                   // model.py:392-393
+                if (pr.valid) P.sigma_out[(long long)pr.rid * N + pr.sidx] = xs > 20.f ? xs : log1pf(expf(xs));
+            }
+        }
+        uint32_t qa[4][4];
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int c = 16 * ks + 8 * (r >> 1) + 2 * t;                           // column of hacc[8 ks + 2 r]
+                qa[ks][r] = pack_h2(fmaxf(hacc[8 * ks + 2 * r] + sb[512 + c], 0.f), fmaxf(hacc[8 * ks + 2 * r + 1] + sb[512 + c + 1], 0.f));
+            }
+        float v1[32];
+        seed_bias<64>(v1, sb + 576, t);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) wgmma_rs_n64(v1, qa[ks], wdesc(sH + WH_V1, ks, 64 * 128));
+        wgmma_commit();
+        wgmma_wait<0>();
+        relu_to_frags<64>(v1, qa);
+        float o[8];
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int c = 8 * j + 2 * t + e;
+                    o[4 * j + 2 * i + e] = c < 3 ? sb[640 + c] : 0.f;
+                }
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) wgmma_rs_n16(o, qa[ks], wdesc(sH + WH_RGB, ks, 16 * 128));
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (t < 2) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                const PtsRow& pr = i ? pr1 : pr0;
+                if (!pr.valid) continue;
+                const long long gp = (long long)pr.rid * N + pr.sidx;
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int c = 2 * t + e;
+                    if (c < 3) P.rgb_out[gp * 3 + c] = (1.f / (1.f + expf(-o[2 * i + e]))) * 1.002f - 0.001f;   // model.py:395-397
                 }
             }
         }
-        if (DBG && P.dbg && gt == 0) {
-            long long* d = P.dbg + (size_t)blockIdx.x * kDbgStride;
-            d[1] = tp_encwait; d[2] = tp_geom;
-        }
-    } else if (warp >= kWinWarp0) {
-        // =====================================================================================
-        // WINDOW WARPS (warp w owns kMapsPerWin consecutive maps of latent, xz, xy, yz).  Each row's 2x2 quad lies inside exactly one 4x4 box
-        // of the lattice anchored at the job's minimum base texel with pitch 3, so the job's 64 rows fall into a handful of boxes;
-        // per distinct box one TMA load stages the 4x4x256-channel window and the lanes scatter their rows' four weights into its
-        // [64 points x 16 texels] tile (rows of other boxes: zeros).
-        // =====================================================================================
-        const int wi = warp - kWinWarp0;
-        uint32_t kcount = 0, wseq = 0;            // wseq: sequence number of the job's first texel window
-        long long tw_wait = 0, tw_enum = 0, tw_bar2 = 0, tw_turn = 0, tw_empty = 0, tw_body = 0, tw_n = 0;
-        TSTART();
-        volatile uint32_t* turn = reinterpret_cast<volatile uint32_t*>(sgen + SM_CNT + 36);
-        const int trole = (wi == 0) ? 1 : (wi == kWinWarps - 1) ? 2 : -1;
-        struct MapRows { uint4 ra, rb; int xm, ym, ka, kb, ca, cb, nwin; };
-        for (int t = blockIdx.x; t < P.n_tiles; t += gridDim.x) {
-            for (int v = 0; v < nv; ++v) {
-                for (int h = 0; h < 2; ++h, ++kcount) {
-                    const uint32_t slot = kcount & 1, use = (kcount >> 1) & 1;
-                    const uint32_t rowinfo = sbase + SM_ROWINFO + slot * SLOT_INFO;
-                    mbar_wait<kProdSleep>(BAR(INFO_READY + slot), use, P.trap, 9);
-                    TLAP(tw_wait);
-                    if (trole >= 0 && lane == 0) TRACE(trole, kcount, 0, 0);
-                    MapRows mr[kMapsPerWin];
-#pragma unroll
-                    for (int mm = 0; mm < kMapsPerWin; ++mm) {
-                        const int m = kMapsPerWin * wi + mm;
-                        mr[mm].ra = lds128(rowinfo + m * 1024 + lane * 16);
-                        mr[mm].rb = lds128(rowinfo + m * 1024 + (lane + 32) * 16);
-                    }
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(BAR(INFO_FREE + slot));              // the rows are in registers
-                    volatile uint32_t* cntw = reinterpret_cast<volatile uint32_t*>(sgen + SM_CNT + slot * 16);
-#pragma unroll
-                    for (int mm = 0; mm < kMapsPerWin; ++mm) {
-                        MapRows& r = mr[mm];
-#ifdef NEO_ABLATE_WINDOWS
-                        const bool la = false, lb = false;          // profiling experiment only: no lookups (wrong results)
-#else
-                        const bool la = r.ra.y != kDeadRow, lb = r.rb.y != kDeadRow;
-#endif
-                        const int xa = (int)r.ra.x, ya = (int)r.ra.y, xb = (int)r.rb.x, yb = (int)r.rb.y;
-                        r.xm = __reduce_min_sync(0xffffffffu, min(la ? xa : 0x7fffffff, lb ? xb : 0x7fffffff));
-                        r.ym = __reduce_min_sync(0xffffffffu, min(la ? ya : 0x7fffffff, lb ? yb : 0x7fffffff));
-                        r.ka = la ? ((((ya - r.ym) / 3) << 16) | ((xa - r.xm) / 3)) : -1;
-                        r.kb = lb ? ((((yb - r.ym) / 3) << 16) | ((xb - r.xm) / 3)) : -1;
-                        // number the distinct boxes (ca / cb = window index of this lane's rows)
-                        r.nwin = 0; r.ca = -1; r.cb = -1;
-                        bool pa = la, pb = lb;
-                        while (true) {
-                            const unsigned ba = __ballot_sync(0xffffffffu, pa), bb = __ballot_sync(0xffffffffu, pb);
-                            if (!(ba | bb)) break;
-                            const int key = ba ? __shfl_sync(0xffffffffu, r.ka, __ffs(ba) - 1) : __shfl_sync(0xffffffffu, r.kb, __ffs(bb) - 1);
-                            if (pa && r.ka == key) { r.ca = r.nwin; pa = false; }
-                            if (pb && r.kb == key) { r.cb = r.nwin; pb = false; }
-                            ++r.nwin;
-                        }
-                        if (lane == 0) cntw[kMapsPerWin * wi + mm] = (uint32_t)r.nwin;
-                    }
-                    // publish the counts BEFORE waiting for ring slots (a job may need more windows than the ring holds: the MMA warp
-                    // consumes them as they arrive).  Sequence numbers are handed out in map order (latent, xz, xy, yz) so that the
-                    // fp32 accumulation order of a point's windows -- and with it every output bit -- is the same on every run.
-                    TLAP(tw_enum);
-                    asm volatile("bar.sync 2, %0;" ::"r"(kWinWarps * 32) : "memory");
-                    const uint32_t c0 = cntw[0], c1 = cntw[1], c2 = cntw[2], c3 = cntw[3];
-                    const int m0 = kMapsPerWin * wi;
-                    const uint32_t seqbase = wseq + (m0 > 0 ? c0 : 0u) + (m0 > 1 ? c1 : 0u) + (m0 > 2 ? c2 : 0u);
-                    wseq += c0 + c1 + c2 + c3;
-                    if (lane == 0) mbar_arrive(BAR(CNT_READY + slot));
-                    TLAP(tw_bar2);
-                    if (DBG) tw_n += mr[0].nwin;
-                    if (trole >= 0 && lane == 0) { TRACE(trole, kcount, 1, c0); if (DBG && P.dbg && blockIdx.x == 0 && kcount < (uint32_t)kTraceJobs) P.dbg[(size_t)gridDim.x * kDbgStride + trole * 1024 + kcount * 8 + 7] = mr[0].nwin; }
-                    uint32_t seq0 = seqbase;
-#pragma unroll
-                    for (int mm = 0; mm < kMapsPerWin; ++mm) {
-                        const MapRows& r = mr[mm];
-                        const int nwin = r.nwin;
-                        if (mm > 0) seq0 += (uint32_t)mr[mm - 1].nwin;
-                        const CUtensorMap* tm = &P.mlp.tmap[kMapsPerWin * wi + mm];
-                        // Ring slots must be acquired in sequence order: a parity wait is only unambiguous while the waiter is at most
-                        // one phase ahead of the barrier, so window s may wait for its slot only after window s - kRing holds it.  The
-                        // window warps therefore take turns for the acquisition (a few instructions per window); the rest runs in parallel.
-                        if (nwin > 0) {
-                            if (lane == 0) {
-                                uint32_t spins = 0;
-                                while (*turn != seq0) {
-                                    if (++spins > 0x2000000u) mbar_timeout(P.trap, 4, (uint32_t)seq0, *turn);
-                                }
-                            }
-                            __syncwarp();
-                        }
-                        TLAP(tw_turn);
-                        // Everything that does not need the ring is done BEFORE the slots are requested (the warp is usually blocked there):
-                        // each row's 16 window-slot weights as four 64-bit words (one per window row: the quad's top pair sits in window
-                        // row by at columns bx, bx+1, the bottom pair in row by+1), relative to the origin of the row's own box.
-                        unsigned long long wa[4], wb[4];
-                        {
-                            const int oxa = r.xm + 3 * (r.ka & 0xffff), oya = r.ym + 3 * (r.ka >> 16);
-                            const int oxb = r.xm + 3 * (r.kb & 0xffff), oyb = r.ym + 3 * (r.kb >> 16);
-                            const bool va = r.ca >= 0, vb = r.cb >= 0;
-                            const int bxa = va ? (int)r.ra.x - oxa : 0, bya = va ? (int)r.ra.y - oya : 0;
-                            const int bxb = vb ? (int)r.rb.x - oxb : 0, byb = vb ? (int)r.rb.y - oyb : 0;
-                            const unsigned long long ta = ((unsigned long long)r.ra.z) << (16 * bxa), ba_ = ((unsigned long long)r.ra.w) << (16 * bxa);
-                            const unsigned long long tb = ((unsigned long long)r.rb.z) << (16 * bxb), bb_ = ((unsigned long long)r.rb.w) << (16 * bxb);
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                wa[j] = !va ? 0ull : (j == bya) ? ta : (j == bya + 1) ? ba_ : 0ull;
-                                wb[j] = !vb ? 0ull : (j == byb) ? tb : (j == byb + 1) ? bb_ : 0ull;
-                            }
-                        }
-                        // Batches of at most kRing / 2 windows: (1) lane k acquires the ring slot of window k and starts its TMA load (the
-                        // turn passes on as soon as this map's last slot is held), (2) every lane stores its two rows into the batch's
-                        // tiles (zeros where the row belongs to another box), (3) ONE proxy fence, (4) lane k signals window k.
-                        for (int done = 0; done < nwin;) {
-                            const int nb = min(nwin - done, kRing / 2);
-                            int my_ox = 0, my_oy = 0;                       // lane k: origin of window done + k
-                            for (int k = 0; k < nb; ++k) {
-                                const int i = done + k;
-                                const unsigned qa = __ballot_sync(0xffffffffu, r.ca == i), qb = __ballot_sync(0xffffffffu, r.cb == i);
-                                const int key = qa ? __shfl_sync(0xffffffffu, r.ka, __ffs(qa) - 1) : __shfl_sync(0xffffffffu, r.kb, __ffs(qb) - 1);
-                                if (lane == k) { my_ox = r.xm + 3 * (key & 0xffff); my_oy = r.ym + 3 * (key >> 16); }
-                            }
-                            if (lane < nb) {
-                                const uint32_t seq = seq0 + (uint32_t)(done + lane), rs = seq % kRing, rpar = (seq / kRing) & 1u;
-                                mbar_wait<kProdSleep>(BAR(WIN_EMPTY + rs), rpar ^ 1u, P.trap, 3);
-                                mbar_expect_tx(BAR(WIN_FULL + rs), WIN_BYTES);
-                                tma_load_window(sbase + SM_WIN + rs * WIN_BYTES, tm, my_ox, my_oy, v * 4, BAR(WIN_FULL + rs));
-                            }
-                            __syncwarp();
-                            if (lane == 0 && done + nb == nwin) *turn = seq0 + (uint32_t)nwin;
-                            TLAP(tw_empty);
-                            const uint32_t rowoff_a = (uint32_t)(lane >> 3) * 256u + (uint32_t)(lane & 7) * 16u, rowoff_b = rowoff_a + 1024u;
-                            for (int k = 0; k < nb; ++k) {
-                                const int i = done + k;
-                                const uint32_t wt = sbase + SM_WT + ((seq0 + (uint32_t)i) % kRing) * WT_BYTES;
-                                const bool ma = r.ca == i, mb = r.cb == i;
-                                sts128(wt + rowoff_a, ma ? make_uint4((uint32_t)wa[0], (uint32_t)(wa[0] >> 32), (uint32_t)wa[1], (uint32_t)(wa[1] >> 32)) : make_uint4(0u, 0u, 0u, 0u));
-                                sts128(wt + rowoff_a + 128u, ma ? make_uint4((uint32_t)wa[2], (uint32_t)(wa[2] >> 32), (uint32_t)wa[3], (uint32_t)(wa[3] >> 32)) : make_uint4(0u, 0u, 0u, 0u));
-                                sts128(wt + rowoff_b, mb ? make_uint4((uint32_t)wb[0], (uint32_t)(wb[0] >> 32), (uint32_t)wb[1], (uint32_t)(wb[1] >> 32)) : make_uint4(0u, 0u, 0u, 0u));
-                                sts128(wt + rowoff_b + 128u, mb ? make_uint4((uint32_t)wb[2], (uint32_t)(wb[2] >> 32), (uint32_t)wb[3], (uint32_t)(wb[3] >> 32)) : make_uint4(0u, 0u, 0u, 0u));
-                            }
-                            fence_proxy_async();                   // the tensor core (async proxy) reads the weight tiles
-                            __syncwarp();
-                            if (lane < nb) mbar_arrive(BAR(WIN_FULL + (seq0 + (uint32_t)(done + lane)) % kRing));
-                            TLAP(tw_body);
-                            done += nb;
-                        }
-                    }
-                    if (trole >= 0 && lane == 0) TRACE(trole, kcount, 3, 0);
-                }
-            }
-        }
-        if (DBG && P.dbg && wi == 0 && lane == 0) {
-            long long* d = P.dbg + (size_t)blockIdx.x * kDbgStride;
-            d[0] = tw_wait; d[24] = tw_enum; d[25] = tw_bar2; d[26] = tw_turn; d[27] = tw_empty; d[28] = tw_body; d[29] = tw_n;
-        }
-    } else if (warp == kMmaWarp) {
-        // =====================================================================================
-        // MMA ISSUE (one thread)
-        // =====================================================================================
-        {
-            // all 32 lanes run this loop (waits included); MMAs/commits are issued by one elected lane
-            uint32_t ph_h = 0, kcount = 0;      // bit b = parity of H_READY[b]
-            uint32_t whead = 0;                 // sequence number of the next texel window to consume (the producers' ring tail runs ahead)
-            long long tm_encwait = 0, tm_hwait = 0, tm_issue = 0, tm_gwait = 0;
-            TSTART();
-            // ENC (K-major, written by row owners) and H (MN-major = point-contiguous, written by neuron owners as 16-byte vectors)
-            const uint32_t id_blk = idesc_f16(128, 32), id_blk_mn = idesc_f16(128, 32, 0, 1), id_head = idesc_f16(128, 80, 1, 0),
-                           id_q = idesc_f16(128, 64), id_rgb = idesc_f16(128, 16), id_half = idesc_f16(128, 64), id_win = idesc_f16(128, 64, 1, 0);
-            const uint32_t dD = tmem + TM_D, dD3 = tmem + TM_D3, dH = tmem + TM_DH;
-            const uint32_t aW0 = tmem + TM_W, aW1 = aW0 + KE / 2, aW2 = aW1 + 64, aW3h = aW2 + 64, aW3e = aW3h + 64;
-            const uint32_t sH = sbase + SM_H, sDIR = sbase + SM_DIR, sWH = sbase + SM_WHEAD;
-            const uint32_t aB = tmem + TM_BIAS;
-            const uint64_t dSEL = desc_sw128(sbase + SM_SEL);          // + 2 l: k-step l = one-hot of layer l
-            auto kaddr = [](uint32_t base, int ks, uint32_t slab_bytes) { return base + (uint32_t)(ks >> 2) * slab_bytes + (uint32_t)(ks & 3) * 32u; };
-            // descriptor of k-step ks = base descriptor + ((ks>>2)*slab + (ks&3)*32) / 16 in the start-address field
-            auto dk = [](uint64_t base, int ks, uint32_t slab_bytes) { return base + (uint64_t)(((uint32_t)(ks >> 2) * slab_bytes + (uint32_t)(ks & 3) * 32u) >> 4); };
-            auto wait_h = [&](int blk, int tag) {
-                TLAP(tm_issue);
-                mbar_wait(BAR(H_READY + blk), (ph_h >> blk) & 1u, P.trap, tag); ph_h ^= 1u << blk;
-                TLAP(tm_hwait);
-                tc_fence_after();
-            };
-            // Colour head of a tile: q -> relu -> 64x64 -> relu -> 64x3.  It is software-pipelined INTO the first job of the CTA's next
-            // tile (stage 0 after layer 1's MMAs, stage 1 after layer 2's), so the tensor pipe and the producers never idle behind
-            // its three dependent round trips; operands live in the h=1 half of the H tile, accumulators in the head accumulator.
-            uint32_t ph_q = 0, ph_done = 0;
-            bool pend = false;
-            const uint32_t sQ = sH + 16384;
-            auto wait_bar = [&](int b, uint32_t& ph, int tag) {
-                TLAP(tm_issue);
-                mbar_wait(BAR(b), ph, P.trap, tag); ph ^= 1;
-                TLAP(tm_hwait);
-                tc_fence_after();
-            };
-            auto color_stage = [&](int stage) {
-                wait_bar(Q_READY, ph_q, 14 + stage);
-                if (elect_one()) {
-                    if (stage == 0) {
-#pragma unroll
-                        for (int ks = 0; ks < 4; ++ks) mma_ss(dH, desc_sw128(sQ + ks * 32), desc_sw128(sWH + WH_V1 + ks * 32), id_q, ks > 0);
-                    } else {
-#pragma unroll
-                        for (int ks = 0; ks < 4; ++ks) mma_ss(dH + 64, desc_sw128(sQ + ks * 32), desc_sw128(sWH + WH_RGB + ks * 32), id_rgb, ks > 0);
-                    }
-                    tc_commit(BAR(CH_READY));
-                }
-                __syncwarp();
-            };
-            uint32_t tcount = 0;
-            for (int t = blockIdx.x; t < P.n_tiles; t += gridDim.x, ++tcount) {
-                for (int v = 0; v < nv; ++v) {
-                    for (int h = 0; h < 2; ++h, ++kcount) {
-                        const uint32_t slot = kcount & 1, use = (kcount >> 1) & 1;
-                        const uint32_t sENC = sbase + SM_ENC + slot * SLOT_ENC;
-                        const uint32_t sHh = sH + h * 16384;                    // MN-major tile of this half (64 points x 128 K)
-                        uint64_t dENC[2], dHb[2];
-                        for (int bb = 0; bb < 2; ++bb) { dENC[bb] = desc_sw128(sENC + bb * 4096); dHb[bb] = desc_mn_sw128(sHh + bb * 64, 16384, 1024); }
-                        TLAP(tm_issue);
-                        mbar_wait(BAR(ENC_READY + slot), use, P.trap, 10);
-                        TLAP(tm_encwait);
-                        if (lane == 0) TRACE(3, kcount, 0, 0);
-                        tc_fence_after();
-                        // Layer 0 of the whole 64-point half (N = 64): D = W0enc . ENC^T (b0 rides on the constant-one input column).
-                        if (elect_one()) {
-#pragma unroll
-                            for (int ks = 0; ks < KE / 16; ++ks) mma_ts(dD, aW0 + ks * 8, dk(dENC[0], ks, SLAB_ENC), id_half, ks > 0);
-                        }
-                        __syncwarp();
-                        TLAP(tm_issue);
-                        mbar_wait(BAR(CNT_READY + slot), use, P.trap, 12);
-                        const volatile uint32_t* cnt = reinterpret_cast<const volatile uint32_t*>(sgen + SM_CNT + slot * 16);
-                        const uint32_t nwin = cnt[0] + cnt[1] + cnt[2] + cnt[3];
-                        if (lane == 0) { TRACE(3, kcount, 1, nwin); if (DBG && P.dbg && blockIdx.x == 0 && kcount < (uint32_t)kTraceJobs) P.dbg[(size_t)gridDim.x * kDbgStride + 3 * 1024 + kcount * 8 + 7] = nwin; }
-                        // Bilinear lookups on the tensor pipe: per staged window, D[channel][point] += WINDOW[texel][channel]^T . TAPW[point][texel]^T
-                        // (A = the TMA-written window, MN-major: 2 channel groups of 64, 16 texels; B = the sparse tap-weight tile), and the
-                        // same for the layer-3 skip accumulator D3 from channel groups 2, 3 (model.py:142-146), which is seeded NOW together with
-                        // W3enc . ENC^T + b3 so that the ENC slot and the windows go back to the producers after layer 0, not after layer 3.
-                        auto win_a = [&](uint32_t rs, int half3) { return desc_mn_sw128(sbase + SM_WIN + rs * WIN_BYTES + half3 * 4096, 2048, 1024); };
-                        auto win_b = [&](uint32_t rs) { return desc_nosw(sbase + SM_WT + rs * WT_BYTES, 128, 256); };
-                        if (nwin <= (uint32_t)kRing) {
-                            if ((uint32_t)lane < nwin) {                     // lane i waits for window i: the waits overlap
-                                const uint32_t seq = whead + (uint32_t)lane;
-                                mbar_wait(BAR(WIN_FULL + seq % kRing), (seq / kRing) & 1u, P.trap, 13);
-                            }
-                            __syncwarp();
-                            tc_fence_after();
-                            TLAP(tm_gwait);
-                            if (elect_one()) {
-                                for (uint32_t i = 0; i < nwin; ++i) {
-                                    const uint32_t rs = (whead + i) % kRing;
-                                    mma_ss(dD, win_a(rs, 0), win_b(rs), id_win, 1);
-                                }
-                                tc_commit(BAR(ACC_READY));
-                                tc_commit(BAR(ACC_READY + 1));
-#pragma unroll
-                                for (int ks = 0; ks < KE / 16; ++ks) mma_ts(dD3, aW3e + ks * 8, dk(dENC[0], ks, SLAB_ENC), id_half, ks > 0);
-                                tc_commit(BAR(ENC_FREE + slot));
-                                for (uint32_t i = 0; i < nwin; ++i) {
-                                    const uint32_t rs = (whead + i) % kRing;
-                                    mma_ss(dD3, win_a(rs, 1), win_b(rs), id_win, 1);
-                                    tc_commit(BAR(WIN_EMPTY + rs));
-                                }
-                            }
-                            __syncwarp();
-                        } else {
-                            // more windows than the ring holds (points spread over the source image): consume and release them one by one
-                            if (elect_one()) {
-#pragma unroll
-                                for (int ks = 0; ks < KE / 16; ++ks) mma_ts(dD3, aW3e + ks * 8, dk(dENC[0], ks, SLAB_ENC), id_half, ks > 0);
-                                tc_commit(BAR(ENC_FREE + slot));
-                            }
-                            __syncwarp();
-                            for (uint32_t i = 0; i < nwin; ++i) {
-                                const uint32_t seq = whead + i, rs = seq % kRing;
-                                mbar_wait(BAR(WIN_FULL + rs), (seq / kRing) & 1u, P.trap, 13);
-                                tc_fence_after();
-                                if (elect_one()) {
-                                    mma_ss(dD, win_a(rs, 0), win_b(rs), id_win, 1);
-                                    mma_ss(dD3, win_a(rs, 1), win_b(rs), id_win, 1);
-                                    tc_commit(BAR(WIN_EMPTY + rs));
-                                }
-                                __syncwarp();
-                            }
-                            TLAP(tm_gwait);
-                            if (elect_one()) {
-                                tc_commit(BAR(ACC_READY));
-                                tc_commit(BAR(ACC_READY + 1));
-                            }
-                            __syncwarp();
-                        }
-                        whead += nwin;
-                        if (lane == 0) TRACE(3, kcount, 2, 0);
-#if NEO_TRUNK_N64
-                        // one N = 64 MMA per k-step covers both 32-point blocks (a tcgen05.mma costs the issuing warp ~40 cycles whatever its
-                        // size): half the instructions per layer; the two epilogue sets still convert their halves concurrently
-                        const uint32_t id_half_mn = idesc_f16(128, 64, 0, 1);
-                        for (int l = 1; l <= 3; ++l) {
-                            const uint32_t aW = (l == 1) ? aW1 : (l == 2 ? aW2 : aW3h);
-                            wait_h(0, 11);                          // layer l-1 of both blocks is in H
-                            wait_h(1, 11);
-                            if (elect_one()) {
-#pragma unroll
-                                for (int ks = 0; ks < 8; ++ks)
-                                    mma_ts((l == 3 ? dD3 : dD), aW + ks * 8, dHb[0] + (uint64_t)(ks * (2048 >> 4)), id_half_mn, (l == 3) || ks > 0);
-                                if (l < 3) {
-                                    mma_ts(dD, aB, dSEL + (uint64_t)(2 * l), id_blk, 1);          // + b_l  (b0, b3: ENC constant column)
-                                    mma_ts(dD + 32, aB, dSEL + (uint64_t)(2 * l), id_blk, 1);
-                                }
-                                tc_commit(BAR(ACC_READY));
-                                tc_commit(BAR(ACC_READY + 1));
-                            }
-                            __syncwarp();
-                            if (pend && v == 0 && h == 0 && l < 3) color_stage(l - 1);
-                        }
-#else
-                        for (int l = 1; l <= 3; ++l) {
-                            const uint32_t aW = (l == 1) ? aW1 : (l == 2 ? aW2 : aW3h);
-                            for (int bb = 0; bb < 2; ++bb) {
-                                wait_h(bb, 11);                     // layer l-1 of this block is in H
-                                if (elect_one()) {
-#pragma unroll
-                                    for (int ks = 0; ks < 8; ++ks)
-                                        mma_ts((l == 3 ? dD3 : dD) + 32 * bb, aW + ks * 8, dHb[bb] + (uint64_t)(ks * (2048 >> 4)), id_blk_mn, (l == 3) || ks > 0);
-                                    if (l < 3) mma_ts(dD + 32 * bb, aB, dSEL + (uint64_t)(2 * l), id_blk, 1);     // + b_l  (b0, b3: ENC constant column)
-                                    tc_commit(BAR(ACC_READY + bb));
-                                }
-                                __syncwarp();
-                            }
-                            if (pend && v == 0 && h == 0 && l < 3) color_stage(l - 1);
-                        }
-#endif
-                        if (lane == 0) TRACE(3, kcount, 3, 0);
-                        wait_h(0, 13);                              // h3 of both blocks written
-                        wait_h(1, 13);
-                        if (lane == 0) TRACE(3, kcount, 4, 0);
-                    }
-                    // the previous tile's colour head (drained during this tile's first job) has left the head accumulator
-                    if (v == 0 && pend) { wait_bar(HEAD_DONE, ph_done, 17); pend = false; }
-                    // head: Dh (+)= H3 . (Whead_h)^T      (128 points on lanes, accumulates the view mean)
-                    if (v == nv - 1) { mbar_wait(BAR(DIR_READY), tcount & 1u, P.trap, 19); tc_fence_after(); }     // the tile's direction encodings are staged
-                    if (elect_one()) {
-#pragma unroll
-                        for (int ks = 0; ks < 8; ++ks)
-                            mma_ss(dH, desc_mn_sw128(sH + ks * 2048, 16384, 1024), desc_sw128(kaddr(sWH + WH_H, ks, 10240)), id_head, (v > 0 || ks > 0));
-                        if (v == nv - 1) {
-#pragma unroll
-                            for (int ks = 0; ks < 2; ++ks)
-                                mma_ss(dH, desc_sw128(sDIR + ks * 32), desc_sw128(sWH + WH_DIR + ks * 32), idesc_f16(128, 80), 1);
-                            tc_commit(BAR(HEAD_READY));
-                            tc_commit(BAR(DIR_FREE));
-                        }
-                    }
-                    __syncwarp();
-                }
-                pend = true;        // colour head of this tile: interleaved with the first job of the next tile (or drained below)
-            }
-            if (pend) { color_stage(0); color_stage(1); wait_bar(HEAD_DONE, ph_done, 18); }
-            if (DBG && P.dbg && lane == 0) {
-                long long* d = P.dbg + (size_t)blockIdx.x * kDbgStride;
-                d[6] = tm_encwait; d[7] = tm_hwait; d[8] = tm_issue; d[13] = tm_gwait;
-            }
-        }
-    } else {
-        // =====================================================================================
-        // EPILOGUE (2 sets of 4 warps; a warp reads the TMEM lane quarter warp % 4).  Set A (warps 0-3) serves the 32-point block 0
-        // of every half-job and the colour head, set B (warps 4-7) block 1: the two blocks' epilogues run concurrently, so the
-        // tensor pipe works on one block's next layer while the other block is being converted.
-        // Trunk: thread = neuron (TMEM lane).  Head: thread = point.
-        // =====================================================================================
-        const int eset = warp >> 2, wq = warp & 3;
-        const int c = wq * 32 + lane;                   // neuron (trunk) / point row (head)
-        const uint32_t lane_base = tmem + ((uint32_t)(wq * 32) << 16);
-        uint32_t ph_acc = 0, ph_head = 0;     // parity of ACC_READY[eset]
-        long long te_accwait = 0, te_gwait = 0, te_work = 0, te_head = 0;
-        long long te_g_j[8] = {0, 0, 0, 0, 0, 0, 0, 0}, te_acc_l[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-        TSTART();
-        const uint32_t hbase = (uint32_t)(c >> 3) * 1024u + (uint32_t)(c & 7) * 128u;     // MN-major H: atom of 8 K rows, row c&7
-        const uint32_t sH = sbase + SM_H, sBias = sbase + SM_BIAS;
-        // ---- head epilogue of tile (g_, q_): thread = point row c.  Three stages, each behind one colour-head MMA; they are
-        //      interleaved with the trunk epilogues of the next tile's first job (after layers 0, 1, 2), or run back to back for
-        //      the CTA's last tile.  Tiles of the colour head live in the h=1 half of H, accumulators in the head accumulator. ----
-        bool pend = false;
-        int pg = 0, pq = 0;
-        uint32_t ph_ch = 0;
-        const uint32_t sQ = sH + 16384;
-        auto head_stage = [&](int stage, int g_, int q_) {
-            TLAP(te_work);
-            const int rl = c & 31, sl = c >> 5;
-            const int slot_r = g_ * kTileRays + rl, s = q_ * kTileSamples + sl;
-            const bool valid = slot_r < P.n_rays && s < N;
-            const int rid = P.ray_order ? P.ray_order[min(slot_r, P.n_rays - 1)] : min(slot_r, P.n_rays - 1);
-            const long long gp = (long long)rid * N + min(s, N - 1);
-            if (stage == 0) {
-                mbar_wait(BAR(HEAD_READY), ph_head, P.trap, 26); ph_head ^= 1;
-                tc_fence_after();
-                {
-                    uint32_t rs[8];
-                    tmem_ld8(lane_base + TM_DH + 64, rs);
-                    tc_wait_ld();
-                    const float raw = __uint_as_float(rs[0]) + lds_f32(sBias + 4 * 644);
-                    const float xs = raw - 1.0f;                                       // model.py:392-393
-                    if (valid) P.sigma_out[gp] = xs > 20.f ? xs : log1pf(expf(xs));
-                }
-                // 16 accumulator columns at a time: the colour head is off the critical path, registers are not
-#pragma unroll 1
-                for (int j = 0; j < 4; ++j) {
-                    uint32_t r[16];
-                    tmem_ld16(lane_base + TM_DH + 16 * j, r);
-                    tc_wait_ld();
-#pragma unroll
-                    for (int c2 = 0; c2 < 2; ++c2) {
-                        const int ch = 2 * j + c2;
-                        float y[8];
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) y[i] = fmaxf(__uint_as_float(r[c2 * 8 + i]) + lds_f32(sBias + 4 * (512 + ch * 8 + i)), 0.f);
-                        sts128(sQ + c * 128 + ((ch ^ (c & 7)) << 4),
-                               make_uint4(pack_h2(y[0], y[1]), pack_h2(y[2], y[3]), pack_h2(y[4], y[5]), pack_h2(y[6], y[7])));
-                    }
-                }
-                tc_fence_before(); fence_proxy_async(); mbar_arrive_warp(BAR(Q_READY), lane);
-            } else if (stage == 1) {
-                mbar_wait(BAR(CH_READY), ph_ch, P.trap, 27); ph_ch ^= 1;
-                tc_fence_after();
-#pragma unroll 1
-                for (int j = 0; j < 4; ++j) {
-                    uint32_t r[16];
-                    tmem_ld16(lane_base + TM_DH + 16 * j, r);
-                    tc_wait_ld();
-#pragma unroll
-                    for (int c2 = 0; c2 < 2; ++c2) {
-                        const int ch = 2 * j + c2;
-                        float y[8];
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) y[i] = fmaxf(__uint_as_float(r[c2 * 8 + i]) + lds_f32(sBias + 4 * (576 + ch * 8 + i)), 0.f);
-                        sts128(sQ + c * 128 + ((ch ^ (c & 7)) << 4),
-                               make_uint4(pack_h2(y[0], y[1]), pack_h2(y[2], y[3]), pack_h2(y[4], y[5]), pack_h2(y[6], y[7])));
-                    }
-                }
-                tc_fence_before(); fence_proxy_async(); mbar_arrive_warp(BAR(Q_READY), lane);
-            } else {
-                mbar_wait(BAR(CH_READY), ph_ch, P.trap, 28); ph_ch ^= 1;
-                tc_fence_after();
-                uint32_t r[16];
-                tmem_ld16(lane_base + TM_DH + 64, r);
-                tc_wait_ld();
-                if (valid) {
-#pragma unroll
-                    for (int k = 0; k < 3; ++k) {
-                        const float a = __uint_as_float(r[k]) + lds_f32(sBias + 4 * (640 + k));
-                        P.rgb_out[gp * 3 + k] = (1.f / (1.f + expf(-a))) * 1.002f - 0.001f;   // model.py:395-397
-                    }
-                }
-                tc_fence_before(); mbar_arrive_warp(BAR(HEAD_DONE), lane);
-                pend = false;
-            }
-            TLAP(te_head);
-        };
-        for (int t = blockIdx.x; t < P.n_tiles; t += gridDim.x) {
-            const int g = t / P.sg, q = t % P.sg;
-            for (int v = 0; v < nv; ++v) {
-                for (int h = 0; h < 2; ++h) {
-                    const uint32_t sHh = sH + h * 16384;
-#pragma unroll 1
-                    for (int l = 0; l < 4; ++l) {
-                        // biases arrive through the bias MMA and the gathered features through the transpose-accumulate MMA, so every
-                        // layer is: TMEM load -> fp16 pack -> packed ReLU -> 4 x 16-byte stores of this neuron's K row
-                        const __half2 zero2 = __floats2half2_rn(0.f, 0.f);
-                        {
-                            const int bb = eset;
-                            unsigned char* hp = sgen + (sHh - sbase) + hbase;
-                            uint32_t r[32];
-                            TLAP(te_work);
-                            mbar_wait(BAR(ACC_READY + bb), ph_acc, P.trap, 20 + l); ph_acc ^= 1u;
-                            if (DBG) { long long t1 = clock64(); te_acc_l[l * 2 + bb] += t1 - _t0; }
-                            TLAP(te_accwait);
-                            tc_fence_after();
-                            tmem_ld32(lane_base + (l == 3 ? TM_D3 : TM_D) + bb * 32, r);
-                            tc_wait_ld();
-#pragma unroll
-                            for (int j4 = 0; j4 < 4; ++j4) {          // 8 consecutive points = one 16-byte vector of this neuron's K row
-                                uint32_t w[4];
-#pragma unroll
-                                for (int i = 0; i < 4; ++i) {
-                                    const uint32_t pk = pack_h2(__uint_as_float(r[8 * j4 + 2 * i]), __uint_as_float(r[8 * j4 + 2 * i + 1]));
-                                    const __half2 hv = __hmax2(*reinterpret_cast<const __half2*>(&pk), zero2);
-                                    w[i] = *reinterpret_cast<const uint32_t*>(&hv);
-                                }
-                                *reinterpret_cast<uint4*>(hp + ((((bb << 2) + j4) ^ (c & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
-                            }
-                            tc_fence_before();
-                            fence_proxy_async();
-                            mbar_arrive_warp(BAR(H_READY + bb), lane);
-                        }
-                        if (eset == 0 && pend && v == 0 && h == 0 && l < 3) head_stage(l, pg, pq);
-                    }
-                }
-            }
-            pend = true; pg = g; pq = q;       // colour head of this tile: interleaved with the next tile's first job (or drained below)
-        }
-        if (eset == 0 && pend) { head_stage(0, pg, pq); head_stage(1, pg, pq); head_stage(2, pg, pq); }
-        if (DBG && P.dbg && threadIdx.x == 0) {
-            long long* d = P.dbg + (size_t)blockIdx.x * kDbgStride;
-            d[9] = te_accwait; d[10] = te_gwait; d[11] = te_work; d[12] = te_head;
-            for (int i = 0; i < 8; ++i) { d[16 + i] = te_g_j[i]; d[40 + i] = te_acc_l[i]; }
-        }
     }
-    // ---- teardown ----
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kMmaWarp) tmem_dealloc(tmem, 512);
-}
-
-// ------------------------------------------------------------------------------------------------
-// self-test of the tensor-core primitives used above (TS-mode MMA with A in TMEM, SW128 operand tiles, SS-mode MMA)
-//   out1[neuron][point] = sum_k W[neuron][k] * X[point][k]   (K = 128, TS mode)
-//   out2[point][n]      = sum_k X[point][k] * Wn[n][k]       (N = 80,  SS mode)
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(128, 1) selftest_kernel(const float* __restrict__ X, const float* __restrict__ W,
-                                                          const float* __restrict__ Wn, float* __restrict__ out1,
-                                                          float* __restrict__ out2, float* __restrict__ out3,
-                                                          float* __restrict__ out4, int* err) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    unsigned char* sgen = smem_raw + (sbase - smem_u32(smem_raw));
-    const uint32_t sX = sbase, sWn = sbase + 32768, sXmn = sbase + 53248, bar = sbase + 86016;
-    volatile uint32_t* slot = reinterpret_cast<volatile uint32_t*>(sgen + 86016 + 16);
-    const int warp = threadIdx.x >> 5, c = threadIdx.x;
-    if (threadIdx.x == 0) { mbar_init(bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-    if (warp == 0) tmem_alloc(sbase + 86016 + 16, 512);
-    __half* xs = reinterpret_cast<__half*>(sgen);
-    __half* ws = reinterpret_cast<__half*>(sgen + 32768);
-    __half* xm = reinterpret_cast<__half*>(sgen + 53248);       // X again, MN-major: two 64-point tiles of 16 KB
-    for (int e = threadIdx.x; e < 128 * 128; e += 128) xs[sw128_off(e / 128, e % 128, 128) / 2] = __float2half_rn(X[e]);
-    for (int e = threadIdx.x; e < 128 * 128; e += 128) {
-        const int n = e / 128, k = e % 128;
-        xm[((n >> 6) * 16384 + mn128_off(n, k)) / 2] = __float2half_rn(X[e]);
-    }
-    for (int e = threadIdx.x; e < 80 * 128; e += 128) ws[sw128_off(e / 128, e % 128, 80) / 2] = __float2half_rn(Wn[e]);
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *slot;
-    const uint32_t lane_base = tmem + ((uint32_t)(warp * 32) << 16);
-    for (int j0 = 0; j0 < 64; j0 += 16) {
-        uint32_t r[16];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) r[i] = pack_h2(W[c * 128 + 2 * (j0 + i)], W[c * 128 + 2 * (j0 + i) + 1]);
-        tmem_st16(lane_base + 256 + j0, r);
-    }
-    tc_wait_st();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (threadIdx.x == 0) {
-        for (int ks = 0; ks < 8; ++ks)
-            mma_ts(tmem + 0, tmem + 256 + ks * 8, desc_sw128(sX + (ks >> 2) * 16384 + (ks & 3) * 32), idesc_f16(128, 128), ks > 0);
-        for (int ks = 0; ks < 8; ++ks)
-            mma_ss(tmem + 128, desc_sw128(sX + (ks >> 2) * 16384 + (ks & 3) * 32), desc_sw128(sWn + (ks >> 2) * 10240 + (ks & 3) * 32),
-                   idesc_f16(128, 80), ks > 0);
-        // MN-major B operand, four N=32 blocks (two per 64-point tile): out3 = W X^T again, columns 256..383 hold W so use D at 384
-        for (int blk = 0; blk < 4; ++blk)
-            for (int ks = 0; ks < 8; ++ks)
-                mma_ts(tmem + 384 + 32 * blk, tmem + 256 + ks * 8,
-                       desc_mn_sw128(sXmn + (blk >> 1) * 16384 + (blk & 1) * 64 + ks * 2048, 16384, 1024), idesc_f16(128, 32, 0, 1), ks > 0);
-        tc_commit(bar);
-    }
-    mbar_wait(bar, 0, err, 99);
-    tc_fence_after();
-    for (int cb = 0; cb < 4; ++cb) {
-        uint32_t r[32];
-        tmem_ld32(lane_base + cb * 32, r);
-        tc_wait_ld();
-        for (int i = 0; i < 32; ++i) out1[c * 128 + cb * 32 + i] = __uint_as_float(r[i]);
-        tmem_ld32(lane_base + 384 + cb * 32, r);
-        tc_wait_ld();
-        for (int i = 0; i < 32; ++i) out3[c * 128 + cb * 32 + i] = __uint_as_float(r[i]);
-    }
-    for (int j = 0; j < 5; ++j) {
-        uint32_t r[16];
-        tmem_ld16(lane_base + 128 + 16 * j, r);
-        tc_wait_ld();
-        for (int i = 0; i < 16; ++i) out2[c * 80 + 16 * j + i] = __uint_as_float(r[i]);
-    }
-    // MN-major A operand (M = 128 points = two 64-groups, LBO 16 KB): out4 = X Wn^T again, into columns 128..207
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    if (threadIdx.x == 0) {
-        for (int ks = 0; ks < 8; ++ks)
-            mma_ss(tmem + 128, desc_mn_sw128(sXmn + ks * 2048, 16384, 1024), desc_sw128(sWn + (ks >> 2) * 10240 + (ks & 3) * 32),
-                   idesc_f16(128, 80, 1, 0), ks > 0);
-        tc_commit(bar);
-    }
-    mbar_wait(bar, 1, err, 98);
-    tc_fence_after();
-    for (int j = 0; j < 5; ++j) {
-        uint32_t r[16];
-        tmem_ld16(lane_base + 128 + 16 * j, r);
-        tc_wait_ld();
-        for (int i = 0; i < 16; ++i) out4[c * 80 + 16 * j + i] = __uint_as_float(r[i]);
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 512);
-}
-
-// self-test of the transpose-accumulate MMA: outa[n][p] = outb[n][p] = X[p][n] (fp16-rounded), X (128 points, 128 channels) staged as the
-// SW128 K-major tile the producers write; outa uses (LBO, SBO) = (K stride, 8-row-group stride), outb the swapped reading of the
-// descriptor fields (exactly one of them is right; the test pins which, the kernel uses that one)
-__global__ void __launch_bounds__(128, 1) selftest_transpose_kernel(const float* __restrict__ X, float* __restrict__ outa,
-                                                                    float* __restrict__ outb, int* err) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    unsigned char* sgen = smem_raw + (sbase - smem_u32(smem_raw));
-    const uint32_t sX = sbase, sI = sbase + 32768, bar = sbase + 32768 + 8192;
-    volatile uint32_t* slot = reinterpret_cast<volatile uint32_t*>(sgen + 32768 + 8192 + 16);
-    const int warp = threadIdx.x >> 5, c = threadIdx.x;
-    if (threadIdx.x == 0) { mbar_init(bar, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-    if (warp == 0) tmem_alloc(sbase + 32768 + 8192 + 16, 512);
-    __half* xs = reinterpret_cast<__half*>(sgen);
-    for (int e = threadIdx.x; e < 128 * 128; e += 128) xs[sw128_off(e / 128, e % 128, 128) / 2] = __float2half_rn(X[e]);
-    ident_fill(sgen + 32768, threadIdx.x, 128);
-    __syncthreads();
-    ident_ones(sgen + 32768, threadIdx.x);
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *slot;
-    const uint32_t lane_base = tmem + ((uint32_t)(warp * 32) << 16);
-    if (threadIdx.x == 0) {
-        for (int var = 0; var < 2; ++var)
-            for (int blk = 0; blk < 4; ++blk)
-                for (int ks = 0; ks < 8; ++ks)
-                    mma_ss(tmem + 128 * var + 32 * blk, desc_ident(sI, ks, var == 1),
-                           desc_sw128(sX + (ks >> 2) * 16384 + blk * 32 * 128 + (ks & 3) * 32), idesc_f16(128, 32), ks > 0);
-        tc_commit(bar);
-    }
-    mbar_wait(bar, 0, err, 97);
-    tc_fence_after();
-    for (int cb = 0; cb < 4; ++cb) {
-        uint32_t r[32];
-        tmem_ld32(lane_base + cb * 32, r);
-        tc_wait_ld();
-        for (int i = 0; i < 32; ++i) outa[c * 128 + cb * 32 + i] = __uint_as_float(r[i]);
-        tmem_ld32(lane_base + 128 + cb * 32, r);
-        tc_wait_ld();
-        for (int i = 0; i < 32; ++i) outb[c * 128 + cb * 32 + i] = __uint_as_float(r[i]);
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 512);
-}
-
-
-// self-test of the texel-window MMA: one TMA box (64 ch x 4 x 4 texels x 4 groups, 128B swizzle) staged as the MN-major A operand,
-// a [64 points x 16 texels] no-swizzle K-major tap-weight tile as B:  out0 / out3 [channel][point] = sum_k win[k][channel (+128)] wt[point][k]
-__global__ void __launch_bounds__(128, 1) selftest_window_kernel(const __grid_constant__ CUtensorMap tmap, int ox, int oy,
-                                                                 const float* __restrict__ wt, float* __restrict__ out0,
-                                                                 float* __restrict__ out3, int* err) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    unsigned char* sgen = smem_raw + (sbase - smem_u32(smem_raw));
-    const uint32_t sWin = sbase, sWt = sbase + WIN_BYTES, bar = sbase + WIN_BYTES + WT_BYTES, bar2 = bar + 8;
-    volatile uint32_t* slot = reinterpret_cast<volatile uint32_t*>(sgen + WIN_BYTES + WT_BYTES + 16);
-    const int warp = threadIdx.x >> 5, c = threadIdx.x;
-    if (threadIdx.x == 0) { mbar_init(bar, 1); mbar_init(bar2, 1); asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-    if (warp == 0) tmem_alloc(sbase + WIN_BYTES + WT_BYTES + 16, 512);
-    for (int e = threadIdx.x; e < 64 * 16; e += 128) {
-        const int r = e / 16, k = e % 16;
-        *reinterpret_cast<__half*>(sgen + WIN_BYTES + (r >> 3) * 256 + (k >> 3) * 128 + (r & 7) * 16 + (k & 7) * 2) = __float2half_rn(wt[e]);
-    }
-    fence_proxy_async();
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *slot;
-    if (threadIdx.x == 0) {
-        mbar_expect_tx(bar, WIN_BYTES);
-        tma_load_window(sWin, &tmap, ox, oy, 0, bar);
-    }
-    mbar_wait(bar, 0, err, 96);
-    tc_fence_after();
-    if (threadIdx.x == 0) {
-        mma_ss(tmem + 0, desc_mn_sw128(sWin, 2048, 1024), desc_nosw(sWt, 128, 256), idesc_f16(128, 64, 1, 0), 0);
-        mma_ss(tmem + 64, desc_mn_sw128(sWin + 4096, 2048, 1024), desc_nosw(sWt, 128, 256), idesc_f16(128, 64, 1, 0), 0);
-        tc_commit(bar2);
-    }
-    mbar_wait(bar2, 0, err, 95);
-    tc_fence_after();
-    const uint32_t lane_base = tmem + ((uint32_t)(warp * 32) << 16);
-    for (int cb = 0; cb < 2; ++cb) {
-        uint32_t r[32];
-        tmem_ld32(lane_base + cb * 32, r);
-        tc_wait_ld();
-        for (int i = 0; i < 32; ++i) out0[c * 64 + cb * 32 + i] = __uint_as_float(r[i]);
-        tmem_ld32(lane_base + 64 + cb * 32, r);
-        tc_wait_ld();
-        for (int i = 0; i < 32; ++i) out3[c * 64 + cb * 32 + i] = __uint_as_float(r[i]);
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem, 512);
-}
-__global__ void selftest_group_kernel(const float* __restrict__ in, int HW, __half* __restrict__ out) {
-    const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= HW * 256) return;
-    const int p = idx / 256, ch = idx % 256;
-    out[((size_t)(ch >> 6) * HW + p) * 64 + (ch & 63)] = __float2half_rn(in[idx]);
 }
 
 }  // namespace tc
@@ -1596,8 +602,7 @@ __global__ void selftest_group_kernel(const float* __restrict__ in, int HW, __ha
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-static long long* g_dbg = nullptr;   // diagnostics only (neo_tc_debug); reset by every scene creation
-static int* g_trap_host = nullptr;   // host-mapped int[8] written by mbar_timeout before a protocol trap
+static int* g_trap_host = nullptr;   // host-mapped int[8] written by load_timeout before a trap
 static int* g_trap_dev = nullptr;
 
 static int trap_buffer() {
@@ -1615,33 +620,9 @@ const char* tc_trap_info() {
     static char buf[256];
     if (!g_trap_host || g_trap_host[0] == 0) return "";
     volatile int* t = g_trap_host;
-    snprintf(buf, sizeof(buf), " [TC field kernel: mbarrier wait timed out: tag %d, CTA %d of %d, thread %d (warp %d), barrier smem 0x%x (index %d), parity %d]",
-             t[0] - 1000, t[1], t[5], t[2], t[2] / 32, (unsigned)t[3], ((unsigned)t[3] % 1024u - (tc::SM_BAR % 1024u)) / 8, t[4]);
+    snprintf(buf, sizeof(buf), " [TC field kernel: weight load timed out: CTA %d of %d, thread %d, barrier smem 0x%x]",
+             t[1], t[5], t[2], (unsigned)t[3]);
     return buf;
-}
-
-// 4-D TMA descriptor over a projected map [nv*4 + group][H][W][64] fp16: box = 64 channels x 4 x 4 texels x 4 groups, 128B swizzle
-// (the field kernel's MN-major A operand), zero fill outside the map.  The driver entry point is fetched through the runtime so
-// the library links against cudart only.
-static int make_window_tmap(CUtensorMap* out, void* base, int W, int H, int nv) {
-    typedef CUresult (*EncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-    static EncodeTiled encode = nullptr;
-    if (!encode) {
-        void* fn = nullptr;
-        cudaDriverEntryPointQueryResult qr;
-        NEO_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qr));
-        if (!fn || qr != cudaDriverEntryPointSuccess) { set_error("cuTensorMapEncodeTiled not available from this driver"); return NEO_ERR_UNSUPPORTED; }
-        encode = reinterpret_cast<EncodeTiled>(fn);
-    }
-    const cuuint64_t dims[4] = {64, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)nv * 4};
-    const cuuint64_t strides[3] = {128, (cuuint64_t)128 * W, (cuuint64_t)128 * W * H};
-    const cuuint32_t box[4] = {64, 4, 4, 4}, estr[4] = {1, 1, 1, 1};
-    const CUresult r = encode(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                              CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d) for a %d x %d map", (int)r, W, H); return NEO_ERR_CUDA; }
-    return NEO_OK;
 }
 
 int gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M, int N, int K,
@@ -1652,7 +633,6 @@ int tc_scene_create(NeoScene* sc, const NeoMLPParams mlps[4], cudaStream_t s) {
     const NeoSceneDesc& d = sc->desc;
     State* st = new State();
     sc->tc_state = st;
-    g_dbg = nullptr;
     const float* planes[3] = {d.planes_xz, d.planes_xy, d.planes_yz};
     // channel-last fp16 copies of the raw feature maps (temporary: shared by the four MLPs' pre-projections) and the packed weight rows
     struct Temps {                                   // handed back to the block pool on every exit path (after the stream has drained)
@@ -1693,22 +673,23 @@ int tc_scene_create(NeoScene* sc, const NeoMLPParams mlps[4], cudaStream_t s) {
         const int in_dim = m.enc_dim + kLocalCh + kWorldCh;
         void* q = nullptr;
         int rc;
-        const int nwords = ((2 * m.KE + 384) / 2) * 128;
-        if ((rc = scene_alloc_bytes(sc, &q, (size_t)nwords * 4))) return rc;
-        m.wimg = (const uint32_t*)q;
-        wimg_kernel<<<(nwords + 255) / 256, 256, 0, s>>>(p, m.enc_dim, m.KE, (uint32_t*)q);
-        NEO_LAUNCH_CHECK("wimg_kernel");
+        const uint32_t tbytes = trunk_bytes(m.KE);
+        if ((rc = scene_alloc_bytes(sc, &q, tbytes))) return rc;
+        m.trunkimg = (const unsigned char*)q;
+        const int nelem = (2 * enc_slabs(m.KE) * 64 + 384) * 128;
+        trunk_img_kernel<<<(nelem + 255) / 256, 256, 0, s>>>(p, m.enc_dim, m.KE, (unsigned char*)q);
+        NEO_LAUNCH_CHECK("trunk_img_kernel");
         void* hb = nullptr; void* bb = nullptr;
         if ((rc = scene_alloc_bytes(sc, &hb, WH_BYTES))) return rc;
-        if ((rc = scene_alloc_bytes(sc, &bb, BIAS_FLOATS * 4))) return rc;
+        if ((rc = scene_alloc_bytes(sc, &bb, BIAS_BYTES))) return rc;
         NEO_CUDA(cudaMemsetAsync(hb, 0, WH_BYTES, s));
+        NEO_CUDA(cudaMemsetAsync(bb, 0, BIAS_BYTES, s));
         head_kernel<<<(80 * 128 + 80 * 64 + 64 * 64 + 16 * 64 + 255) / 256, 256, 0, s>>>(p, d.nv, (unsigned char*)hb, (float*)bb);
         NEO_LAUNCH_CHECK("head_kernel");
-        m.headimg = (const uint4*)hb;
+        m.headimg = (const unsigned char*)hb;
         m.bias = (const float*)bb;
-        // pre-projected feature maps [P0 | P3], stored as 64-channel groups [nv*4 + group][H][W][64] + their TMA descriptors.
-        // P = F . Wsel^T is a plain contraction over the raw channels: on tcgen05 through gemm_f16 (csrc/gemm_tc.cu), one N = 64 GEMM
-        // per (view, channel group) writing its plane of the grouped layout directly (fp16 features x fp16 weights, fp32 accumulate).
+        // pre-projected feature maps [P0 | P3] in pmap_logical channel order, [nv][H][W][256]: P = F . Wsel^T is a plain contraction
+        // over the raw channels, one N = 256 gemm_f16 per view (fp16 features x fp16 weights, fp32 accumulate)
         for (int k = 0; k < 4; ++k) {
             const int C = k ? kWorldCh : kLocalCh, mh = k ? d.plane_h : d.lat_h, mw = k ? d.plane_w : d.lat_w, hw = mh * mw;
             const int col = m.enc_dim + (k ? kLocalCh : 0);
@@ -1718,10 +699,8 @@ int tc_scene_create(NeoScene* sc, const NeoMLPParams mlps[4], cudaStream_t s) {
             wsel_kernel<<<(256 * C + 255) / 256, 256, 0, s>>>(p.w0, in_dim, col, p.w3, 128 + in_dim, 128 + col, C, wsel);
             NEO_LAUNCH_CHECK("wsel_kernel");
             for (int v = 0; v < d.nv; ++v)
-                for (int g = 0; g < 4; ++g)
-                    if ((rc = gemm_f16(feat16[k] + (size_t)v * hw * C, C, wsel + (size_t)g * 64 * C, C, nullptr,
-                                       (__half*)pp + ((size_t)(v * 4 + g) * hw) * 64, 64, hw, 64, C, 0, s))) return rc;
-            if ((rc = make_window_tmap(&m.tmap[k], pp, mw, mh, d.nv))) return rc;
+                if ((rc = gemm_f16(feat16[k] + (size_t)v * hw * C, C, wsel, C, nullptr, (__half*)pp + (size_t)v * hw * 256, 256, hw, 256, C, 0, s)))
+                    return rc;
         }
         NEO_CUDA(cudaStreamSynchronize(s));          // wsel is reused by the next MLP
     }
@@ -1732,7 +711,6 @@ int tc_scene_create(NeoScene* sc, const NeoMLPParams mlps[4], cudaStream_t s) {
 void tc_scene_free(NeoScene* sc) {
     if (sc && sc->tc_state) { delete reinterpret_cast<tc::State*>(sc->tc_state); sc->tc_state = nullptr; }
 }
-
 
 int launch_field_tc(const NeoScene* sc, const NeoRays* rays, const float* far, const float* t, int N, int mlp_index,
                     float* rgb, float* sigma, cudaStream_t s) {
@@ -1752,25 +730,24 @@ int launch_field_tc(const NeoScene* sc, const NeoRays* rays, const float* far, c
     P.sg = (N + kTileSamples - 1) / kTileSamples;
     const long long groups = ((long long)rays->n_rays + kTileRays - 1) / kTileRays;
     const long long n_tiles = groups * P.sg;
-    if (n_tiles > 0x7fffffffLL) { set_error("too many tiles"); return NEO_ERR_UNSUPPORTED; }
+    if (n_tiles > 0x3fffffffLL) { set_error("too many tiles"); return NEO_ERR_UNSUPPORTED; }
     P.n_tiles = (int)n_tiles;
     P.far_unc = 3.0f;
     P.sc = sc->dev;
     P.mlp = st->mlp[mlp_index];
-    P.rgb_out = rgb; P.sigma_out = sigma; P.err = sc->err_flag;
+    P.rgb_out = rgb; P.sigma_out = sigma;
     { int rc0 = trap_buffer(); if (rc0) return rc0; }
     P.trap = g_trap_dev;
-    P.dbg = g_dbg;
-    const int grid = (int)(n_tiles < n_sm ? n_tiles : n_sm);
-    const size_t smem = SM_TOTAL + 1024;
-    auto launch = [&](auto kern) -> int {
+    const long long ctas = (n_tiles + kWarpgroups - 1) / kWarpgroups;
+    const int grid = (int)(ctas < n_sm ? ctas : n_sm);
+    auto launch = [&](auto kern, size_t smem) -> int {
         NEO_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, kThreads, smem, s>>>(P);
         return NEO_OK;
     };
     int rc;
-    if (mlp_index & 1) rc = g_dbg ? launch(field_tc_kernel<4, true>) : launch(field_tc_kernel<4, false>);
-    else rc = g_dbg ? launch(field_tc_kernel<3, true>) : launch(field_tc_kernel<3, false>);
+    if (mlp_index & 1) rc = launch(field_tc_kernel<4>, SmemMap<96>::TOTAL + 1024);
+    else rc = launch(field_tc_kernel<3>, SmemMap<64>::TOTAL + 1024);
     if (rc != NEO_OK) return rc;
     NEO_LAUNCH_CHECK("field_tc_kernel");
     return NEO_OK;
@@ -1778,51 +755,6 @@ int launch_field_tc(const NeoScene* sc, const NeoRays* rays, const float* far, c
 
 }  // namespace neo
 
-// X (128,128) W (128,128) Wn (80,128) device fp32 -> out1 = out3 (128,128) = W X^T (K-major / MN-major B), out2 = out4 (128,80) = X Wn^T
-// (K-major / MN-major A), fp16 operands
-extern "C" int neo_tc_selftest(const float* X, const float* W, const float* Wn, float* out1, float* out2, float* out3, float* out4,
-                               void* stream) {
-    using namespace neo;
-    const size_t smem = 86016 + 64 + 1024;
-    NEO_CUDA(cudaFuncSetAttribute(tc::selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    tc::selftest_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(X, W, Wn, out1, out2, out3, out4, nullptr);
-    NEO_LAUNCH_CHECK("selftest_kernel");
-    return NEO_OK;
-}
-
-// Debug: cycle accounting of the TC field kernel.  buf = device array of 148*16 int64 (zeroed by the caller) or NULL to disable.
-// Per CTA: [0] pts [1] wait ENC_FREE [2] geometry [3] producer bar [4] wait G_FREE [5] gather | [6] MMA wait ENC_READY
-// [7] MMA wait H_READY [8] MMA issue | [9] epi wait ACC [10] epi wait G [11] epi work [12] epi head
-extern "C" int neo_tc_selftest_transpose(const float* X, float* outa, float* outb, void* stream) {
-    using namespace neo;
-    const size_t smem = 32768 + 8192 + 64 + 1024;
-    NEO_CUDA(cudaFuncSetAttribute(tc::selftest_transpose_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    tc::selftest_transpose_kernel<<<1, 128, smem, (cudaStream_t)stream>>>(X, outa, outb, nullptr);
-    NEO_LAUNCH_CHECK("selftest_transpose_kernel");
-    return NEO_OK;
-}
-// texels (H*W, 256) fp32 texel-major, wt (64,16) fp32 -> out0 / out3 (128,64): the bilinear-blend MMA of one 4x4 window at (ox, oy)
-extern "C" int neo_tc_selftest_window(const float* texels, int H, int W, int ox, int oy, const float* wt, float* out0, float* out3,
-                                      void* stream) {
-    using namespace neo;
-    if (H < 1 || W < 1 || !texels || !wt || !out0 || !out3) { set_error("neo_tc_selftest_window: bad arguments"); return NEO_ERR_INVALID; }
-    cudaStream_t s = (cudaStream_t)stream;
-    __half* grouped = nullptr;
-    NEO_CUDA(cudaMalloc(&grouped, (size_t)H * W * 256 * sizeof(__half)));
-    tc::selftest_group_kernel<<<(H * W * 256 + 255) / 256, 256, 0, s>>>(texels, H * W, grouped);
-    alignas(64) CUtensorMap tm;
-    int rc = make_window_tmap(&tm, grouped, W, H, 1);
-    if (rc == NEO_OK) {
-        const size_t smem = tc::WIN_BYTES + tc::WT_BYTES + 64 + 1024;
-        cudaFuncSetAttribute(tc::selftest_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        tc::selftest_window_kernel<<<1, 128, smem, s>>>(tm, ox, oy, wt, out0, out3, nullptr);
-        cudaError_t e = cudaGetLastError();
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) rc = cuda_fail(e, "selftest_window_kernel");
-    }
-    cudaFree(grouped);
-    return rc;
-}
 extern "C" int neo_tc_enc_column(int in_ch, int col) {
     using namespace neo::tc;
     if ((in_ch != 3 && in_ch != 4) || col < 0 || col >= (in_ch == 3 ? 64 : 96)) return -3;
@@ -1832,4 +764,3 @@ extern "C" int neo_tc_enc_column(int in_ch, int col) {
     return (in_ch == 3) ? enc_col_ref_index<3>(col) : enc_col_ref_index<4>(col);
 }
 extern "C" const char* neo_tc_trap_info(void) { return neo::tc_trap_info(); }
-extern "C" int neo_tc_debug(long long* buf) { neo::g_dbg = buf; return NEO_OK; }

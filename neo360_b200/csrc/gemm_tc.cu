@@ -1,456 +1,93 @@
-// Generic dense layer on tcgen05 tensor cores (sm_100a):  C[M][N] = act(A[M][K] . W[N][K]^T + bias)   fp16 operands, fp32 accumulate.
+// Generic dense layer on Hopper tensor cores (sm_90a):  C[M][N] = act(A[M][K] . W[N][K]^T + bias)   fp16 operands, fp32 accumulate.
 // A and W are K-major (row-major activations, nn.Linear weights), so both operands are staged by 2-D TMA tile loads
-// (cp.async.bulk.tensor.2d, 128-byte swizzle) straight into the layout the MMA reads.  Used by the tensor-core paths of the wide
-// MLPs: Mip-NeRF 360's 8 x 1024 NeRF MLP and 4 x 256 proposal MLPs (models/mipnerf360/model.py:30-195).
+// (cp.async.bulk.tensor.2d, 128-byte swizzle) straight into the layout wgmma reads.  Used by the tensor-core paths of the wide
+// MLPs: Mip-NeRF 360's 8 x 1024 NeRF MLP and 4 x 256 proposal MLPs (models/mipnerf360/model.py:30-195), vanilla NeRF, the encoder
+// and the per-scene pre-projection of the NeO-360 feature maps.
 //
-// One persistent CTA per SM walks (m-tile, n-tile) pairs, n fastest so the CTAs working at the same time share A tiles in L2.
-// 192 threads: warp 0 = TMA producer (one lane), warp 1 = MMA issue (one lane) + TMEM allocation, warps 2-5 = epilogue (TMEM lane
-// quarter warp % 4).  4-stage shared-memory ring (A 128 x 64, W BN x 64 per stage), two TMEM accumulators (2 x BN columns) so the
-// epilogue of tile i (tcgen05.ld -> bias -> ReLU -> fp16 -> per-warp shared-memory transpose -> whole 128-byte lines to global)
-// overlaps the MMAs of tile i + 1.
-// Large problems with N % 256 == 0 (the 1024- and 256-wide layers over millions of rows) run the CTA-pair variant further down
-// (gemm_f16_pair_kernel: tcgen05.mma.cta_group::2, 256 x 256 tiles, 6-stage ring); the single-CTA kernel serves everything else.
+// One CTA per 128 x BN output tile: warp 8 = TMA producer (one lane), warps 0-7 = two consumer warpgroups, each owning 64 rows of the
+// tile (wgmma m64nBNk16, accumulators in registers).  3-stage shared-memory ring (A 128 x 64, W BN x 64 per stage) with full / empty
+// mbarriers; two CTAs fit on an SM, so one CTA's epilogue (bias -> ReLU -> fp16 -> global) overlaps the other's main loop.
 #include "common.cuh"
+#include "hopper.cuh"
 #include <cuda.h>
 #include <cuda_fp16.h>
-#include <cstdlib>
 
 namespace neo {
 namespace gemm {
+using namespace hopper;
 
-constexpr int BM = 128, BK = 64, kStages = 4, kThreads = 192;
+constexpr int BM = 128, BK = 64, kStages = 3, kConsumerWarps = 8, kThreads = (kConsumerWarps + 1) * 32;
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) { asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count)); }
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-// bounded wait: a protocol bug traps instead of hanging the GPU
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p, q;\n\t.reg .u32 c;\n\t"
-        "mov.u32 c, 0;\n\t"
-        "mov.u32 %0, 1;\n\t"
-        "GEMM_WAIT_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2, %3;\n\t"
-        "@p bra GEMM_DONE_%=;\n\t"
-        "add.u32 c, c, 1;\n\t"
-        "setp.lt.u32 q, c, 0x4000000;\n\t"
-        "@q bra GEMM_WAIT_%=;\n\t"
-        "mov.u32 %0, 0;\n\t"
-        "GEMM_DONE_%=:\n\t}"
-        : "=r"(ok) : "r"(bar), "r"(parity), "r"(2000u) : "memory");
-    if (!ok) asm volatile("trap;");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tmap, int c0, int c1, uint32_t bar) {
-    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                 ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(bar) : "memory");
-}
-// K-major, 128-byte-swizzled operand descriptor: rows of 128 B (64 fp16), 8-row groups 1024 B apart
-__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024u >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-__host__ __device__ constexpr uint32_t idesc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accum), "r"(0u) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
-    __half2 h = __floats2half2_rn(a, b);
-    return *reinterpret_cast<uint32_t*>(&h);
-}
-
-// Epilogue of one warp for one accumulator tile: its 32 TMEM lanes (rows) x NCOLS columns -> bias -> ReLU -> fp16 -> global.
-// A lane owns a ROW of the accumulator, so storing straight from registers would touch 32 different rows per instruction (32 partial
-// sectors each).  Instead every 64 columns are transposed through a 4 KB per-warp staging tile ([32 rows][128 B], 16-byte pieces
-// XOR-swizzled by row: conflict-free both ways) and leave as whole 128-byte lines, 4 rows per store instruction.
-constexpr uint32_t kEpiStage = 32 * 128;           // bytes per epilogue warp
-template <int NCOLS>
-__device__ __forceinline__ void epilogue_rows(uint32_t tmem_lanes /*lane base + accumulator column*/, uint32_t stage, const float* __restrict__ bias,
-                                              __half* __restrict__ C, long long ldc, long long row0 /*first of the warp's 32 rows*/, long long M,
-                                              int n0, int relu, int lane) {
-#pragma unroll 1
-    for (int cc = 0; cc < NCOLS / 64; ++cc) {
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            uint32_t r[32];
-            tmem_ld32(tmem_lanes + cc * 64 + h * 32, r);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                float v[8];
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    float x = __uint_as_float(r[8 * j + i]) + (bias ? __ldg(bias + n0 + cc * 64 + h * 32 + 8 * j + i) : 0.f);
-                    v[i] = relu ? fmaxf(x, 0.f) : x;
-                }
-                const uint32_t piece = (uint32_t)(4 * h + j) ^ (uint32_t)(lane & 7);
-                asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(stage + lane * 128 + piece * 16), "r"(pack_h2(v[0], v[1])),
-                             "r"(pack_h2(v[2], v[3])), "r"(pack_h2(v[4], v[5])), "r"(pack_h2(v[6], v[7])) : "memory");
-            }
-        }
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            const int rr = i * 4 + (lane >> 3), p = lane & 7;
-            uint4 val;
-            asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(val.x), "=r"(val.y), "=r"(val.z), "=r"(val.w)
-                         : "r"(stage + rr * 128 + ((p ^ (rr & 7)) * 16)) : "memory");
-            if (row0 + rr < M) *reinterpret_cast<uint4*>(C + (row0 + rr) * ldc + n0 + cc * 64 + p * 8) = val;
-        }
-        __syncwarp();
-    }
-}
+template <int BN> struct Acc;
+template <> struct Acc<128> {
+    static __device__ __forceinline__ void mma(float (&d)[64], uint64_t a, uint64_t b) { wgmma_ss_n128(d, a, b); }
+};
+template <> struct Acc<64> {
+    static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b) { wgmma_ss_n64(d, a, b); }
+};
 
 template <int BN>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kThreads, 2)
 gemm_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const float* __restrict__ bias,
-                __half* __restrict__ C, long long M, int N, int K, long long ldc, int relu) {
+                __half* __restrict__ C, long long M, int K, long long ldc, int relu) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    unsigned char* sgen = smem_raw + (sbase - smem_u32(smem_raw));
     constexpr uint32_t A_BYTES = BM * BK * 2, W_BYTES = BN * BK * 2, STAGE = A_BYTES + W_BYTES;
     const uint32_t bar0 = sbase + kStages * STAGE;
     auto FULL = [&](int s) { return bar0 + 8u * s; };
     auto EMPTY = [&](int s) { return bar0 + 8u * (kStages + s); };
-    auto ACC_FULL = [&](int a) { return bar0 + 8u * (2 * kStages + a); };
-    auto ACC_EMPTY = [&](int a) { return bar0 + 8u * (2 * kStages + 2 + a); };
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(sgen + kStages * STAGE + 8 * (2 * kStages + 4));
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t epi_stage = sbase + ((kStages * STAGE + 8 * (2 * kStages + 4) + 16 + 127) & ~127u) + (warp & 3) * kEpiStage;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(ACC_FULL(a), 1); mbar_init(ACC_EMPTY(a), 4); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        for (int s = 0; s < kStages; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), kConsumerWarps / 4); }
+        mbar_init_fence();
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sbase + kStages * STAGE + 8 * (2 * kStages + 4)), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const int n_tiles_n = N / BN;
-    const long long n_tiles = ((M + BM - 1) / BM) * n_tiles_n;
     const int kblocks = K / BK;
+    const long long m0 = (long long)blockIdx.x * BM;
+    const int n0 = blockIdx.y * BN;
 
-    if (warp == 0) {
+    if (warp == kConsumerWarps) {
         if (lane == 0) {
-            uint32_t it = 0;
-            for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                const int m0 = (int)(tile / n_tiles_n) * BM, n0 = (int)(tile % n_tiles_n) * BN;
-                for (int kb = 0; kb < kblocks; ++kb, ++it) {
-                    const uint32_t s = it % kStages, ph = (it / kStages) & 1u;
-                    mbar_wait(EMPTY(s), ph ^ 1u);
-                    mbar_expect_tx(FULL(s), STAGE);
-                    tma_load_2d(sbase + s * STAGE, &tmA, kb * BK, m0, FULL(s));
-                    tma_load_2d(sbase + s * STAGE + A_BYTES, &tmW, kb * BK, n0, FULL(s));
-                }
+            for (int kb = 0; kb < kblocks; ++kb) {
+                const uint32_t s = kb % kStages, ph = (kb / kStages) & 1u;
+                mbar_wait(EMPTY(s), ph ^ 1u);
+                mbar_expect_tx(FULL(s), STAGE);
+                tma_load_2d(sbase + s * STAGE, &tmA, kb * BK, (int)m0, FULL(s));
+                tma_load_2d(sbase + s * STAGE + A_BYTES, &tmW, kb * BK, n0, FULL(s));
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            uint32_t it = 0, tcount = 0;
-            constexpr uint32_t idesc = idesc_f16(BM, BN);
-            for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-                const uint32_t acc = tcount & 1u, aph = (tcount >> 1) & 1u;
-                mbar_wait(ACC_EMPTY(acc), aph ^ 1u);                 // the epilogue has drained this accumulator
-                tc_fence_after();
-                const uint32_t d = tmem + acc * BN;
-                for (int kb = 0; kb < kblocks; ++kb, ++it) {
-                    const uint32_t s = it % kStages, ph = (it / kStages) & 1u;
-                    mbar_wait(FULL(s), ph);
-                    tc_fence_after();
-                    const uint32_t sa = sbase + s * STAGE, sw = sa + A_BYTES;
+        return;
+    }
+    const int wg = warp >> 2;
+    float acc[BN / 2];
 #pragma unroll
-                    for (int ks = 0; ks < BK / 16; ++ks)
-                        mma_ss(d, desc_sw128(sa + ks * 32), desc_sw128(sw + ks * 32), idesc, (kb > 0 || ks > 0) ? 1u : 0u);
-                    tc_commit(EMPTY(s));                             // the stage returns to the producer when these MMAs are done
-                }
-                tc_commit(ACC_FULL(acc));
-            }
-        }
-    } else {
-        const int q = warp & 3;                                      // TMEM lane quarter this warp may read
-        const uint32_t lane_base = tmem + ((uint32_t)(q * 32) << 16);
-        uint32_t tcount = 0;
-        for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-            const uint32_t acc = tcount & 1u, aph = (tcount >> 1) & 1u;
-            const long long m0 = (tile / n_tiles_n) * BM;
-            const int n0 = (int)(tile % n_tiles_n) * BN;
-            mbar_wait(ACC_FULL(acc), aph);
-            tc_fence_after();
-            epilogue_rows<BN>(lane_base + acc * BN, epi_stage, bias, C, ldc, m0 + q * 32, M, n0, relu, lane);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(ACC_EMPTY(acc));
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------
-// Weight-stationary variant for the 256-wide layers (N == 256, K <= 256: vanilla NeRF's 8 x 256 trunk, the Mip-NeRF 360 proposal
-// MLPs): the whole weight matrix (<= 128 KB fp16) is loaded into shared memory ONCE per CTA and only the activation tiles stream through
-// the ring.  These layers are activation-bandwidth bound (1 KB of HBM traffic per 131 kFLOP row); re-fetching the 128 KB weight tile for
-// every 64 KB activation tile, as the generic kernels do, triples the L2 -> SM traffic for nothing.
-// ------------------------------------------------------------------------------------------------
-constexpr int kStagesWS = 5, BNW = 256;
-__global__ void __launch_bounds__(kThreads, 1)
-gemm_f16_ws_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const float* __restrict__ bias,
-                   __half* __restrict__ C, long long M, int K, long long ldc, int relu) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    unsigned char* sgen = smem_raw + (sbase - smem_u32(smem_raw));
-    constexpr uint32_t A_BYTES = BM * BK * 2, WK_BYTES = BNW * BK * 2, W_MAX = 4 * WK_BYTES;      // resident weights: up to 4 k-blocks of 32 KB
-    const uint32_t ring = sbase + W_MAX;
-    const uint32_t bar0 = ring + kStagesWS * A_BYTES;
-    auto FULL = [&](int s) { return bar0 + 8u * s; };
-    auto EMPTY = [&](int s) { return bar0 + 8u * (kStagesWS + s); };
-    auto ACC_FULL = [&](int a) { return bar0 + 8u * (2 * kStagesWS + a); };
-    auto ACC_EMPTY = [&](int a) { return bar0 + 8u * (2 * kStagesWS + 2 + a); };
-    const uint32_t W_FULL = bar0 + 8u * (2 * kStagesWS + 4);
-    const uint32_t slot_off = W_MAX + kStagesWS * A_BYTES + 8 * (2 * kStagesWS + 5);
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(sgen + slot_off);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t epi_stage = sbase + ((slot_off + 16 + 127) & ~127u) + (warp & 3) * kEpiStage;
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kStagesWS; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(ACC_FULL(a), 1); mbar_init(ACC_EMPTY(a), 4); }
-        mbar_init(W_FULL, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(sbase + slot_off), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const long long n_tiles = (M + BM - 1) / BM;
-    const int kblocks = K / BK;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            mbar_expect_tx(W_FULL, kblocks * WK_BYTES);
-            for (int kb = 0; kb < kblocks; ++kb) tma_load_2d(sbase + kb * WK_BYTES, &tmW, kb * BK, 0, W_FULL);
-            uint32_t it = 0;
-            for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                const int m0 = (int)tile * BM;
-                for (int kb = 0; kb < kblocks; ++kb, ++it) {
-                    const uint32_t s = it % kStagesWS, ph = (it / kStagesWS) & 1u;
-                    mbar_wait(EMPTY(s), ph ^ 1u);
-                    mbar_expect_tx(FULL(s), A_BYTES);
-                    tma_load_2d(ring + s * A_BYTES, &tmA, kb * BK, m0, FULL(s));
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            uint32_t it = 0, tcount = 0;
-            constexpr uint32_t idesc = idesc_f16(BM, BNW);
-            mbar_wait(W_FULL, 0);
-            for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-                const uint32_t acc = tcount & 1u, aph = (tcount >> 1) & 1u;
-                mbar_wait(ACC_EMPTY(acc), aph ^ 1u);
-                tc_fence_after();
-                const uint32_t d = tmem + acc * BNW;
-                for (int kb = 0; kb < kblocks; ++kb, ++it) {
-                    const uint32_t s = it % kStagesWS, ph = (it / kStagesWS) & 1u;
-                    mbar_wait(FULL(s), ph);
-                    tc_fence_after();
-                    const uint32_t sa = ring + s * A_BYTES, sw = sbase + kb * WK_BYTES;
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < kblocks; ++kb) {
+        const uint32_t s = kb % kStages, ph = (kb / kStages) & 1u;
+        mbar_wait(FULL(s), ph);
+        const uint32_t sa = sbase + s * STAGE + wg * 64 * 128, sw = sbase + s * STAGE + A_BYTES;
+        wgmma_fence();
 #pragma unroll
-                    for (int ks = 0; ks < BK / 16; ++ks)
-                        mma_ss(d, desc_sw128(sa + ks * 32), desc_sw128(sw + ks * 32), idesc, (kb > 0 || ks > 0) ? 1u : 0u);
-                    tc_commit(EMPTY(s));
-                }
-                tc_commit(ACC_FULL(acc));
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        const uint32_t lane_base = tmem + ((uint32_t)(q * 32) << 16);
-        uint32_t tcount = 0;
-        for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++tcount) {
-            const uint32_t acc = tcount & 1u, aph = (tcount >> 1) & 1u;
-            mbar_wait(ACC_FULL(acc), aph);
-            tc_fence_after();
-            epilogue_rows<BNW>(lane_base + acc * BNW, epi_stage, bias, C, ldc, tile * BM + q * 32, M, 0, relu, lane);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(ACC_EMPTY(acc));
-        }
+        for (int ks = 0; ks < BK / 16; ++ks) Acc<BN>::mma(acc, desc_sw128(sa + ks * 32), desc_sw128(sw + ks * 32));
+        wgmma_commit();
+        wgmma_wait<1>();                                   // the previous k-block's MMAs are done: its stage goes back to the producer
+        if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(EMPTY((kb - 1) % kStages));
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------
-// CTA-pair variant (cta_group::2): the two SMs of a cluster of 2 compute ONE 256 x 256 tile.  Each CTA stages its own 128 rows of A and
-// HALF of the W tile (128 of the 256 output columns); the pair's tensor cores read both halves of W, so per MMA cycle each SM pulls
-// 32 KB instead of 48 KB through L2 -> SM (the single-CTA kernel is bound there: ncu r2, 54 % tensor pipe at 3.5 TB/s DRAM).
-// Protocol (CUTLASS sm100 2-SM pipeline semantics, cutlass/pipeline/sm100_pipeline.hpp):
-//   * both CTAs issue their TMA loads with .cta_group::2; the transaction bytes of BOTH land on the LEADER's FULL barrier (peer bit of
-//     the barrier address cleared), which the leader arms with the pair's total byte count;
-//   * only the leader (cluster rank 0) issues tcgen05.mma.cta_group::2; tcgen05.commit.cta_group::2 with multicast mask 0b11 releases
-//     the shared-memory stage in both CTAs and publishes the accumulator to both epilogues;
-//   * each CTA's epilogue drains its own 128 TMEM lanes (its 128 rows x 256 columns) and arrives on the leader's ACC_EMPTY barrier.
-// ------------------------------------------------------------------------------------------------
-constexpr int kStages2 = 6, BN2 = 256;
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;        // clears the CTA-rank bit of a shared::cluster address: "the even CTA of the pair"
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ uint32_t cluster_id_x() { uint32_t r; asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r)); return r; }
-__device__ __forceinline__ uint32_t n_clusters_x() { uint32_t r; asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair(uint32_t dst, const CUtensorMap* tmap, int c0, int c1, uint32_t leader_bar) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-                 ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(leader_bar & kPeerBitMask) : "memory");
-}
-__device__ __forceinline__ void mma_ss_pair(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accum), "r"(0u) : "memory");
-}
-__device__ __forceinline__ void tc_commit_pair(uint32_t bar) {          // arrives on `bar` of BOTH CTAs when the pair's MMAs so far are done
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_leader(uint32_t bar) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(bar & kPeerBitMask) : "memory");
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kThreads, 1)
-gemm_f16_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW, const float* __restrict__ bias,
-                     __half* __restrict__ C, long long M, int N, int K, long long ldc, int relu) {
-    extern __shared__ __align__(1024) unsigned char smem_raw[];
-    const uint32_t sbase = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    unsigned char* sgen = smem_raw + (sbase - smem_u32(smem_raw));
-    constexpr uint32_t A_BYTES = BM * BK * 2, W_BYTES = (BN2 / 2) * BK * 2, STAGE = A_BYTES + W_BYTES;
-    const uint32_t bar0 = sbase + kStages2 * STAGE;
-    auto FULL = [&](int s) { return bar0 + 8u * s; };
-    auto EMPTY = [&](int s) { return bar0 + 8u * (kStages2 + s); };
-    auto ACC_FULL = [&](int a) { return bar0 + 8u * (2 * kStages2 + a); };
-    auto ACC_EMPTY = [&](int a) { return bar0 + 8u * (2 * kStages2 + 2 + a); };
-    const uint32_t tmem_slot_addr = bar0 + 8u * (2 * kStages2 + 4);
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(sgen + kStages2 * STAGE + 8 * (2 * kStages2 + 4));
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t epi_stage = sbase + ((kStages2 * STAGE + 8 * (2 * kStages2 + 4) + 16 + 127) & ~127u) + (warp & 3) * kEpiStage;
-    const uint32_t rank = cluster_ctarank();
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kStages2; ++s) { mbar_init(FULL(s), 1); mbar_init(EMPTY(s), 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(ACC_FULL(a), 1); mbar_init(ACC_EMPTY(a), 8); }     // 4 epilogue warps x 2 CTAs (leader's copy is the live one)
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot_addr), "r"(512u) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                    // the peer's barriers are initialised before anything is signalled across the pair
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
-    const int n_tiles_n = N / BN2;
-    const long long n_tiles = ((M + 2 * BM - 1) / (2 * BM)) * n_tiles_n;
-    const int kblocks = K / BK;
-    const long long cid = cluster_id_x(), ncl = n_clusters_x();
-
-    if (warp == 0) {
-        if (lane == 0) {
-            uint32_t it = 0;
-            for (long long tile = cid; tile < n_tiles; tile += ncl) {
-                const long long m0 = (tile / n_tiles_n) * (2 * BM) + (long long)rank * BM;
-                const int n0 = (int)(tile % n_tiles_n) * BN2 + (int)rank * (BN2 / 2);
-                for (int kb = 0; kb < kblocks; ++kb, ++it) {
-                    const uint32_t s = it % kStages2, ph = (it / kStages2) & 1u;
-                    mbar_wait(EMPTY(s), ph ^ 1u);
-                    if (rank == 0) mbar_expect_tx(FULL(s), 2 * STAGE);
-                    tma_load_2d_pair(sbase + s * STAGE, &tmA, kb * BK, (int)m0, FULL(s));
-                    tma_load_2d_pair(sbase + s * STAGE + A_BYTES, &tmW, kb * BK, n0, FULL(s));
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0 && rank == 0) {
-            uint32_t it = 0, tcount = 0;
-            constexpr uint32_t idesc = idesc_f16(2 * BM, BN2);
-            for (long long tile = cid; tile < n_tiles; tile += ncl, ++tcount) {
-                const uint32_t acc = tcount & 1u, aph = (tcount >> 1) & 1u;
-                mbar_wait(ACC_EMPTY(acc), aph ^ 1u);                 // both epilogues have drained this accumulator
-                tc_fence_after();
-                const uint32_t d = tmem + acc * BN2;
-                for (int kb = 0; kb < kblocks; ++kb, ++it) {
-                    const uint32_t s = it % kStages2, ph = (it / kStages2) & 1u;
-                    mbar_wait(FULL(s), ph);
-                    tc_fence_after();
-                    const uint32_t sa = sbase + s * STAGE, sw = sa + A_BYTES;
+    wgmma_wait<0>();
+    const int t = lane & 3;
+    const long long row0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
-                    for (int ks = 0; ks < BK / 16; ++ks)
-                        mma_ss_pair(d, desc_sw128(sa + ks * 32), desc_sw128(sw + ks * 32), idesc, (kb > 0 || ks > 0) ? 1u : 0u);
-                    tc_commit_pair(EMPTY(s));
-                }
-                tc_commit_pair(ACC_FULL(acc));
-            }
-        }
-    } else {
-        const int q = warp & 3;
-        const uint32_t lane_base = tmem + ((uint32_t)(q * 32) << 16);
-        uint32_t tcount = 0;
-        for (long long tile = cid; tile < n_tiles; tile += ncl, ++tcount) {
-            const uint32_t acc = tcount & 1u, aph = (tcount >> 1) & 1u;
-            const long long m0 = (tile / n_tiles_n) * (2 * BM) + (long long)rank * BM;
-            const int n0 = (int)(tile % n_tiles_n) * BN2;
-            mbar_wait(ACC_FULL(acc), aph);
-            tc_fence_after();
-            epilogue_rows<BN2>(lane_base + acc * BN2, epi_stage, bias, C, ldc, m0 + q * 32, M, n0, relu, lane);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_leader(ACC_EMPTY(acc));
+    for (int j = 0; j < BN / 8; ++j) {
+        const int col = n0 + 8 * j + 2 * t;
+        const float b0 = bias ? __ldg(bias + col) : 0.f, b1 = bias ? __ldg(bias + col + 1) : 0.f;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const long long r = row0 + 8 * i;
+            float v0 = acc[4 * j + 2 * i] + b0, v1 = acc[4 * j + 2 * i + 1] + b1;
+            if (relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+            if (r < M) *reinterpret_cast<__half2*>(C + r * ldc + col) = __floats2half2_rn(v0, v1);
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                    // neither CTA frees tensor memory (or exits) while its peer may still touch the pair's state
-    if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(512u) : "memory");
 }
 
 // out[r][c] = fp16(in[r][c]) for c < cols_in, 0 for cols_in <= c < cols_out          (weight / activation packing with K padding)
@@ -492,48 +129,12 @@ static int launch(const __half* A, long long lda, const __half* W, long long ldw
     int rc;
     if ((rc = make_tmap_2d(&tmA, A, M, K, lda, BM))) return rc;
     if ((rc = make_tmap_2d(&tmW, W, N, K, ldw, BN))) return rc;
-    static int n_sm_of[64] = {0};
-    int dev = 0;
-    NEO_CUDA(cudaGetDevice(&dev));
-    if (dev < 0 || dev >= 64) { set_error("device index %d out of range", dev); return NEO_ERR_UNSUPPORTED; }
-    if (!n_sm_of[dev]) NEO_CUDA(cudaDeviceGetAttribute(&n_sm_of[dev], cudaDevAttrMultiProcessorCount, dev));
-    const long long tiles = ((M + BM - 1) / BM) * (N / BN);
-    const int grid = (int)(tiles < n_sm_of[dev] ? tiles : n_sm_of[dev]);
-    const size_t smem = (((size_t)kStages * (BM * BK * 2 + BN * BK * 2) + 8 * (2 * kStages + 4) + 16 + 127) & ~(size_t)127) + 4 * kEpiStage + 1024;
+    const long long m_tiles = (M + BM - 1) / BM;
+    if (m_tiles > 0x7fffffffLL) { set_error("gemm_f16: M = %lld is too large", M); return NEO_ERR_UNSUPPORTED; }
+    const size_t smem = (size_t)kStages * (BM * BK * 2 + BN * BK * 2) + 8 * 2 * kStages + 1024;
     NEO_CUDA(cudaFuncSetAttribute(gemm_f16_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    gemm_f16_kernel<BN><<<grid, kThreads, smem, s>>>(tmA, tmW, bias, C, M, N, K, ldc, relu);
+    gemm_f16_kernel<BN><<<dim3((unsigned)m_tiles, N / BN), kThreads, smem, s>>>(tmA, tmW, bias, C, M, K, ldc, relu);
     NEO_LAUNCH_CHECK("gemm_f16_kernel");
-    return NEO_OK;
-}
-
-static int launch_ws(const __half* A, long long lda, const __half* W, long long ldw, const float* bias, __half* C, long long ldc, long long M,
-                     int K, int relu, int n_sm, cudaStream_t s) {
-    alignas(64) CUtensorMap tmA, tmW;
-    int rc;
-    if ((rc = make_tmap_2d(&tmA, A, M, K, lda, BM))) return rc;
-    if ((rc = make_tmap_2d(&tmW, W, BNW, K, ldw, BNW))) return rc;
-    const long long tiles = (M + BM - 1) / BM;
-    const int grid = (int)(tiles < n_sm ? tiles : n_sm);
-    const size_t smem = (((size_t)4 * BNW * BK * 2 + (size_t)kStagesWS * BM * BK * 2 + 8 * (2 * kStagesWS + 5) + 16 + 127) & ~(size_t)127) + 4 * kEpiStage + 1024;
-    NEO_CUDA(cudaFuncSetAttribute(gemm_f16_ws_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    gemm_f16_ws_kernel<<<grid, kThreads, smem, s>>>(tmA, tmW, bias, C, M, K, ldc, relu);
-    NEO_LAUNCH_CHECK("gemm_f16_ws_kernel");
-    return NEO_OK;
-}
-
-static int launch_pair(const __half* A, long long lda, const __half* W, long long ldw, const float* bias, __half* C, long long ldc, long long M,
-                       int N, int K, int relu, int n_sm, cudaStream_t s) {
-    alignas(64) CUtensorMap tmA, tmW;
-    int rc;
-    if ((rc = make_tmap_2d(&tmA, A, M, K, lda, BM))) return rc;
-    if ((rc = make_tmap_2d(&tmW, W, N, K, ldw, BN2 / 2))) return rc;
-    const long long tiles = ((M + 2 * BM - 1) / (2 * BM)) * (N / BN2);
-    const long long pairs = n_sm / 2;
-    const int grid = 2 * (int)(tiles < pairs ? tiles : pairs);
-    const size_t smem = (((size_t)kStages2 * (BM * BK * 2 + (BN2 / 2) * BK * 2) + 8 * (2 * kStages2 + 4) + 16 + 127) & ~(size_t)127) + 4 * kEpiStage + 1024;
-    NEO_CUDA(cudaFuncSetAttribute(gemm_f16_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    gemm_f16_pair_kernel<<<grid, kThreads, smem, s>>>(tmA, tmW, bias, C, M, N, K, ldc, relu);
-    NEO_LAUNCH_CHECK("gemm_f16_pair_kernel");
     return NEO_OK;
 }
 
@@ -550,27 +151,6 @@ int gemm_f16(const void* A, long long lda, const void* W, long long ldw, const f
     }
     const __half *a = (const __half*)A, *w = (const __half*)W;
     __half* c = (__half*)C;
-    if (N % 256 == 0) {
-        // CTA pairs (256 x 256 tiles) once there is a tile for every pair of SMs; NEO_GEMM_PAIR=0 keeps the single-CTA kernel (A/B runs)
-        static int use_pair = -1, use_ws = 1;
-        static int n_sm_of[64] = {0};              // per device: a process may drive several GPUs
-        if (use_pair < 0) {
-            const char* e = getenv("NEO_GEMM_PAIR");
-            const char* e2 = getenv("NEO_GEMM_WS");
-            use_ws = !(e2 && e2[0] == '0');
-            use_pair = !(e && e[0] == '0');
-        }
-        int dev = 0;
-        NEO_CUDA(cudaGetDevice(&dev));
-        if (dev < 0 || dev >= 64) { set_error("device index %d out of range", dev); return NEO_ERR_UNSUPPORTED; }
-        if (!n_sm_of[dev]) NEO_CUDA(cudaDeviceGetAttribute(&n_sm_of[dev], cudaDevAttrMultiProcessorCount, dev));
-        const int n_sm = n_sm_of[dev];
-        // 256-wide layer with a weight matrix that fits shared memory and at least one row tile per SM: weight-stationary kernel
-        if (use_ws && N == 256 && K <= 256 && (M + BM - 1) / BM >= n_sm) return launch_ws(a, lda, w, ldw, bias, c, ldc, M, K, relu, n_sm, s);
-        const long long tiles2 = ((M + 2 * BM - 1) / (2 * BM)) * (N / 256);
-        if (use_pair && tiles2 >= n_sm / 2) return launch_pair(a, lda, w, ldw, bias, c, ldc, M, N, K, relu, n_sm, s);
-        return launch<256>(a, lda, w, ldw, bias, c, ldc, M, N, K, relu, s);
-    }
     if (N % 128 == 0) return launch<128>(a, lda, w, ldw, bias, c, ldc, M, N, K, relu, s);
     return launch<64>(a, lda, w, ldw, bias, c, ldc, M, N, K, relu, s);
 }

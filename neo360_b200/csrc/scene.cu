@@ -291,4 +291,4 @@ extern "C" size_t neo_scene_bytes(const NeoScene* sc) { return sc ? sc->bytes : 
 
 namespace neo { const char* last_error(); }
 extern "C" const char* neo_last_error(void) { return neo::last_error(); }
-extern "C" const char* neo_version(void) { return "neo360_b200 0.1.0 sm_100a"; }
+extern "C" const char* neo_version(void) { return "neo360_b200 0.1.0 sm_90a"; }

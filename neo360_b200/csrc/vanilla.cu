@@ -386,7 +386,7 @@ extern "C" int neo_vanilla_render_fwd(const NeoVanilla* v, const NeoRays* rays, 
         }
         long long total = (long long)n * N;
         if (cfg->precision == NEO_PREC_TC) {
-            // NeRFMLP (models/vanilla_nerf/model.py:44-125) layer by layer on tcgen05 (csrc/gemm_tc.cu), fp16 activations; the skip concatenation
+            // NeRFMLP (models/vanilla_nerf/model.py:44-125) layer by layer on the tensor cores (csrc/gemm_tc.cu), fp16 activations; the skip concatenation
             // by keeping h4 and the encoding in ONE buffer (layer 5 is a single K = 320 GEMM)
             const NeoVanilla::Mlp& m = v->mlp[lvl];
             __half* buf[2] = {(__half*)w.A16[0], (__half*)w.A16[1]};

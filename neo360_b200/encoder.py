@@ -9,7 +9,7 @@
     encoder_tp_fusion_conv.py:472-597    GridEncoder.forward       forward(): ResNet features and the three floor-plan conv stacks stay in the
                                                                    host framework; everything between them -- 64^3 x NV grid lookup,
                                                                    DepthPillarEncoder, three pillar aggregators, softmax-weighted pillar sums
-                                                                   (2.7 TFLOP per scene) -- runs in hand-written CUDA on tcgen05
+                                                                   (2.7 TFLOP per scene) -- runs in hand-written CUDA on the tensor cores
                                                                    (`neo_grid_encoder_dense`, csrc/encoder.cu + csrc/gemm_tc.cu) when no
                                                                    gradient is required; under autograd the same algebra runs as framework ops.
 """
@@ -142,7 +142,7 @@ class GridEncoder(nn.Module):
         fp = lambda t: t.permute(0, 3, 1, 2)
         return fp((lat * w_xz).sum(2)), fp((lat * w_xy).sum(3)), fp((lat * w_yz).sum(1))      # xz, xy, yz: (NV, 512, 64, 64)
 
-    # ---- the dense part, hand-written CUDA (tcgen05) ----
+    # ---- the dense part, hand-written CUDA (wgmma) ----
     def dense_cuda(self, latent, poses, focal, c, W, H):
         if not latent.is_cuda:
             raise RuntimeError("neo360_b200 needs CUDA tensors (no CPU fallback)")

@@ -65,7 +65,7 @@ class MipNeRF360(nn.Module):
     def __init__(self, num_prop_samples: int = 64, num_nerf_samples: int = 32, num_levels: int = 3, precision: str = "fp32",
                  **reference_defaults):
         super().__init__()
-        self.precision = precision          # "fp32": CUDA-core SGEMM chain (tight parity); "tc": every dense layer on tcgen05 (fp16 operands)
+        self.precision = precision          # "fp32": CUDA-core SGEMM chain (tight parity); "tc": every dense layer on the tensor cores (fp16 operands)
         if num_levels != 3 or reference_defaults:
             raise NotImplementedError("reference defaults only (models/mipnerf360/model.py:199-223)")
         self.num_prop_samples, self.num_nerf_samples = num_prop_samples, num_nerf_samples

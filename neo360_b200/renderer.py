@@ -10,7 +10,7 @@
 (model.py:525-527 / 577-579).  The encoder (GridEncoder, out of scope: SURVEY.md section 8(f1)) is hoisted out of the
 chunk loop (quirk Q5): call `set_scene(...)` once per scene with its outputs, or pass them in the `rays` dict under
 `planes_xz|planes_xy|planes_yz|latent`; or hand an `encoder` module to the constructor and it is run once per new set
-of `src_*` tensors.  All arithmetic runs in libneo360_b200.so (hand-written CUDA, sm_100a); there is no CPU fallback.
+of `src_*` tensors.  All arithmetic runs in libneo360_b200.so (hand-written CUDA, sm_90a); there is no CPU fallback.
 """
 from __future__ import annotations
 
@@ -192,7 +192,7 @@ class NeRF_TP(nn.Module):
             raise RuntimeError("no scene: call set_scene(...) or pass planes_*/latent in `rays`, or give an encoder")
         need = 1 << PRECISIONS[self.precision]
         if self._param_key != self._params_version() or not (self._scene.mask & need):
-            # the packed weights (fp32 transposes, TMEM image, W0/W3-projected feature maps) are stale, or the scene was last built for
+            # the packed weights (fp32 transposes, swizzled weight images, W0/W3-projected feature maps) are stale, or the scene was last built for
             # another use (a training step leaves a cameras-only scene): re-pack from the kept inputs
             src = self._scene_src
             a = self._scene_inputs

@@ -3,7 +3,7 @@
 `NeRF.forward(rays, randomized, white_bkgd, near, far)` returns the reference's `list[2]` of `(comp_rgb, acc, depth)`
 (model.py:214).  Parameter names and shapes equal the reference's (`coarse_mlp.pts_linears.0.weight`, ...), so its checkpoints
 load.  Arithmetic (csrc/vanilla.cu): `self.precision = "fp32"` (default) runs the layers on fp32 CUDA cores in the reference
-formulation; `"tc"` runs them as fp16 tcgen05 GEMMs with fp32 accumulation (csrc/gemm_tc.cu).  CUDA only, no CPU fallback."""
+formulation; `"tc"` runs them as fp16 wgmma GEMMs with fp32 accumulation (csrc/gemm_tc.cu).  CUDA only, no CPU fallback."""
 from __future__ import annotations
 
 import ctypes as C

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 @pytest.fixture(scope="session")

@@ -28,7 +28,7 @@ def test_header_symbols_all_exported(lib):
 
 
 def test_version_and_error_string(lib):
-    assert b"sm_100a" in lib.neo_version()
+    assert b"sm_90a" in lib.neo_version()
     assert isinstance(lib.neo_last_error(), bytes)
 
 

@@ -1,6 +1,6 @@
 """Tri-plane builder (SURVEY.md 8(f1)): neo360_b200.encoder.GridEncoder against vectors minted from the UNMODIFIED reference module
 (oracle/make_golden_encoder.py: state dicts bit-identical under the same seed, outputs bit-identical on CPU), and the hand-written
-CUDA dense part (tcgen05) against the module's own fp32 framework-op form."""
+CUDA dense part (wgmma) against the module's own fp32 framework-op form."""
 import os
 
 import numpy as np
@@ -40,7 +40,7 @@ def test_grid_encoder_framework_form_matches_reference_vectors():
 
 @pytest.mark.gpu
 def test_grid_encoder_cuda_dense_part(tmp_path):
-    """GPU: `neo_grid_encoder_dense` (gather + DepthPillarEncoder + pillar aggregators on tcgen05, fp16 operands) against the fp32
+    """GPU: `neo_grid_encoder_dense` (gather + DepthPillarEncoder + pillar aggregators on the tensor cores, fp16 operands) against the fp32
     framework-op form of the same module and weights; then the whole forward against the reference planes.
     Stated: pillar sums within 2e-2 of their scale (fp16 weights / activations through 4 dense layers + softmax); planes within 3e-2 of scale."""
     assert torch.cuda.is_available()

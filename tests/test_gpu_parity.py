@@ -1,5 +1,5 @@
 """GPU parity: the CUDA path (through the C ABI) against the oracle on the same seeded inputs and against the golden
-vectors minted from the unmodified reference.  Tolerances are stated per test.  Run with `-m gpu` on a B200."""
+vectors minted from the unmodified reference.  Tolerances are stated per test.  Run with `-m gpu` on an H100."""
 import numpy as np
 import pytest
 import torch
@@ -295,71 +295,6 @@ def test_chunked_frame_matches_oracle_chunk_loop(cuda):
 
 # ---------------- tensor-core path (NEO_PREC_TC) ----------------
 
-def test_tc_primitives_selftest(cuda):
-    """TS-mode tcgen05.mma (A in TMEM), SW128 K-major operand tiles, SS-mode MMA, TMEM loads -- against torch matmul
-    on the fp16-rounded operands (exact products, fp32 accumulation: tolerance 1e-3 on O(10) sums)."""
-    from neo360_b200 import _lib as L
-    lib = L.load()
-    g = torch.Generator().manual_seed(0)
-    X = torch.randn(128, 128, generator=g).to(cuda)
-    W = torch.randn(128, 128, generator=g).to(cuda)
-    Wn = torch.randn(80, 128, generator=g).to(cuda)
-    o1 = torch.zeros(128, 128, device=cuda)
-    o2 = torch.zeros(128, 80, device=cuda)
-    o3 = torch.zeros(128, 128, device=cuda)
-    o4 = torch.zeros(128, 80, device=cuda)
-    L.check(lib.neo_tc_selftest(L.ptr(X), L.ptr(W), L.ptr(Wn), L.ptr(o1), L.ptr(o2), L.ptr(o3), L.ptr(o4), torch.cuda.current_stream().cuda_stream))
-    torch.cuda.synchronize()
-    Xh, Wh, Wnh = X.half().float(), W.half().float(), Wn.half().float()
-    assert md(o1, Wh @ Xh.T) < 1e-3
-    assert md(o2, Xh @ Wnh.T) < 1e-3
-    print("MN-major B max err", md(o3, Wh @ Xh.T), " MN-major A max err", md(o4, Xh @ Wnh.T))
-    assert md(o3, Wh @ Xh.T) < 1e-3          # MN-major (point-contiguous) B operand, N=32 blocks at 64-byte offsets
-    assert md(o4, Xh @ Wnh.T) < 1e-3          # MN-major A operand, M=128 as two 64-point groups
-
-
-def test_tc_selftest_transpose(cuda):
-    """Transpose-accumulate MMA (identity A operand in a no-swizzle K-major tile, gathered features as the SW128 K-major B
-    operand): exact transposition of the fp16-rounded input.  `outa` is the descriptor reading the kernel uses."""
-    from neo360_b200 import _lib as L
-    lib = L.load()
-    g = torch.Generator().manual_seed(1)
-    X = torch.randn(128, 128, generator=g).to(cuda)
-    oa = torch.zeros(128, 128, device=cuda)
-    ob = torch.zeros(128, 128, device=cuda)
-    L.check(lib.neo_tc_selftest_transpose(L.ptr(X), L.ptr(oa), L.ptr(ob), torch.cuda.current_stream().cuda_stream))
-    torch.cuda.synchronize()
-    ref = X.half().float().T
-    print("transpose MMA: (LBO=K stride, SBO=row-group stride) err", md(oa, ref), " swapped err", md(ob, ref))
-    assert md(oa, ref) == 0.0
-
-
-def test_tc_selftest_window(cuda):
-    """Texel-window MMA (the bilinear lookups of the TC field kernel): one TMA box load of a 4x4x256-channel window (128B swizzle,
-    zero fill outside the map) as the MN-major A operand, a sparse [64 points x 16 texels] no-swizzle K-major tap-weight tile as B.
-    Exact in fp16 products / fp32 accumulation, including windows that straddle or miss the map."""
-    from neo360_b200 import _lib as L
-    lib = L.load()
-    g = torch.Generator().manual_seed(2)
-    H, W = 6, 7
-    tex = torch.randn(H * W, 256, generator=g)
-    for ox, oy in ((1, 1), (-1, -2), (5, 4), (3, 2), (-4, 0), (0, 6)):
-        wt = torch.rand(64, 16, generator=g) * (torch.rand(64, 16, generator=g) < 0.3)
-        o0 = torch.zeros(128, 64, device=cuda)
-        o3 = torch.zeros(128, 64, device=cuda)
-        L.check(lib.neo_tc_selftest_window(L.ptr(tex.to(cuda)), H, W, ox, oy, L.ptr(wt.to(cuda)), L.ptr(o0), L.ptr(o3),
-                                           torch.cuda.current_stream().cuda_stream))
-        torch.cuda.synchronize()
-        win = torch.zeros(16, 256)
-        for k in range(16):
-            y, x = oy + k // 4, ox + k % 4
-            if 0 <= y < H and 0 <= x < W:
-                win[k] = tex[y * W + x]
-        ref = (wt.half().double() @ win.half().double()).T.float()          # (256, 64)
-        print("window MMA at", (ox, oy), "err", md(o0, ref[:128]), md(o3, ref[128:]))
-        assert md(o0, ref[:128]) < 1e-5 and md(o3, ref[128:]) < 1e-5
-
-
 def test_field_eval_tc_vs_oracle(cuda):
     """TC field (fp16 operands, pre-projected features, folded head) against the oracle on identical t-values.
     Stated tolerance: |rgb| 2e-2, sigma 2e-2 + 2% (fp16 operand rounding through a 6-layer gained MLP)."""
@@ -431,7 +366,7 @@ def test_vanilla_nerf_vs_reference_vectors(cuda, tag):
 
 @pytest.mark.parametrize("tag", ["v_tiny", "v_cfg1"])
 def test_vanilla_nerf_tc_vs_reference_vectors(cuda, tag):
-    """Vanilla NeRF with the 8 x 256 MLP layer by layer on tcgen05 (NEO_PREC_TC, fp16 weights / activations) against outputs of the
+    """Vanilla NeRF with the 8 x 256 MLP layer by layer on the tensor cores (NEO_PREC_TC, fp16 weights / activations) against outputs of the
     UNMODIFIED reference module (v_cfg1 = BASELINE configs[0]).  Stated: L-inf <= 3e-2 on rgb / acc, PSNR >= 40 dB; coarse sample
     positions bit-exact."""
     import os
@@ -510,7 +445,7 @@ def test_mip360_vs_reference_vectors(cuda, tag):
 
 @pytest.mark.parametrize("tag", ["m_tiny", "m_small"])
 def test_mip360_tc_vs_reference_vectors(cuda, tag):
-    """Mip-NeRF 360 with every dense layer on tcgen05 (NEO_PREC_TC: fp16 weights / activations, fp32 accumulate, csrc/gemm_tc.cu) against
+    """Mip-NeRF 360 with every dense layer on the tensor cores (NEO_PREC_TC: fp16 weights / activations, fp32 accumulate, csrc/gemm_tc.cu) against
     outputs of the UNMODIFIED reference module.  Stated: level-0 sample positions exact (no MLP upstream); renderings L-inf <= 3e-2 and
     PSNR >= 35 dB per level; fp32 CUDA path of the same weights within the same bound (it is itself within 2e-4 of the reference)."""
     import os
@@ -719,7 +654,7 @@ def test_output_side_psnr_and_frames(cuda, tmp_path):
 @pytest.mark.parametrize("M,N,K,relu", [(1000, 1024, 512, 1), (257, 256, 1536, 1), (4096, 128, 320, 1), (130, 64, 64, 0), (70000, 1024, 1024, 1),
                                           (20001, 256, 128, 0), (19000, 512, 1536, 1), (40000, 256, 256, 1), (19000, 256, 64, 1)])
 def test_tc_dense_vs_torch(cuda, M, N, K, relu):
-    """The tensor-core dense layer of the wide MLPs (csrc/gemm_tc.cu: TMA tile loads + tcgen05, fp16 operands, fp32 accumulate) against a
+    """The tensor-core dense layer of the wide MLPs (csrc/gemm_tc.cu: TMA tile loads + wgmma, fp16 operands, fp32 accumulate) against a
     plain PyTorch fp32 reference of the same op on the fp16-rounded operands; ragged M, every N tile width (64/128/256), K up to 1536; 
     (70000,1024,1024) and (19000,512,1536) have a 256 x 256 tile for every SM pair and run the cta_group::2 kernel (gemm_f16_pair_kernel);
     the N = 256, K <= 256 shapes with a row tile for every SM run the weight-stationary kernel (gemm_f16_ws_kernel).
