@@ -312,6 +312,12 @@ int neo_profile_read(float* field_ms, int* n_field, unsigned long long* launches
  * register accumulators): A (M,K), W (N,K) fp32 device, bias (N) or NULL -> out (M,N) fp32 = act(fp16(A) . fp16(W)^T + bias)
  * rounded to fp16.  K % 64 == 0, N % 64 == 0.  Synchronises the stream (allocates its fp16 staging buffers). */
 int neo_tc_dense(const float* A, const float* W, const float* bias, long long M, int N, int K, int relu, float* out, void* stream);
+/* The same kernel on caller-owned fp16 operands with explicit row strides (in elements), as the library's own callers use it:
+ * C (M,N; row stride ldc) = act(A (M,K; lda) . W (N,K; ldw)^T + bias) rounded to fp16; A, W, C fp16 device, bias (N) fp32 or NULL.
+ * K % 64 == 0, N % 64 == 0, strides % 8 == 0, lda, ldw >= K, ldc >= N, 16-byte aligned pointers.  Writes only columns [0, N) of
+ * rows [0, M) of C, so A may sit in other columns of C's own rows.  Asynchronous on `stream`. */
+int neo_tc_gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M,
+                    int N, int K, int relu, void* stream);
 /* Host-side view of the TC kernel's encoding-column layout (csrc/field_tc.cu enc_col<>): for in_ch = 3|4 and operand column
  * `col` in [0, KE = 64|96) returns the reference's positional-encoding index (helper.py:121-125 order) in [0, 21*in_ch),
  * -1 for the constant-one (bias) column, -2 for a zero padding column, -3 for invalid arguments.  Pure host code (no GPU). */

@@ -123,6 +123,8 @@ SYMBOLS = {
     "neo_profile": (C.c_int, [C.c_int]),
     "neo_profile_read": (C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_int), C.POINTER(C.c_ulonglong), C.POINTER(C.c_double)]),
     "neo_tc_dense": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "neo_tc_gemm_f16": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong, C.c_longlong,
+                                  C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "neo_tc_enc_column": (C.c_int, [C.c_int, C.c_int]),
     "neo_tc_trap_info": (C.c_char_p, []),
     "neo_last_error": (C.c_char_p, []),

@@ -141,14 +141,18 @@ static int launch(const __half* A, long long lda, const __half* W, long long ldw
 }  // namespace gemm
 
 // C (M x N, row stride ldc) = act(A (M x K, row stride lda) . W (N x K, row stride ldw)^T + bias); fp16 in / out, fp32 accumulate.
-// K % 64 == 0, N % 64 == 0, 16-byte aligned rows.
+// K % 64 == 0, N % 64 == 0, 16-byte aligned rows.  Only columns [0, N) of rows [0, M) of C are written, so A may live in other
+// columns of C's own rows (the Mip-NeRF 360 and vanilla NeRF activation buffers keep [h | features] side by side).
 int gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M, int N, int K,
              int relu, cudaStream_t s) {
     using namespace gemm;
-    if (M <= 0 || N <= 0 || K <= 0 || (K % BK) || (N % 64) || (lda % 8) || (ldw % 8) || (ldc % 8)) {
-        set_error("gemm_f16: need M,N,K > 0, K %% 64 == 0, N %% 64 == 0 and row strides %% 8 == 0 (got M=%lld N=%d K=%d lda=%lld ldw=%lld ldc=%lld)", M, N, K, lda, ldw, ldc);
+    if (!A || !W || !C) { set_error("gemm_f16: null operand"); return NEO_ERR_INVALID; }
+    if (M <= 0 || N <= 0 || K <= 0 || (K % BK) || (N % 64) || (lda % 8) || (ldw % 8) || (ldc % 8) || lda < K || ldw < K || ldc < N) {
+        set_error("gemm_f16: need M,N,K > 0, K %% 64 == 0, N %% 64 == 0, row strides %% 8 == 0, lda, ldw >= K and ldc >= N "
+                  "(got M=%lld N=%d K=%d lda=%lld ldw=%lld ldc=%lld)", M, N, K, lda, ldw, ldc);
         return NEO_ERR_INVALID;
     }
+    if (((uintptr_t)A | (uintptr_t)W | (uintptr_t)C) & 15u) { set_error("gemm_f16: operands must be 16-byte aligned"); return NEO_ERR_INVALID; }
     const __half *a = (const __half*)A, *w = (const __half*)W;
     __half* c = (__half*)C;
     if (N % 128 == 0) return launch<128>(a, lda, w, ldw, bias, c, ldc, M, N, K, relu, s);
@@ -194,4 +198,10 @@ extern "C" int neo_tc_dense(const float* A, const float* W, const float* bias, l
     }
     cudaFree(a); cudaFree(w); cudaFree(c);
     return rc;
+}
+
+// Stage-level entry point of gemm_f16 itself, at the strides and aliasing its callers use: fp16 device operands, asynchronous on `stream`.
+extern "C" int neo_tc_gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M,
+                               int N, int K, int relu, void* stream) {
+    return neo::gemm_f16(A, lda, W, ldw, bias, C, ldc, M, N, K, relu, (cudaStream_t)stream);
 }

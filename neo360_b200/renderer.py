@@ -324,8 +324,10 @@ class NeRF_TP(nn.Module):
                                              torch.cuda.current_stream().cuda_stream))
         return out
 
-    def field_eval(self, rays, far, t_vals, mlp_index: int, chunk: int = 0, precision: Optional[str] = None):
-        """`predict` (model.py:343-407) of one branch: t/s (n,N) -> rgb (n,N,3), sigma (n,N,1)."""
+    def field_eval(self, rays, far, t_vals, mlp_index: int, chunk: int = 0, precision: Optional[str] = None,
+                   ray_order: Optional[torch.Tensor] = None):
+        """`predict` (model.py:343-407) of one branch: t/s (n,N) -> rgb (n,N,3), sigma (n,N,1).  `ray_order` (n) int32, a permutation
+        of the rays, only changes the order in which the TC kernel visits them (NeoRays.ray_order); rows stay indexed by ray."""
         o, d, vd = (rays[k].contiguous().float() for k in ("rays_o", "rays_d", "viewdirs"))
         t = t_vals.contiguous().float()
         fr = far.reshape(-1).contiguous().float()
@@ -333,6 +335,11 @@ class NeRF_TP(nn.Module):
         r = L.NeoRays()
         r.n_rays, r.chunk = n, int(chunk)
         r.rays_o, r.rays_d, r.viewdirs = L.ptr(o), L.ptr(d), L.ptr(vd)
+        if ray_order is not None:
+            if ray_order.dtype != torch.int32 or ray_order.numel() != n or ray_order.device != t.device:
+                raise ValueError("ray_order must be an int32 permutation of the rays on their device")
+            ray_order = ray_order.contiguous()
+            r.ray_order = ray_order.data_ptr()
         rgb = torch.empty(n, N, 3, device=t.device)
         sig = torch.empty(n, N, 1, device=t.device)
         with torch.cuda.device(t.device):

@@ -44,10 +44,24 @@ def test_argument_validation_without_gpu(lib):
     assert lib.neo_field_eval(None, None, None, None, 8, 0, 0, None, None, None) == -1
 
 
+def test_gemm_f16_argument_validation_without_gpu(lib):
+    """neo_tc_gemm_f16 rejects, before touching the GPU, what the dense-layer kernel cannot do (the pointers are never dereferenced)."""
+    p = 1 << 20
+    assert lib.neo_tc_gemm_f16(p, 64, p, 64, None, p, 64, 8, 64, 48, 0, None) == -1        # K % 64
+    assert lib.neo_tc_gemm_f16(p, 64, p, 64, None, p, 96, 8, 96, 64, 0, None) == -1        # N % 64
+    assert lib.neo_tc_gemm_f16(p, 32, p, 64, None, p, 64, 8, 64, 64, 0, None) == -1        # lda < K
+    assert lib.neo_tc_gemm_f16(p, 64, p, 40, None, p, 64, 8, 64, 64, 0, None) == -1        # ldw < K (and % 8)
+    assert lib.neo_tc_gemm_f16(p, 64, p, 64, None, p, 32, 8, 64, 64, 0, None) == -1        # ldc < N
+    assert lib.neo_tc_gemm_f16(p, 64, p, 64, None, p, 64, 0, 64, 64, 0, None) == -1        # M = 0
+    assert lib.neo_tc_gemm_f16(p + 2, 64, p, 64, None, p, 64, 8, 64, 64, 0, None) == -1    # A not 16-byte aligned
+    assert lib.neo_tc_gemm_f16(None, 64, p, 64, None, p, 64, 8, 64, 64, 0, None) == -1
+    assert b"gemm_f16" in lib.neo_last_error()
+
+
 @pytest.mark.parametrize("in_ch,ke", [(3, 64), (4, 96)])
 def test_tc_encoding_column_layout_is_a_permutation(lib, in_ch, ke):
-    """The TC kernel orders the positional-encoding columns per coordinate (x, sin 2^k x, cos 2^k x) so that the double-angle
-    recurrence applies; the weight image is permuted with the same table.  It must cover every reference column
+    """The TC kernel orders the positional-encoding columns per coordinate (x, sin 2^k x, cos 2^k x); the weight image is permuted
+    with the same table.  It must cover every reference column
     (helper.py:121-125 order) exactly once, carry exactly one constant-one (bias) column and only zero padding otherwise."""
     cols = [lib.neo_tc_enc_column(in_ch, c) for c in range(ke)]
     ref = sorted(c for c in cols if c >= 0)

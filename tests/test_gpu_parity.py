@@ -391,10 +391,10 @@ def test_vanilla_nerf_tc_vs_reference_vectors(cuda, tag):
 
 
 def test_tc_blocked_frame_order_is_pure_scheduling(cuda):
-    """NEO_PREC_TC with NeoRays.ray_order (8x4 pixel blocks) against the identity order.  The ray order decides which 64 points
-    share a job and therefore how a point's texel windows are grouped, i.e. the order of its fp32 accumulation on the tensor pipe:
-    the pixels agree to accumulation rounding (stated: 1e-3 on rgb in [0,1] / depth), not bit for bit.  (Line 243 keeps the
-    bit-exact check for the fp32 CUDA-core path.)"""
+    """NEO_PREC_TC with NeoRays.ray_order (8x4 pixel blocks) against the identity order: bit-identical.  The ray order only decides
+    which tile and row of the field kernel a point lands in; its blend is a per-thread fp32 loop in a fixed order and a wgmma row
+    does not depend on the other rows, so nothing about a point's arithmetic changes (test_gpu_tc_kernels.py checks the same per
+    point with random orders and sub-batches)."""
     W, H, nc, nf = 48, 36, 24, 12
     net, osc, P = make_net(cuda, (W, H), (24, 32), nc, nf, 2, precisions=("tc",), precision="tc")
     pose = synth.target_pose(11, 100)
@@ -405,7 +405,7 @@ def test_tc_blocked_frame_order_is_pure_scheduling(cuda):
         b = net.render_rays_test(rays, chunk=512, img_wh=(W, H))
     net.check()
     for k in ("rgb", "fg_rgb", "bg_rgb", "depth"):
-        assert md(a[k], b[k]) < 1e-3, k
+        assert md(a[k], b[k]) == 0, (k, md(a[k], b[k]))
 
 
 # ---------------- Mip-NeRF 360 (row a18) ----------------
@@ -556,10 +556,10 @@ def test_tc_randomized_and_train_tuple(cuda, golden):
 def test_full_size_frame_properties(cuda):
     """Whole-frame companion of test_headline_config_vs_oracle (which compares whole chunks of this frame with the oracle): at the
     benchmark's full size the oracle takes ~1 h per frame, so the rest of the frame is covered by size-independent properties:
-    (1) idempotence: two renders of the same frame are bit-identical (no race in the persistent tensor-core kernel; texel windows
-        are accumulated in a fixed order);
-    (2) the 8x4-pixel-block schedule is pure scheduling: a 16 384-ray prefix rendered in row-major order agrees up to the fp32
-        accumulation order of each point's texel windows (stated: 1e-3);
+    (1) idempotence: two renders of the same frame are bit-identical (no race in the persistent tensor-core kernel; every point's
+        texels are blended in a fixed order);
+    (2) the 8x4-pixel-block schedule is pure scheduling: a 16 384-ray prefix rendered on its own in row-major order is
+        bit-identical to the same rays of the blocked whole-frame render (a point's result does not depend on its tile or row);
     (3) the tensor-core path agrees with the reference-formulation fp32 CUDA path (itself within 2e-4 of the reference vectors
         at the small sizes) on those rays: L-inf <= 3e-2 on rgb and acc, PSNR >= 40 dB;
     (4) range / compositing invariants: rgb in [-1e-3, 1+1e-3]-ish after compositing, 0 <= acc <= 1 + 1e-5, depth >= 0."""
@@ -586,7 +586,7 @@ def test_full_size_frame_properties(cuda):
     net.check()
     for k in ("rgb", "fg_rgb", "bg_rgb", "depth", "fg_acc"):
         assert md(a[k], b[k]) == 0, ("not idempotent", k)
-        assert md(a[k][:n], c[k]) < 1e-3, ("block order changed the result", k)
+        assert md(a[k][:n], c[k]) == 0, ("block order changed the result", k, md(a[k][:n], c[k]))
     assert a["rgb"].shape == (W * H, 3) and torch.isfinite(a["rgb"]).all() and torch.isfinite(a["depth"]).all()
     assert float(a["rgb"].min()) >= -2e-3 and float(a["rgb"].max()) <= 1.0 + 2e-3
     assert float(a["fg_acc"].min()) >= 0.0 and float(a["fg_acc"].max()) <= 1.0 + 1e-5
@@ -654,11 +654,10 @@ def test_output_side_psnr_and_frames(cuda, tmp_path):
 @pytest.mark.parametrize("M,N,K,relu", [(1000, 1024, 512, 1), (257, 256, 1536, 1), (4096, 128, 320, 1), (130, 64, 64, 0), (70000, 1024, 1024, 1),
                                           (20001, 256, 128, 0), (19000, 512, 1536, 1), (40000, 256, 256, 1), (19000, 256, 64, 1)])
 def test_tc_dense_vs_torch(cuda, M, N, K, relu):
-    """The tensor-core dense layer of the wide MLPs (csrc/gemm_tc.cu: TMA tile loads + wgmma, fp16 operands, fp32 accumulate) against a
-    plain PyTorch fp32 reference of the same op on the fp16-rounded operands; ragged M, every N tile width (64/128/256), K up to 1536; 
-    (70000,1024,1024) and (19000,512,1536) have a 256 x 256 tile for every SM pair and run the cta_group::2 kernel (gemm_f16_pair_kernel);
-    the N = 256, K <= 256 shapes with a row tile for every SM run the weight-stationary kernel (gemm_f16_ws_kernel).
-    Stated: |err| <= 2e-3 * max|ref| (fp32 accumulation order + the fp16 rounding of the output)."""
+    """The fp32 wrapper neo_tc_dense (fp32 -> fp16 staging, gemm_f16, fp16 -> fp32) against a plain PyTorch fp32 reference of the same
+    op on the fp16-rounded operands, ragged M, N = 64 (BN = 64 tiles) and multiples of 128, K up to 1536.  Stated: |err| <= 2e-3 *
+    max|ref| (fp32 accumulation order + the fp16 rounding of the output).  gemm_f16 itself is held to an element-wise bound at its
+    callers' strides and aliasing in test_gpu_tc_kernels.py."""
     from neo360_b200 import _lib as L
     lib = L.load()
     g = torch.Generator().manual_seed(M + N + K)
