@@ -318,6 +318,11 @@ int neo_tc_dense(const float* A, const float* W, const float* bias, long long M,
  * rows [0, M) of C, so A may sit in other columns of C's own rows.  Asynchronous on `stream`. */
 int neo_tc_gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M,
                     int N, int K, int relu, void* stream);
+/* Stage-level entry point of the tiny-N head used by the vanilla NeRF, Mip-NeRF 360 and encoder tensor-core paths (csrc/mip.cu
+ * rowdot_f16): out (M,N) fp32 = H (M,K; row stride ld) fp16 . W (N,K)^T fp32 + b (N) fp32, fp32 accumulation.  N in {1, 3},
+ * K % 8 == 0, ld % 8 == 0, K <= ld, N*K*4 <= 48 KB, H 16-byte aligned, no NULL pointer; M <= 0 does nothing.  Writes only rows
+ * [0, M) of out.  Asynchronous on `stream`. */
+int neo_tc_rowdot_f16(const void* H, long long ld, int K, const float* W, const float* b, int N, long long M, float* out, void* stream);
 /* Host-side view of the TC kernel's encoding-column layout (csrc/field_tc.cu enc_col<>): for in_ch = 3|4 and operand column
  * `col` in [0, KE = 64|96) returns the reference's positional-encoding index (helper.py:121-125 order) in [0, 21*in_ch),
  * -1 for the constant-one (bias) column, -2 for a zero padding column, -3 for invalid arguments.  Pure host code (no GPU). */

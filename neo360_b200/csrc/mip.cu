@@ -220,8 +220,9 @@ __global__ void features_kernel(const float* __restrict__ rays_o, const float* _
 
 // tensor-core path: fp16 rows of the activation buffer (row stride ld16 halfs, 504 features + 8 zero columns = 1 KB per sample).
 // Thread = (sample, basis direction): 12 samples x 21 directions per block, no idle lanes.  The per-sample Gaussian is computed once
-// into shared memory; sin / cos of the 12 octaves come from three accurate sincosf calls (octaves 0, 4, 8) and exact angle doubling in
-// between (error <= 8 ulp, below the fp32 rounding of the reference's own `x + pi/2` argument at those magnitudes and far below fp16);
+// into shared memory; sin / cos of the 12 octaves come from three accurate sincosf calls (octaves 0, 4, 8) and angle doubling in
+// between.  Against float64 features rounded to fp16 (oracle/tc_paths_model.py), the field's per-point error stays fp16 rounding noise:
+// tests/test_gpu_tc_paths.py measured up to 3.3e-4 in rgb and 5.3e-4 in density (pre-activation units) per point on an H100;
 // the row is assembled in shared memory and leaves as 16-byte coalesced stores (the 2-byte scattered stores of the warp-per-sample
 // kernel were the bottleneck: r2 launch list, 15.9 % of the Mip-NeRF 360 frame).
 constexpr int kFeatSamples = 12, kFeatThreads = kFeatSamples * kBasis;     // 252
@@ -463,6 +464,8 @@ __global__ void __launch_bounds__(256) rowdot_f16_kernel(const __half* __restric
 int launch_rowdot_f16(const void* H, long long ld, int K, const float* W, const float* b, int N, long long M, float* out, cudaStream_t s) {
     if (M <= 0) return NEO_OK;
     if ((K % 8) || (ld % 8) || (N != 1 && N != 3)) { set_error("rowdot_f16: K %% 8, ld %% 8 and N in {1, 3} required (K=%d ld=%lld N=%d)", K, ld, N); return NEO_ERR_INVALID; }
+    if (K <= 0 || ld < K || (size_t)N * K * sizeof(float) > 48 * 1024) { set_error("rowdot_f16: need 0 < K <= ld and N*K*4 <= 48 KB (K=%d ld=%lld N=%d)", K, ld, N); return NEO_ERR_INVALID; }
+    if (!H || !W || !b || !out || (reinterpret_cast<uintptr_t>(H) & 15)) { set_error("rowdot_f16: null pointer or H not 16-byte aligned"); return NEO_ERR_INVALID; }
     const unsigned grid = (unsigned)((M + 8 * 4 * mip::kRowdotIters - 1) / (8 * 4 * mip::kRowdotIters));
     const size_t smem = (size_t)N * K * sizeof(float);
     if (N == 1) mip::rowdot_f16_kernel<1><<<grid, 256, smem, s>>>((const __half*)H, ld, K, W, b, M, out);
@@ -578,6 +581,11 @@ int mlp_tc(const NeoMipMLPParams& p, const WSM& w, long long M, int n, const flo
     return NEO_OK;
 }
 }  // namespace
+
+// Stage-level entry point of rowdot_f16, the tiny-N head of the vanilla NeRF, Mip-NeRF 360 and encoder paths.
+extern "C" int neo_tc_rowdot_f16(const void* H, long long ld, int K, const float* W, const float* b, int N, long long M, float* out, void* stream) {
+    return neo::launch_rowdot_f16(H, ld, K, W, b, N, M, out, (cudaStream_t)stream);
+}
 
 extern "C" size_t neo_mip_workspace_bytes(int n_rays, const NeoMipCfg* cfg, int nerf_width) {
     if (n_rays <= 0 || check(cfg) || nerf_width < 64) return 0;

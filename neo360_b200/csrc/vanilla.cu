@@ -165,8 +165,10 @@ __global__ void __launch_bounds__(kThreads) field_kernel(NeoVanilla::Mlp m, cons
 }
 
 // ---- tensor-core path: positional encodings as fp16 rows (63 -> 64, 27 -> 64 zero padded), activations of the heads ----
-// One thread per sample row: the point and its 10 octaves (one sincosf per coordinate + exact angle doubling: error <= 2^9 ulp = 3e-5,
-// far below the fp16 the row is stored in), then the direction encoding of its ray (4 octaves).  Rows are 128 bytes; a lane owns a row,
+// One thread per sample row: the point and its 10 octaves (one sincosf per coordinate, then angle doubling, whose error grows with the
+// octave), then the direction encoding of its ray (4 octaves).  Against exact sin / cos of the fp32 point rounded to fp16
+// (oracle/tc_paths_model.py), the field's per-point error stays fp16 rounding noise: tests/test_gpu_tc_paths.py measured up to 1.5e-3 in
+// rgb and 4.3e-3 in sigma (pre-activation units) per point, 1.9e-4 / 3.4e-4 per case mean, on an H100.  Rows are 128 bytes; a lane owns a row,
 // so each row is assembled in a per-warp shared-memory tile ([32 rows][128 B], 16-byte pieces XOR-swizzled by row) and written out as
 // whole lines, 4 rows per store instruction (the one-thread-per-element version spent 15 % of the frame here).
 __device__ __forceinline__ void put_h(unsigned char* stage, int lane, int c, float v) {

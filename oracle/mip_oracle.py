@@ -45,12 +45,12 @@ def sample_intervals(t, w_logits, n, u_jitter: Optional[Tensor] = None, domain=(
     """helper.py:343-396 (single_jitter=True).  u_jitter (B,1) replaces torch.rand when randomized."""
     if u_jitter is None:
         pad = 1 / (2 * n)
-        u = torch.linspace(pad, 1 - pad - EPS, n)
+        u = torch.linspace(pad, 1 - pad - EPS, n, device=t.device)
         u = torch.broadcast_to(u, t.shape[:-1] + (n,))
     else:
         u_max = EPS + (1 - EPS) / n
         max_jitter = (1 - u_max) / (n - 1) - EPS
-        u = torch.linspace(0, 1 - u_max, n) + u_jitter * max_jitter
+        u = torch.linspace(0, 1 - u_max, n, device=t.device) + u_jitter * max_jitter
     u = u.type_as(t)
     w = F.softmax(w_logits, dim=-1)
     cw = torch.cumsum(w[..., :-1], -1).clip(max=1.0)
@@ -74,7 +74,7 @@ def cast_cone(tdist, o, d, radii):
     mean = d[..., None, :] * t_mean[..., None]
     dmag = torch.sum(d ** 2, -1, keepdim=True).clip(min=1e-10)
     d_outer = d[..., :, None] * d[..., None, :]
-    null_outer = torch.eye(3) - d[..., :, None] * (d / dmag)[..., None, :]
+    null_outer = torch.eye(3, dtype=d.dtype, device=d.device) - d[..., :, None] * (d / dmag)[..., None, :]
     cov = t_var[..., None, None] * d_outer[..., None, :, :] + r_var[..., None, None] * null_outer[..., None, :, :]
     return mean + o[..., None, :], cov
 
@@ -87,8 +87,9 @@ def contract(mean, cov):
     f = (2 * r - 1) / r2
     z = torch.where(inside, mean, f * mean)
     g = (2 - 2 * r) / (r2 * r2)
-    J = f[..., None] * torch.eye(3) + g[..., None] * mean[..., :, None] * mean[..., None, :]
-    J = torch.where(inside[..., None], torch.eye(3).expand_as(J), J)
+    eye = torch.eye(3, dtype=mean.dtype, device=mean.device)
+    J = f[..., None] * eye + g[..., None] * mean[..., :, None] * mean[..., None, :]
+    J = torch.where(inside[..., None], eye.expand_as(J), J)
     return z, J @ cov @ J.transpose(-1, -2)
 
 
@@ -96,14 +97,14 @@ def ipe_features(mean, cov, basis, min_deg=0, max_deg=12):
     """lift_and_diagonalize + integrated_pos_enc (helper.py:70-88): -> (..., 504)."""
     m = mean @ basis
     v = torch.sum(basis[None, None] * (cov @ basis), dim=-2)
-    scales = 2.0 ** torch.arange(min_deg, max_deg, dtype=mean.dtype)
+    scales = 2.0 ** torch.arange(min_deg, max_deg, dtype=mean.dtype, device=mean.device)
     sm = (m[..., None, :] * scales[:, None]).reshape(*m.shape[:-1], -1)
     sv = (v[..., None, :] * scales[:, None] ** 2).reshape(*v.shape[:-1], -1)
     return torch.exp(-0.5 * torch.cat([sv, sv], -1)) * torch.sin(torch.cat([sm, sm + 0.5 * math.pi], -1))
 
 
 def dir_enc(x, deg=4):
-    scales = 2.0 ** torch.arange(0, deg, dtype=x.dtype)
+    scales = 2.0 ** torch.arange(0, deg, dtype=x.dtype, device=x.device)
     xb = (x[..., None, :] * scales[:, None]).reshape(*x.shape[:-1], -1)
     return torch.cat([x, torch.sin(torch.cat([xb, xb + 0.5 * math.pi], -1))], -1)
 
@@ -118,7 +119,7 @@ def mlp(P: Dict[str, Tensor], pre: str, feats: Tensor, viewdirs: Tensor, depth: 
             x = torch.cat([x, feats], -1)
     density = F.softplus(lin("density_layer", x)[..., 0] - 1.0)
     if disable_rgb:
-        return density, torch.zeros(*feats.shape[:-1], 3)
+        return density, torch.zeros(*feats.shape[:-1], 3, dtype=feats.dtype, device=feats.device)
     beta = lin("bottleneck_layer", x)
     de = dir_enc(viewdirs)
     y = torch.relu(lin("views_linear.0", torch.cat([beta, torch.broadcast_to(de[..., None, :], beta.shape[:-1] + (de.shape[-1],))], -1)))

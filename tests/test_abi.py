@@ -58,6 +58,20 @@ def test_gemm_f16_argument_validation_without_gpu(lib):
     assert b"gemm_f16" in lib.neo_last_error()
 
 
+def test_rowdot_f16_argument_validation_without_gpu(lib):
+    """neo_tc_rowdot_f16 rejects, before touching the GPU, what the head kernel cannot do (the pointers are never dereferenced)."""
+    p = 1 << 20
+    assert lib.neo_tc_rowdot_f16(p, 256, 256, p, p, 2, 8, p, None) == -1        # N not in {1, 3}
+    assert lib.neo_tc_rowdot_f16(p, 256, 252, p, p, 1, 8, p, None) == -1        # K % 8
+    assert lib.neo_tc_rowdot_f16(p, 260, 256, p, p, 1, 8, p, None) == -1        # ld % 8
+    assert lib.neo_tc_rowdot_f16(p, 128, 256, p, p, 1, 8, p, None) == -1        # ld < K
+    assert lib.neo_tc_rowdot_f16(p, 8192, 8192, p, p, 3, 8, p, None) == -1      # weights exceed 48 KB of shared memory
+    assert lib.neo_tc_rowdot_f16(p + 2, 256, 256, p, p, 1, 8, p, None) == -1    # H not 16-byte aligned
+    assert lib.neo_tc_rowdot_f16(p, 256, 256, p, None, 1, 8, p, None) == -1     # NULL bias
+    assert b"rowdot_f16" in lib.neo_last_error()
+    assert lib.neo_tc_rowdot_f16(None, 256, 256, None, None, 1, 0, None, None) == 0   # M = 0: nothing to do
+
+
 @pytest.mark.parametrize("in_ch,ke", [(3, 64), (4, 96)])
 def test_tc_encoding_column_layout_is_a_permutation(lib, in_ch, ke):
     """The TC kernel orders the positional-encoding columns per coordinate (x, sin 2^k x, cos 2^k x); the weight image is permuted
