@@ -177,7 +177,8 @@ int neo_sample_pdf(const float* rays_o, const float* rays_d, const float* far, c
                    const float* weights, int n_rays, int n_old, int num_samples, int in_sphere,
                    float far_uncontracted, const float* u_rand, float* t_vals, float* pts, float* pts_linear,
                    void* stream);
-/* models/neo360/helper.py:128-171.  rgb (n,N,3), sigma (n,N), t (n,N). */
+/* models/neo360/helper.py:128-171.  rgb (n,N,3), sigma (n,N), t (n,N).  in_sphere 1 = fg (reads rays_d and far), 0 = bg (descending s),
+ * 2 = vanilla NeRF (reads rays_d); any other value, or a NULL input the branch reads, is NEO_ERR_INVALID.  Outputs may be NULL. */
 int neo_volumetric_rendering(const float* rgb, const float* sigma, const float* t_vals, const float* rays_d,
                              const float* far, int n_rays, int N, int white_bkgd, int in_sphere, float* comp_rgb,
                              float* acc, float* weights, float* bg_lambda, float* depth, void* stream);
@@ -187,7 +188,8 @@ int neo_volumetric_rendering(const float* rgb, const float* sigma, const float* 
  * planes may be NULL (then that output is skipped).  out_local / out_world: (nv*M, C), rows ordered (view, point). */
 int neo_index_maps(const NeoScene* scene, const float* pts, int M, int C, const float* latent_cl, const float* xz_cl, const float* xy_cl,
                    const float* yz_cl, float* out_local, float* out_world, void* stream);
-/* Backward of neo_index_maps: scatter-add of the row gradients (nv*M, C) into zero-initialised channel-last gradient maps. */
+/* Backward of neo_index_maps: scatter-add of the row gradients (nv*M, C) into zero-initialised channel-last gradient maps.  Row gradients
+ * and gradient maps must be 16-byte aligned (float4 reductions). */
 int neo_index_maps_bwd(const NeoScene* scene, const float* pts, int M, int C, const float* g_local, const float* g_world,
                        float* g_latent_cl, float* g_xz_cl, float* g_xy_cl, float* g_yz_cl, void* stream);
 /* encoder_tp_fusion_conv.py:122-209: pts (M,3) world -> (nv*M,128), rows ordered (view, point). */
@@ -203,12 +205,13 @@ int neo_clipped_sq_err(const float* pred, const float* gt, long long n, double* 
  * NeRFPPMLP are differentiated by the host framework (plain library GEMMs) in neo360_b200/training.py.  Sample positions carry no
  * gradient (the reference detaches them, helper.py:225). */
 /* d(volumetric_rendering)/d(rgb, sigma): upstream gradients of comp_rgb (n,3), acc (n), weights (n,N), bg_lambda (n), depth (n) -- any
- * may be NULL -- -> d_rgb (n,N,3), d_sigma (n,N).  Same rgb / sigma / t / rays_d / far as the forward call. */
+ * may be NULL -- -> d_rgb (n,N,3), d_sigma (n,N).  Same rgb / sigma / t / rays_d / far as the forward call; in_sphere 0 or 1. */
 int neo_volumetric_rendering_bwd(const float* rgb, const float* sigma, const float* t_vals, const float* rays_d, const float* far,
                                  int n_rays, int N, int white_bkgd, int in_sphere, const float* g_comp_rgb, const float* g_acc,
                                  const float* g_weights, const float* g_bg_lambda, const float* g_depth, float* d_rgb, float* d_sigma,
                                  void* stream);
-/* d(index_grid)/d(planes): g_out (nv*M,128) -> ACCUMULATES into channel-last gradient maps (nv, plane_h, plane_w, 128) x3 (zeroed by the caller). */
+/* d(index_grid)/d(planes): g_out (nv*M,128) -> ACCUMULATES into channel-last gradient maps (nv, plane_h, plane_w, 128) x3 (zeroed by the caller).
+ * g_out and the gradient maps of this and neo_index_local_bwd must be 16-byte aligned. */
 int neo_index_grid_bwd(const NeoScene* scene, const float* pts, int M, const float* g_out, float* g_planes_xz, float* g_planes_xy,
                        float* g_planes_yz, void* stream);
 /* d(get_local_feats)/d(latent): g_out (nv*M,512) -> ACCUMULATES into the channel-last gradient map (nv, lat_h, lat_w, 512). */

@@ -164,6 +164,10 @@ extern "C" int neo_check_async(const NeoScene* sc, void* stream) {
 }
 
 // ---- stage-level entry points ----
+namespace {
+// index_bwd_kernel reads its row gradients and reduces into the gradient maps as float4 (16-byte vector atomics)
+bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+}  // namespace
 extern "C" int neo_get_rays(int H, int W, float focal, const float* c2w, float* o, float* vd, float* rd, float* radii, void* stream) {
     if (H < 2 || W < 1 || !c2w) { set_error("neo_get_rays: bad arguments"); return NEO_ERR_INVALID; }
     return launch_get_rays(H, W, focal, c2w, o, vd, rd, radii, (cudaStream_t)stream);
@@ -198,6 +202,11 @@ extern "C" int neo_volumetric_rendering(const float* rgb, const float* sigma, co
                                         int N, int white, int in_sphere, float* comp, float* acc, float* w, float* lam, float* depth,
                                         void* stream) {
     if (n <= 0 || N < 1) { set_error("neo_volumetric_rendering: bad sizes"); return NEO_ERR_INVALID; }
+    if (in_sphere < 0 || in_sphere > 2) { set_error("neo_volumetric_rendering: in_sphere must be 0, 1 or 2 (got %d)", in_sphere); return NEO_ERR_INVALID; }
+    if (!rgb || !sigma || !t || (in_sphere && !d) || (in_sphere == 1 && !far)) {
+        set_error("neo_volumetric_rendering: null rgb / sigma / t, or rays_d (in_sphere 1, 2) / far (in_sphere 1)");
+        return NEO_ERR_INVALID;
+    }
     return launch_composite(rgb, sigma, t, d, far, n, N, white, in_sphere, comp, acc, w, lam, depth, (cudaStream_t)stream);
 }
 extern "C" int neo_clipped_sq_err(const float* pred, const float* gt, long long n, double* out_sum, void* stream) {
@@ -209,14 +218,20 @@ extern "C" int neo_volumetric_rendering_bwd(const float* rgb, const float* sigma
                                             const float* g_lam, const float* g_depth, float* d_rgb, float* d_sigma, void* stream) {
     if (n <= 0 || N < 1 || !rgb || !sigma || !t || !d_rgb || !d_sigma) { set_error("neo_volumetric_rendering_bwd: bad arguments"); return NEO_ERR_INVALID; }
     if (in_sphere != 0 && in_sphere != 1) { set_error("neo_volumetric_rendering_bwd: in_sphere must be 0 or 1"); return NEO_ERR_UNSUPPORTED; }
+    if (in_sphere && (!d || !far)) { set_error("neo_volumetric_rendering_bwd: in_sphere 1 reads rays_d and far"); return NEO_ERR_INVALID; }
     return launch_composite_bwd(rgb, sigma, t, d, far, n, N, white, in_sphere, g_comp, g_acc, g_w, g_lam, g_depth, d_rgb, d_sigma, (cudaStream_t)stream);
 }
 extern "C" int neo_index_grid_bwd(const NeoScene* sc, const float* pts, int M, const float* g_out, float* g_xz, float* g_xy, float* g_yz, void* stream) {
     if (!sc || M <= 0 || !pts || !g_out || !g_xz || !g_xy || !g_yz) { set_error("neo_index_grid_bwd: bad arguments"); return NEO_ERR_INVALID; }
+    if (!aligned16(g_out) || !aligned16(g_xz) || !aligned16(g_xy) || !aligned16(g_yz)) {
+        set_error("neo_index_grid_bwd: g_out and the gradient maps must be 16-byte aligned");
+        return NEO_ERR_INVALID;
+    }
     return launch_index_bwd(sc, pts, M, 0, g_out, nullptr, g_xz, g_xy, g_yz, (cudaStream_t)stream);
 }
 extern "C" int neo_index_local_bwd(const NeoScene* sc, const float* pts, int M, const float* g_out, float* g_latent, void* stream) {
     if (!sc || M <= 0 || !pts || !g_out || !g_latent) { set_error("neo_index_local_bwd: bad arguments"); return NEO_ERR_INVALID; }
+    if (!aligned16(g_out) || !aligned16(g_latent)) { set_error("neo_index_local_bwd: g_out and g_latent must be 16-byte aligned"); return NEO_ERR_INVALID; }
     return launch_index_bwd(sc, pts, M, 1, g_out, g_latent, nullptr, nullptr, nullptr, (cudaStream_t)stream);
 }
 extern "C" int neo_index_maps(const NeoScene* sc, const float* pts, int M, int C, const float* latent_cl, const float* xz_cl, const float* xy_cl,
@@ -231,6 +246,10 @@ extern "C" int neo_index_maps_bwd(const NeoScene* sc, const float* pts, int M, i
                                   float* g_xz_cl, float* g_xy_cl, float* g_yz_cl, void* stream) {
     if (!sc || M <= 0 || !pts || C < 4 || (C % 4) || (g_local && !g_latent_cl) || (g_world && !(g_xz_cl && g_xy_cl && g_yz_cl)) || !(g_local || g_world)) {
         set_error("neo_index_maps_bwd: bad arguments");
+        return NEO_ERR_INVALID;
+    }
+    if (!aligned16(g_local) || !aligned16(g_world) || !aligned16(g_latent_cl) || !aligned16(g_xz_cl) || !aligned16(g_xy_cl) || !aligned16(g_yz_cl)) {
+        set_error("neo_index_maps_bwd: row gradients and gradient maps must be 16-byte aligned");
         return NEO_ERR_INVALID;
     }
     return launch_index_maps_bwd(sc, pts, M, C, g_local, g_world, g_latent_cl, g_xz_cl, g_xy_cl, g_yz_cl, (cudaStream_t)stream);

@@ -72,6 +72,36 @@ def test_rowdot_f16_argument_validation_without_gpu(lib):
     assert lib.neo_tc_rowdot_f16(None, 256, 256, None, None, 1, 0, None, None) == 0   # M = 0: nothing to do
 
 
+def test_train_stage_argument_validation_without_gpu(lib):
+    """The compositing entry points reject NULL inputs the branch reads and an unknown in_sphere; the lookup backward entry points
+    reject row gradients / gradient maps that their float4 reductions cannot address -- all before touching the GPU (the data
+    pointers are never dereferenced)."""
+    p = 1 << 20
+    fwd = lambda rgb, sig, t, d, far, ins: lib.neo_volumetric_rendering(rgb, sig, t, d, far, 4, 8, 0, ins, p, p, p, None, p, None)
+    for args in ((None, p, p, p, p, 1), (p, None, p, p, p, 0), (p, p, None, p, p, 0),
+                 (p, p, p, None, p, 1), (p, p, p, p, None, 1), (p, p, p, None, None, 2),         # fg reads rays_d and far, vanilla rays_d
+                 (p, p, p, p, p, 3), (p, p, p, p, p, -1)):
+        assert fwd(*args) == -1, args
+    assert b"neo_volumetric_rendering" in lib.neo_last_error()
+    bwd = lambda rgb, sig, t, d, far, ins: lib.neo_volumetric_rendering_bwd(rgb, sig, t, d, far, 4, 8, 0, ins, p, None, None, None, None,
+                                                                            p, p, None)
+    for args in ((None, p, p, p, p, 1), (p, None, p, p, p, 0), (p, p, None, p, p, 0), (p, p, p, None, p, 1), (p, p, p, p, None, 1)):
+        assert bwd(*args) == -1, args
+    assert bwd(p, p, p, p, p, 2) == -5 and bwd(p, p, p, p, p, -1) == -5
+    # a zero-filled host block stands in for the scene: should the alignment check ever be skipped, the launcher reads nv = 0 from it
+    # and fails with an error code instead of dereferencing a wild pointer
+    scene = C.create_string_buffer(4096)
+    sc = C.addressof(scene)
+    assert lib.neo_index_grid_bwd(sc, p, 8, p + 4, p, p, p, None) == -1                  # g_out
+    assert lib.neo_index_grid_bwd(sc, p, 8, p, p, p + 8, p, None) == -1                  # g_xy
+    assert lib.neo_index_local_bwd(sc, p, 8, p, p + 4, None) == -1                       # g_latent
+    assert lib.neo_index_local_bwd(sc, p, 8, p + 12, p, None) == -1
+    assert lib.neo_index_maps_bwd(sc, p, 8, 256, p + 4, None, p, None, None, None, None) == -1    # g_local
+    assert lib.neo_index_maps_bwd(sc, p, 8, 256, None, p, None, p, p, p + 12, None) == -1         # g_yz
+    assert lib.neo_index_maps_bwd(sc, p, 8, 256, p, None, p + 8, None, None, None, None) == -1    # g_latent
+    assert b"16-byte" in lib.neo_last_error()
+
+
 @pytest.mark.parametrize("in_ch,ke", [(3, 64), (4, 96)])
 def test_tc_encoding_column_layout_is_a_permutation(lib, in_ch, ke):
     """The TC kernel orders the positional-encoding columns per coordinate (x, sin 2^k x, cos 2^k x); the weight image is permuted

@@ -1,5 +1,6 @@
-"""Training path (SURVEY.md 8(f2), 8(e) training row): backward of the hand-written stages against autograd through the oracle,
-the assembled differentiable NeRF_TP.forward against the oracle's gradients, and the flat-buffer gradient all-reduce (gloo, CPU)."""
+"""Training path (SURVEY.md 8(f2), 8(e) training row): the assembled differentiable NeRF_TP.forward against the oracle's gradients and
+the flat-buffer gradient all-reduce (gloo, CPU).  The hand-written backward stages on their own are checked against float64 in
+tests/test_gpu_train_stages.py."""
 import os
 import socket
 
@@ -24,39 +25,6 @@ def cuda():
     return torch.device("cuda:0")
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("in_sphere", [True, False])
-def test_composite_backward_vs_autograd(cuda, in_sphere):
-    """neo_volumetric_rendering_bwd against torch autograd through the oracle's composite (helper.py:128-171 semantics):
-    gradients w.r.t. rgb and sigma for upstream gradients on every output (comp, acc, weights, bg_lambda, depth).  Stated: 2e-5 relative."""
-    from neo360_b200.training import _Composite
-    g = torch.Generator().manual_seed(3)
-    n, N = 37, 29
-    rgb = torch.rand(n, N, 3, generator=g).requires_grad_(True)
-    sig = (torch.rand(n, N, 1, generator=g) * 3).requires_grad_(True)
-    t = torch.sort(torch.rand(n, N, generator=g), -1, descending=not in_sphere)[0]
-    d = torch.randn(n, 3, generator=g)
-    d = d / d.norm(dim=-1, keepdim=True)
-    far = t.max(-1, keepdim=True)[0] + 0.1
-    coef = [torch.randn(n, 3, generator=g), torch.randn(n, generator=g), torch.randn(n, N, generator=g), torch.randn(n, 1, generator=g),
-            torch.randn(n, generator=g)]
-
-    def loss_of(out):
-        comp, acc, w, lam, depth = out
-        l = (comp * coef[0].to(comp.device)).sum() + (acc * coef[1].to(comp.device)).sum() + (w * coef[2].to(comp.device)).sum() + \
-            (depth * coef[4].to(comp.device)).sum()
-        if in_sphere:
-            l = l + (lam * coef[3].to(comp.device)).sum()
-        return l
-
-    loss_of(orc.composite(rgb, sig, t, d, True, in_sphere, far)).backward()
-    r2, s2 = rgb.detach().to(cuda).requires_grad_(True), sig.detach().to(cuda).requires_grad_(True)
-    loss_of(_Composite.apply(r2, s2, t.to(cuda), d.to(cuda), far.to(cuda), True, in_sphere)).backward()
-    scale = float(sig.grad.abs().max())
-    assert md(r2.grad, rgb.grad) < 2e-5 * max(1.0, float(rgb.grad.abs().max()))
-    assert md(s2.grad, sig.grad) < 2e-5 * max(1.0, scale), (md(s2.grad, sig.grad), scale)
-
-
 def _tiny(cuda, nv=3):
     from neo360_b200 import NeRF_TP
     W, H, nc, nf = 32, 24, 8, 4
@@ -70,30 +38,6 @@ def _tiny(cuda, nv=3):
     sel = torch.arange(100, 100 + 24)
     rays = {"rays_o": ro[sel].contiguous(), "rays_d": rd[sel].contiguous(), "viewdirs": vd[sel].contiguous()}
     return net, sc, P, rays, (W, H, nc, nf)
-
-
-@pytest.mark.gpu
-def test_lookup_backward_vs_autograd(cuda):
-    """neo_index_grid_bwd / neo_index_local_bwd against autograd through the oracle's explicit bilinear lookups: gradients w.r.t. the
-    three tri-planes and the latent image, including points that project outside the maps.  Stated: 1e-4 of the gradient scale."""
-    from neo360_b200.training import _Lookup
-    net, sc, P, rays, (W, H, nc, nf) = _tiny(cuda)
-    g = torch.Generator().manual_seed(4)
-    pts = (torch.rand(300, 3, generator=g) - 0.5) * 1.6
-    maps = {k: sc[k].clone().requires_grad_(True) for k in ("planes_xz", "planes_xy", "planes_yz", "latent")}
-    osc = orc.Scene(maps["planes_xz"], maps["planes_xy"], maps["planes_yz"], maps["latent"], sc["src_poses"],
-                    float(sc["src_focal"][0]), float(sc["src_c"][0, 0]), float(sc["src_c"][0, 1]), W, H)
-    cam = orc.world2camera(pts, sc["src_poses"])
-    cw, cl = torch.randn(3 * 300, 128, generator=g), torch.randn(3 * 300, 512, generator=g)
-    ((orc.triplane_lookup(cam, osc).reshape(-1, 128) * cw).sum() + (orc.local_lookup(cam, osc).reshape(-1, 512) * cl).sum()).backward()
-    dmaps = {k: sc[k].to(cuda).requires_grad_(True) for k in maps}
-    net.set_scene(*[dmaps[k] for k in ("planes_xz", "planes_xy", "planes_yz", "latent")], *[sc[k].to(cuda) for k in ("src_poses", "src_focal", "src_c")],
-                  sc["img_wh"], precisions=["fp32"])
-    world, local = _Lookup.apply(pts.to(cuda), dmaps["planes_xz"], dmaps["planes_xy"], dmaps["planes_yz"], dmaps["latent"], net)
-    ((world * cw.to(cuda)).sum() + (local * cl.to(cuda)).sum()).backward()
-    for k in maps:
-        scale = float(maps[k].grad.abs().max())
-        assert scale > 0 and md(dmaps[k].grad, maps[k].grad) < 1e-4 * scale, (k, md(dmaps[k].grad, maps[k].grad), scale)
 
 
 @pytest.mark.gpu
