@@ -312,16 +312,13 @@ int neo_profile(int enable);
 int neo_profile_read(float* field_ms, int* n_field, unsigned long long* launches, double* points);
 
 /* Stage-level entry point of the tensor-core dense layer used by the wide MLPs (csrc/gemm_tc.cu: 2-D TMA tile loads, wgmma with
- * register accumulators): A (M,K), W (N,K) fp32 device, bias (N) or NULL -> out (M,N) fp32 = act(fp16(A) . fp16(W)^T + bias)
- * rounded to fp16.  K % 64 == 0, N % 64 == 0.  Synchronises the stream (allocates its fp16 staging buffers). */
-int neo_tc_dense(const float* A, const float* W, const float* bias, long long M, int N, int K, int relu, float* out, void* stream);
-/* The same kernel on caller-owned fp16 operands with explicit row strides (in elements), as the library's own callers use it:
+ * register accumulators), on caller-owned fp16 operands with explicit row strides (in elements), as the library's own callers use it:
  * C (M,N; row stride ldc) = act(A (M,K; lda) . W (N,K; ldw)^T + bias) rounded to fp16; A, W, C fp16 device, bias (N) fp32 or NULL.
  * K % 64 == 0, N % 64 == 0, strides % 8 == 0, lda, ldw >= K, ldc >= N, 16-byte aligned pointers.  Writes only columns [0, N) of
  * rows [0, M) of C, so A may sit in other columns of C's own rows.  Asynchronous on `stream`. */
 int neo_tc_gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M,
                     int N, int K, int relu, void* stream);
-/* Stage-level entry point of the tiny-N head used by the vanilla NeRF, Mip-NeRF 360 and encoder tensor-core paths (csrc/mip.cu
+/* Stage-level entry point of the tiny-N head used by the vanilla NeRF, Mip-NeRF 360 and encoder tensor-core paths (csrc/gemm_tc.cu
  * rowdot_f16): out (M,N) fp32 = H (M,K; row stride ld) fp16 . W (N,K)^T fp32 + b (N) fp32, fp32 accumulation.  N in {1, 3},
  * K % 8 == 0, ld % 8 == 0, K <= ld, N*K*4 <= 48 KB, H 16-byte aligned, no NULL pointer; M <= 0 does nothing.  Writes only rows
  * [0, M) of out.  Asynchronous on `stream`. */

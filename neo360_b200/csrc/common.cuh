@@ -3,6 +3,7 @@
 // a value feeds a discrete decision (sample positions, CDF brackets); see SURVEY.md Appendix A.
 #pragma once
 #include <cuda_runtime.h>
+#include <cuda_fp16.h>
 #include <stdint.h>
 #include <math.h>
 #include <vector>
@@ -178,7 +179,68 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
-// ---- host-side launchers shared between translation units ----
+// Column c of the reference positional encoding of x[0..ich) (helper.py:121-125, also the vanilla NeRF and Mip-NeRF 360 direction
+// encodings): [x | sin(x 2^k), k-major, k < deg | sin(x 2^k + pi/2)].  The fp32 parity paths depend on this exact mul / add / sinf
+// sequence; the tensor-core paths' angle-doubling encodings are different arithmetic and do not use it.
+__device__ __forceinline__ float pos_enc_col(const float* x, int ich, int deg, int c) {
+    if (c < ich) return x[c];
+    int q = c - ich;
+    const bool shifted = q >= ich * deg;
+    if (shifted) q -= ich * deg;
+    const float xb = mul_(x[q % ich], (float)(1 << (q / ich)));
+    return sinf(shifted ? add_(xb, 1.57079637f) : xb);
+}
+
+// Head activations of the reference MLPs: density = softplus_(raw - 1), rgb = rgb_act(raw)   (models/neo360/model.py:392-397)
+__device__ __forceinline__ float softplus_(float x) { return x > 20.f ? x : log1pf(expf(x)); }
+__device__ __forceinline__ float sigmoid_(float x) { return 1.f / (1.f + expf(-x)); }
+__device__ __forceinline__ float rgb_act(float x) { return sigmoid_(x) * 1.002f - 0.001f; }
+
+// acc[r] += A[r][0..K) . Wt[0..K)[j] for ROWS rows of A (row stride lda, 16-byte aligned rows); Wt is (in, out) with row stride ldw.
+// One thread per output neuron j: the weight loads are coalesced across the block, the activation rows are shared-memory broadcasts.
+template <int ROWS>
+__device__ __forceinline__ void dense_rows(const float* __restrict__ Wt, int ldw, int K, const float* __restrict__ A, int lda, float* acc, int j) {
+    int k = 0;
+    for (; k + 4 <= K; k += 4) {
+        float w0 = __ldg(Wt + (size_t)(k + 0) * ldw + j), w1 = __ldg(Wt + (size_t)(k + 1) * ldw + j);
+        float w2 = __ldg(Wt + (size_t)(k + 2) * ldw + j), w3 = __ldg(Wt + (size_t)(k + 3) * ldw + j);
+#pragma unroll
+        for (int r = 0; r < ROWS; ++r) {
+            float4 a = *reinterpret_cast<const float4*>(A + r * lda + k);
+            acc[r] = fmaf(a.w, w3, fmaf(a.z, w2, fmaf(a.y, w1, fmaf(a.x, w0, acc[r]))));
+        }
+    }
+    for (; k < K; ++k) {
+        float w0 = __ldg(Wt + (size_t)k * ldw + j);
+#pragma unroll
+        for (int r = 0; r < ROWS; ++r) acc[r] = fmaf(A[r * lda + k], w0, acc[r]);
+    }
+}
+
+template <class T> __device__ __forceinline__ T from_f32(float v);
+template <> __device__ __forceinline__ float from_f32<float>(float v) { return v; }
+template <> __device__ __forceinline__ __half from_f32<__half>(float v) { return __float2half_rn(v); }
+
+// ---- host side shared between translation units ----
+// Bump allocation of a caller-provided workspace: every block starts on a 256-byte boundary.  With base == nullptr it only counts,
+// so the same carving code computes the workspace size and the pointers.
+struct Carve {
+    unsigned char* base;
+    size_t used;
+    template <class T> T* take(size_t count) {
+        T* p = base ? reinterpret_cast<T*>(base + used) : nullptr;
+        used += (count * sizeof(T) + 255) & ~size_t(255);
+        return p;
+    }
+};
+
+// Copies n floats of a workspace result to an optional output; NULL (not wanted) or the same buffer is a no-op.
+inline int copy_out(float* dst, const float* src, size_t n, cudaStream_t s) {
+    if (!dst || dst == src) return NEO_OK;
+    NEO_CUDA(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    return NEO_OK;
+}
+
 struct MLPFp32 {   // weights transposed to (in, out) for coalesced reads by output-neuron threads
     int in_ch, enc_dim, in_dim;   // 3|4, 63|84, enc+512+128
     const float *w0t, *b0, *w1t, *b1, *w2t, *b2, *w3t, *b3, *wbt, *bb, *wsig, *bsig, *wv0t, *bv0, *wv1t, *bv1, *wrgb, *brgb;
@@ -204,6 +266,11 @@ int scene_alloc_bytes(NeoScene* sc, void** p, size_t bytes);
 // the same shape: a scene change then costs its kernels, not cudaMalloc / cudaFree (which are slow, erratic and device-synchronising).
 int pool_alloc(void** p, size_t bytes);
 void pool_release(void* p, size_t bytes);
+// (n, C, HW) fp32 -> (n, HW, C) fp32 or fp16 (round to nearest): channel-last copies of feature maps
+int launch_nchw_to_nhwc(const float* in, float* out, int n, int C, int HW, cudaStream_t s);
+int launch_nchw_to_nhwc(const float* in, __half* out, int n, int C, int HW, cudaStream_t s);
+// nn.Linear weight (out_f, in_f) -> (in_f, out_f), for the CUDA-core MLPs' coalesced weight reads (dense_rows)
+int launch_transpose(const float* w, float* wt, int out_f, int in_f, cudaStream_t s);
 // sampling.cu
 int launch_far(const float* o, const float* d, int n, float* far, int* err, cudaStream_t s);
 int launch_sample_coarse(const float* o, const float* d, const float* far, int n, int num_samples, int in_sphere,
@@ -241,4 +308,9 @@ int tc_scene_create(NeoScene* sc, const NeoMLPParams mlps[4], cudaStream_t s);
 void tc_scene_free(NeoScene* sc);
 int launch_field_tc(const NeoScene* sc, const NeoRays* rays, const float* far, const float* t, int N, int mlp_index,
                     float* rgb, float* sigma, cudaStream_t s);
+// gemm_tc.cu: the tensor-core dense layer, fp16 operand packing and the tiny-N head (contracts at their definitions)
+int gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M, int N, int K,
+             int relu, cudaStream_t s);
+int f32_to_f16_pad(const float* in, long long rows, int cols_in, long long ld_in, void* out, int cols_out, long long ld_out, cudaStream_t s);
+int launch_rowdot_f16(const void* H, long long ld, int K, const float* W, const float* b, int N, long long M, float* out, cudaStream_t s);
 }  // namespace neo

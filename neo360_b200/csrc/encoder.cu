@@ -9,11 +9,6 @@
 #include <cuda_fp16.h>
 
 namespace neo {
-int gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M, int N, int K,
-             int relu, cudaStream_t s);
-int f32_to_f16_pad(const float* in, long long rows, int cols_in, long long ld_in, void* out, int cols_out, long long ld_out, cudaStream_t s);
-int launch_rowdot_f16(const void* H, long long ld, int K, const float* W, const float* b, int N, long long M, float* out, cudaStream_t s);
-
 namespace enc {
 
 constexpr int kG = 64, kNC = kG * kG * kG, kLat = 512, kIn = 518, kLd = 576;      // 518 -> 576 (multiple of 64) zero padded
@@ -26,23 +21,6 @@ __device__ __forceinline__ float lin(float a, float b, int i, int n) {
 __device__ __forceinline__ void cell_xyz(int cell, float* x) {
     const int ix = cell / (kG * kG), iy = (cell / kG) % kG, iz = cell % kG;
     x[0] = lin(-1.f, 1.f, ix, kG); x[1] = lin(-1.f, 1.f, iy, kG); x[2] = lin(0.f, 1.f, iz, kG);     // side_lengths [1,1,1]: z in [0,1]
-}
-
-// (n, C, HW) -> (n, HW, C)
-__global__ void to_channel_last_kernel(const float* __restrict__ in, float* __restrict__ out, int C, int HW) {
-    __shared__ float tile[32][33];
-    const int n = blockIdx.z, c0 = blockIdx.y * 32, p0 = blockIdx.x * 32;
-    const float* src = in + (size_t)n * C * HW;
-    float* dst = out + (size_t)n * C * HW;
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const int c = c0 + i, p = p0 + threadIdx.x;
-        if (c < C && p < HW) tile[i][threadIdx.x] = src[(size_t)c * HW + p];
-    }
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const int p = p0 + i, c = c0 + threadIdx.x;
-        if (c < C && p < HW) dst[(size_t)p * C + c] = tile[threadIdx.x][i];
-    }
 }
 
 // one block (128 threads = 512 channels / 4) per (view, grid cell): row = [latent lookup (512) | cam xyz (3) | direction (3) | 0 ...]
@@ -134,20 +112,16 @@ __global__ void __launch_bounds__(128) pillar_sum_kernel(const __half* __restric
     o[0] = a0; o[(size_t)kG * kG] = a1; o[(size_t)2 * kG * kG] = a2; o[(size_t)3 * kG * kG] = a3;
 }
 
-struct Cv {
-    unsigned char* base; size_t used;
-    void* take(size_t bytes) { bytes = (bytes + 255) & ~size_t(255); void* p = base ? base + used : nullptr; used += bytes; return p; }
-};
 struct WS { float* lat_cl; __half *X, *Ha, *Hb, *L, *W; float* logits; };
-size_t carve(Cv& c, int nv, int lh, int lw, WS& w) {
+size_t carve(Carve& c, int nv, int lh, int lw, WS& w) {
     const size_t R = (size_t)nv * kNC;
-    w.lat_cl = (float*)c.take((size_t)nv * lh * lw * kLat * 4);
-    w.X = (__half*)c.take(R * kLd * 2);
-    w.Ha = (__half*)c.take(R * kLat * 2);
-    w.Hb = (__half*)c.take(R * kLat * 2);
-    w.L = (__half*)c.take(R * kLd * 2);
-    w.W = (__half*)c.take(((size_t)kLat * kLd + 2 * (size_t)kLat * kLat + 3 * (size_t)kLat * kLd) * 2);
-    w.logits = (float*)c.take(R * 4);
+    w.lat_cl = c.take<float>((size_t)nv * lh * lw * kLat);
+    w.X = c.take<__half>(R * kLd);
+    w.Ha = c.take<__half>(R * kLat);
+    w.Hb = c.take<__half>(R * kLat);
+    w.L = c.take<__half>(R * kLd);
+    w.W = c.take<__half>((size_t)kLat * kLd + 2 * (size_t)kLat * kLat + 3 * (size_t)kLat * kLd);
+    w.logits = c.take<float>(R);
     return c.used;
 }
 
@@ -158,7 +132,7 @@ using namespace neo;
 
 extern "C" size_t neo_grid_encoder_workspace_bytes(int nv, int lat_h, int lat_w) {
     if (nv < 1 || lat_h < 2 || lat_w < 2) return 0;
-    enc::Cv c{nullptr, 0};
+    Carve c{nullptr, 0};
     enc::WS w;
     return enc::carve(c, nv, lat_h, lat_w, w);
 }
@@ -172,17 +146,13 @@ extern "C" int neo_grid_encoder_dense(const NeoGridEncoderParams* p, const float
         return NEO_ERR_INVALID;
     }
     cudaStream_t s = (cudaStream_t)stream;
-    Cv c{(unsigned char*)workspace, 0};
+    Carve c{static_cast<unsigned char*>(workspace), 0};
     WS w;
     const size_t need = carve(c, nv, lat_h, lat_w, w);
     if (!workspace || workspace_bytes < need) { set_error("workspace too small: need %zu bytes, got %zu", need, workspace_bytes); return NEO_ERR_WORKSPACE; }
     const long long R = (long long)nv * kNC;
     int rc;
-    {
-        dim3 grid((lat_h * lat_w + 31) / 32, (kLat + 31) / 32, nv), block(32, 8);
-        to_channel_last_kernel<<<grid, block, 0, s>>>(latent, w.lat_cl, kLat, lat_h * lat_w);
-        NEO_LAUNCH_CHECK("encoder to_channel_last_kernel");
-    }
+    if ((rc = launch_nchw_to_nhwc(latent, w.lat_cl, nv, kLat, lat_h * lat_w, s))) return rc;
     // latent_scaling = size / (size - 1) * 2 ; scale = latent_scaling / image_size   (encoder_pn.py:119, 204-206)
     const float sx = (float)lat_w / ((float)lat_w - 1.0f) * 2.0f / (float)img_w, sy = (float)lat_h / ((float)lat_h - 1.0f) * 2.0f / (float)img_h;
     grid_gather_kernel<<<(unsigned)R, 128, 0, s>>>(w.lat_cl, lat_h, lat_w, src_poses, focal, cx, cy, sx, sy, w.X);

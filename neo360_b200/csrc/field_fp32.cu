@@ -18,29 +18,6 @@ struct RowGeo {
     int valid;
 };
 
-template <int ROWS>
-__device__ __forceinline__ void dense_acc(const float* __restrict__ Wt, int K, const float* __restrict__ A, int lda,
-                                          float* acc, int j) {
-    int k = 0;
-    for (; k + 4 <= K; k += 4) {
-        float w0 = __ldg(Wt + (size_t)(k + 0) * kHidden + j), w1 = __ldg(Wt + (size_t)(k + 1) * kHidden + j);
-        float w2 = __ldg(Wt + (size_t)(k + 2) * kHidden + j), w3 = __ldg(Wt + (size_t)(k + 3) * kHidden + j);
-#pragma unroll
-        for (int r = 0; r < ROWS; ++r) {
-            float4 a = *reinterpret_cast<const float4*>(A + r * lda + k);
-            acc[r] = fmaf(a.w, w3, fmaf(a.z, w2, fmaf(a.y, w1, fmaf(a.x, w0, acc[r]))));
-        }
-    }
-    for (; k < K; ++k) {
-        float w0 = __ldg(Wt + (size_t)k * kHidden + j);
-#pragma unroll
-        for (int r = 0; r < ROWS; ++r) acc[r] = fmaf(A[r * lda + k], w0, acc[r]);
-    }
-}
-
-__device__ __forceinline__ float softplus_(float x) { return x > 20.f ? x : log1pf(expf(x)); }
-__device__ __forceinline__ float sigmoid_(float x) { return 1.f / (1.f + expf(-x)); }
-
 template <int NV>
 __global__ void __launch_bounds__(kThreads)
 field_fp32_kernel(SceneDev sc, MLPFp32 mlp, const float* __restrict__ rays_o, const float* __restrict__ rays_d,
@@ -104,37 +81,12 @@ field_fp32_kernel(SceneDev sc, MLPFp32 mlp, const float* __restrict__ rays_o, co
     for (int e = j; e < ROWS * enc; e += kThreads) {
         int r = e / enc, c = e % enc;
         const RowGeo& rg = geo[r];
-        float val = 0.f;
-        if (rg.valid) {
-            if (c < ich) val = rg.enc_in[c];
-            else {
-                int q = c - ich;
-                int half = ich * kPosDeg;
-                bool shifted = q >= half;
-                if (shifted) q -= half;
-                int k = q / ich, cc = q % ich;
-                float xb = mul_(rg.enc_in[cc], (float)(1 << k));
-                val = sinf(shifted ? add_(xb, 1.57079637f) : xb);
-            }
-        }
-        X[r * ldx + c] = val;
+        X[r * ldx + c] = rg.valid ? pos_enc_col(rg.enc_in, ich, kPosDeg, c) : 0.f;
     }
     for (int e = j; e < ROWS * 28; e += kThreads) {
         int r = e / 28, c = e % 28;
         const RowGeo& rg = geo[r];
-        float val = 0.f;
-        if (rg.valid && c < kDirEnc) {
-            if (c < 3) val = rg.dir[c];
-            else {
-                int q = c - 3;
-                bool shifted = q >= 12;
-                if (shifted) q -= 12;
-                int k = q / 3, cc = q % 3;
-                float xb = mul_(rg.dir[cc], (float)(1 << k));
-                val = sinf(shifted ? add_(xb, 1.57079637f) : xb);
-            }
-        }
-        Dn[e] = val;
+        Dn[e] = (rg.valid && c < kDirEnc) ? pos_enc_col(rg.dir, 3, 4, c) : 0.f;
     }
     for (int r = 0; r < ROWS; ++r) {
         const RowGeo& rg = geo[r];
@@ -178,15 +130,15 @@ field_fp32_kernel(SceneDev sc, MLPFp32 mlp, const float* __restrict__ rays_o, co
 #pragma unroll
         for (int r = 0; r < ROWS; ++r) H[r * ldh + j] = fmaxf(acc[r], 0.f);
     };
-    bias_init(mlp.b0); dense_acc<ROWS>(mlp.w0t, in_dim, X, ldx, acc, j); store_relu(Ha); __syncthreads();
-    bias_init(mlp.b1); dense_acc<ROWS>(mlp.w1t, kHidden, Ha, ldh, acc, j); store_relu(Hb); __syncthreads();
-    bias_init(mlp.b2); dense_acc<ROWS>(mlp.w2t, kHidden, Hb, ldh, acc, j); store_relu(Ha); __syncthreads();
+    bias_init(mlp.b0); dense_rows<ROWS>(mlp.w0t, kHidden, in_dim, X, ldx, acc, j); store_relu(Ha); __syncthreads();
+    bias_init(mlp.b1); dense_rows<ROWS>(mlp.w1t, kHidden, kHidden, Ha, ldh, acc, j); store_relu(Hb); __syncthreads();
+    bias_init(mlp.b2); dense_rows<ROWS>(mlp.w2t, kHidden, kHidden, Hb, ldh, acc, j); store_relu(Ha); __syncthreads();
     bias_init(mlp.b3);
-    dense_acc<ROWS>(mlp.w3t, kHidden, Ha, ldh, acc, j);                              // [h2 | inputs]
-    dense_acc<ROWS>(mlp.w3t + (size_t)kHidden * kHidden, in_dim, X, ldx, acc, j);
-    store_relu(Hb); __syncthreads();                                                // Hb = h3 (per view)
+    dense_rows<ROWS>(mlp.w3t, kHidden, kHidden, Ha, ldh, acc, j);                              // [h2 | inputs]
+    dense_rows<ROWS>(mlp.w3t + (size_t)kHidden * kHidden, kHidden, in_dim, X, ldx, acc, j);
+    store_relu(Hb); __syncthreads();                                                          // Hb = h3 (per view)
     // bottleneck (per view) -> Ha ; hbar = mean_v h3 -> density
-    bias_init(mlp.bb); dense_acc<ROWS>(mlp.wbt, kHidden, Hb, ldh, acc, j);
+    bias_init(mlp.bb); dense_rows<ROWS>(mlp.wbt, kHidden, kHidden, Hb, ldh, acc, j);
 #pragma unroll
     for (int r = 0; r < ROWS; ++r) Ha[r * ldh + j] = acc[r];
     {
@@ -257,7 +209,7 @@ field_fp32_kernel(SceneDev sc, MLPFp32 mlp, const float* __restrict__ rays_o, co
         if (gp < total) {
             float a = __ldg(mlp.brgb + c);
             for (int k = 0; k < 64; ++k) a = fmaf(q1[p * 68 + k], __ldg(mlp.wrgb + c * 64 + k), a);
-            rgb_out[gp * 3 + c] = sigmoid_(a) * 1.002f - 0.001f;                     // model.py:395-397
+            rgb_out[gp * 3 + c] = rgb_act(a);                                       // model.py:395-397
         }
     }
 }

@@ -91,23 +91,7 @@ struct Params {
 // ------------------------------------------------------------------------------------------------
 // Per scene and MLP the latent columns of layers 0 and 3 are applied to the raw feature maps once (linearity of the lookups):
 // P[v][pixel][p] = sum_c Wsel[p][c] * F[v][c][pixel],  p in [0,256) = [P0 | P3] in pmap_logical order -- a plain contraction, run on
-// the tensor cores by gemm_f16 (csrc/gemm_tc.cu) from the two operands prepared below.
-// (n, C, HW) fp32 -> (n, HW, C) fp16: the A operand (pixels x channels, K-major) of the tensor-core pre-projection
-__global__ void nchw_to_nhwc_f16_kernel(const float* __restrict__ in, __half* __restrict__ out, int C, int HW) {
-    __shared__ float tile[32][33];
-    const int n = blockIdx.z, c0 = blockIdx.y * 32, p0 = blockIdx.x * 32;
-    const float* src = in + (size_t)n * C * HW;
-    __half* dst = out + (size_t)n * C * HW;
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const int c = c0 + i, p = p0 + threadIdx.x;
-        if (c < C && p < HW) tile[i][threadIdx.x] = src[(size_t)c * HW + p];
-    }
-    __syncthreads();
-    for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-        const int p = p0 + i, c = c0 + threadIdx.x;
-        if (c < C && p < HW) dst[(size_t)p * C + c] = __float2half_rn(tile[threadIdx.x][i]);
-    }
-}
+// the tensor cores by gemm_f16 (csrc/gemm_tc.cu) from the channel-last fp16 maps (launch_nchw_to_nhwc) and the weight rows below.
 // Wsel[p][c] fp16, p in [0,256): logical row r = pmap_logical(p); rows 0..127 = W0[r][col0 + c], rows 128..255 = W3[r - 128][col3 + c]
 // (the latent columns of layers 0 and 3)
 __global__ void wsel_kernel(const float* __restrict__ w0, int ld0, int col0, const float* __restrict__ w3, int ld3, int col3, int C, __half* __restrict__ out) {
@@ -547,7 +531,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
             for (int i = 0; i < 2; ++i) {
                 const PtsRow& pr = i ? pr1 : pr0;
                 const float xs = (hacc[32 + 2 * i] + sb[644]) - 1.0f;                   // model.py:392-393
-                if (pr.valid) P.sigma_out[(long long)pr.rid * N + pr.sidx] = xs > 20.f ? xs : log1pf(expf(xs));
+                if (pr.valid) P.sigma_out[(long long)pr.rid * N + pr.sidx] = softplus_(xs);
             }
         }
         uint32_t qa[4][4];
@@ -590,7 +574,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const int c = 2 * t + e;
-                    if (c < 3) P.rgb_out[gp * 3 + c] = (1.f / (1.f + expf(-o[2 * i + e]))) * 1.002f - 0.001f;   // model.py:395-397
+                    if (c < 3) P.rgb_out[gp * 3 + c] = rgb_act(o[2 * i + e]);   // model.py:395-397
                 }
             }
         }
@@ -625,9 +609,6 @@ const char* tc_trap_info() {
     return buf;
 }
 
-int gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M, int N, int K,
-             int relu, cudaStream_t s);       // csrc/gemm_tc.cu
-
 int tc_scene_create(NeoScene* sc, const NeoMLPParams mlps[4], cudaStream_t s) {
     using namespace tc;
     const NeoSceneDesc& d = sc->desc;
@@ -656,9 +637,7 @@ int tc_scene_create(NeoScene* sc, const NeoMLPParams mlps[4], cudaStream_t s) {
             const int C = k ? kWorldCh : kLocalCh, hw = k ? d.plane_h * d.plane_w : d.lat_h * d.lat_w;
             tmp.bytes[k] = (size_t)d.nv * hw * C * 2;
             if ((rc = pool_alloc((void**)&feat16[k], tmp.bytes[k]))) return rc;
-            dim3 grid((hw + 31) / 32, (C + 31) / 32, d.nv), block(32, 8);
-            nchw_to_nhwc_f16_kernel<<<grid, block, 0, s>>>(srcs[k], feat16[k], C, hw);
-            NEO_LAUNCH_CHECK("nchw_to_nhwc_f16_kernel");
+            if ((rc = launch_nchw_to_nhwc(srcs[k], feat16[k], d.nv, C, hw, s))) return rc;
         }
         if ((rc = pool_alloc((void**)&wsel, (size_t)256 * kLocalCh * 2))) return rc;
     }

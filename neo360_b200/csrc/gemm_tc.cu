@@ -7,6 +7,8 @@
 // One CTA per 128 x BN output tile: warp 8 = TMA producer (one lane), warps 0-7 = two consumer warpgroups, each owning 64 rows of the
 // tile (wgmma m64nBNk16, accumulators in registers).  3-stage shared-memory ring (A 128 x 64, W BN x 64 per stage) with full / empty
 // mbarriers; two CTAs fit on an SM, so one CTA's epilogue (bias -> ReLU -> fp16 -> global) overlaps the other's main loop.
+//
+// Beside it: f32_to_f16_pad (weight / activation packing) and rowdot_f16, the N = 1 / 3 density and rgb heads of the same paths.
 #include "common.cuh"
 #include "hopper.cuh"
 #include <cuda.h>
@@ -100,6 +102,53 @@ __global__ void f32_to_f16_pad_kernel(const float* __restrict__ in, long long ro
     out[r * ld_out + c] = __float2half_rn(c < cols_in ? in[r * ld_in + c] : 0.f);
 }
 
+// ---- tiny-N head: out[m][c] = sum_k fp16 h[m][k] * w[c][k] + b[c]  (density: N = 1, rgb: N = 3) ----
+// HBM-bound (one pass over the activation rows).  8 lanes per row, 4 rows per warp: every load instruction fetches four whole
+// 128-byte lines; the weights sit in shared memory (fp32, read as broadcast float4); 3 shuffles finish a row.
+constexpr int kRowdotIters = 4;          // row groups per warp: 8 warps x 4 rows x 4 = 128 rows per block
+template <int N>
+__global__ void __launch_bounds__(256) rowdot_f16_kernel(const __half* __restrict__ H, long long ld, int K, const float* __restrict__ Wt,
+                                                         const float* __restrict__ b, long long M, float* __restrict__ out) {
+    extern __shared__ __align__(16) float wsm[];          // [N][K]
+    for (int i = threadIdx.x; i < N * K; i += blockDim.x) wsm[i] = Wt[i];
+    __syncthreads();
+    const int lane = threadIdx.x & 31, sub = lane & 7, rsel = lane >> 3, warp = threadIdx.x >> 5;
+    float bias[N];
+#pragma unroll
+    for (int c = 0; c < N; ++c) bias[c] = b[c];
+#pragma unroll 1
+    for (int it = 0; it < kRowdotIters; ++it) {
+        const long long m = (((long long)blockIdx.x * kRowdotIters + it) * 8 + warp) * 4 + rsel;
+        float acc[N];
+#pragma unroll
+        for (int c = 0; c < N; ++c) acc[c] = 0.f;
+        if (m < M) {
+            const __half* h = H + m * ld;
+            for (int k = sub * 8; k < K; k += 64) {
+                const uint4 v = *reinterpret_cast<const uint4*>(h + k);
+                const __half2* hv = reinterpret_cast<const __half2*>(&v);
+                const float2 f0 = __half22float2(hv[0]), f1 = __half22float2(hv[1]), f2 = __half22float2(hv[2]), f3 = __half22float2(hv[3]);
+#pragma unroll
+                for (int c = 0; c < N; ++c) {
+                    const float4 w0 = *reinterpret_cast<const float4*>(wsm + c * K + k), w1 = *reinterpret_cast<const float4*>(wsm + c * K + k + 4);
+                    acc[c] = fmaf(f0.x, w0.x, fmaf(f0.y, w0.y, fmaf(f1.x, w0.z, fmaf(f1.y, w0.w,
+                             fmaf(f2.x, w1.x, fmaf(f2.y, w1.y, fmaf(f3.x, w1.z, fmaf(f3.y, w1.w, acc[c]))))))));
+                }
+            }
+        }
+#pragma unroll
+        for (int c = 0; c < N; ++c) {
+            acc[c] += __shfl_xor_sync(0xffffffffu, acc[c], 1);
+            acc[c] += __shfl_xor_sync(0xffffffffu, acc[c], 2);
+            acc[c] += __shfl_xor_sync(0xffffffffu, acc[c], 4);
+        }
+        if (m < M && sub == 0) {
+#pragma unroll
+            for (int c = 0; c < N; ++c) out[m * N + c] = acc[c] + bias[c];
+        }
+    }
+}
+
 static int make_tmap_2d(CUtensorMap* out, const void* base, long long rows, int K, long long ld, int box_rows) {
     typedef CUresult (*EncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -165,43 +214,29 @@ int f32_to_f16_pad(const float* in, long long rows, int cols_in, long long ld_in
     NEO_LAUNCH_CHECK("f32_to_f16_pad_kernel");
     return NEO_OK;
 }
+// out (M x N) fp32 = H (M x K, fp16, row stride ld) . W (N x K, fp32)^T + b: the density / rgb heads of the vanilla NeRF, Mip-NeRF 360 and
+// encoder tensor-core paths.
+int launch_rowdot_f16(const void* H, long long ld, int K, const float* W, const float* b, int N, long long M, float* out, cudaStream_t s) {
+    if (M <= 0) return NEO_OK;
+    if ((K % 8) || (ld % 8) || (N != 1 && N != 3)) { set_error("rowdot_f16: K %% 8, ld %% 8 and N in {1, 3} required (K=%d ld=%lld N=%d)", K, ld, N); return NEO_ERR_INVALID; }
+    if (K <= 0 || ld < K || (size_t)N * K * sizeof(float) > 48 * 1024) { set_error("rowdot_f16: need 0 < K <= ld and N*K*4 <= 48 KB (K=%d ld=%lld N=%d)", K, ld, N); return NEO_ERR_INVALID; }
+    if (!H || !W || !b || !out || (reinterpret_cast<uintptr_t>(H) & 15)) { set_error("rowdot_f16: null pointer or H not 16-byte aligned"); return NEO_ERR_INVALID; }
+    const unsigned grid = (unsigned)((M + 8 * 4 * gemm::kRowdotIters - 1) / (8 * 4 * gemm::kRowdotIters));
+    const size_t smem = (size_t)N * K * sizeof(float);
+    if (N == 1) gemm::rowdot_f16_kernel<1><<<grid, 256, smem, s>>>((const __half*)H, ld, K, W, b, M, out);
+    else gemm::rowdot_f16_kernel<3><<<grid, 256, smem, s>>>((const __half*)H, ld, K, W, b, M, out);
+    NEO_LAUNCH_CHECK("rowdot_f16_kernel");
+    return NEO_OK;
+}
 
 }  // namespace neo
-
-// Stage-level entry point (self-test / parity test of the tensor-core dense layer): A (M,K), W (N,K) fp32 device -> out (M,N) fp32 =
-// act(fp16(A) . fp16(W)^T + bias) rounded to fp16, computed by gemm_f16_kernel.  K % 64 == 0, N % 64 == 0.
-extern "C" int neo_tc_dense(const float* A, const float* W, const float* bias, long long M, int N, int K, int relu, float* out, void* stream);
-
-namespace neo { namespace gemm {
-__global__ void f16_to_f32_kernel(const __half* __restrict__ in, long long n, float* __restrict__ out) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = __half2float(in[i]);
-}
-} }
-
-extern "C" int neo_tc_dense(const float* A, const float* W, const float* bias, long long M, int N, int K, int relu, float* out, void* stream) {
-    using namespace neo;
-    if (!A || !W || !out || M <= 0) { set_error("neo_tc_dense: bad arguments"); return NEO_ERR_INVALID; }
-    cudaStream_t s = (cudaStream_t)stream;
-    __half *a = nullptr, *w = nullptr, *c = nullptr;
-    NEO_CUDA(cudaMalloc(&a, (size_t)M * K * 2));
-    NEO_CUDA(cudaMalloc(&w, (size_t)N * K * 2));
-    NEO_CUDA(cudaMalloc(&c, (size_t)M * N * 2));
-    int rc = f32_to_f16_pad(A, M, K, K, a, K, K, s);
-    if (!rc) rc = f32_to_f16_pad(W, N, K, K, w, K, K, s);
-    if (!rc) rc = gemm_f16(a, K, w, K, bias, c, N, M, N, K, relu, s);
-    if (!rc) {
-        gemm::f16_to_f32_kernel<<<(unsigned)(((long long)M * N + 255) / 256), 256, 0, s>>>(c, (long long)M * N, out);
-        cudaError_t e = cudaGetLastError();
-        if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess) rc = cuda_fail(e, "neo_tc_dense");
-    }
-    cudaFree(a); cudaFree(w); cudaFree(c);
-    return rc;
-}
 
 // Stage-level entry point of gemm_f16 itself, at the strides and aliasing its callers use: fp16 device operands, asynchronous on `stream`.
 extern "C" int neo_tc_gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M,
                                int N, int K, int relu, void* stream) {
     return neo::gemm_f16(A, lda, W, ldw, bias, C, ldc, M, N, K, relu, (cudaStream_t)stream);
+}
+// Stage-level entry point of rowdot_f16, the tiny-N head of the vanilla NeRF, Mip-NeRF 360 and encoder paths.
+extern "C" int neo_tc_rowdot_f16(const void* H, long long ld, int K, const float* W, const float* b, int N, long long M, float* out, void* stream) {
+    return neo::launch_rowdot_f16(H, ld, K, W, b, N, M, out, (cudaStream_t)stream);
 }

@@ -276,42 +276,14 @@ __global__ void __launch_bounds__(kFeatThreads) features16_kernel(const float* _
     }
 }
 
-// direction encoding broadcast to samples: DE[m][27]
-__global__ void dir16_kernel(const float* __restrict__ viewdirs, long long M, int n, __half* __restrict__ out, long long ld, int pad) {
+// direction encoding broadcast to samples: out[m][c] for c < cols (27, or the fp16 operand's 64 with zero padding), row stride ld
+template <class T>
+__global__ void dir_kernel(const float* __restrict__ viewdirs, long long M, int n, T* __restrict__ out, long long ld, int cols) {
     const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (gid >= M * pad) return;
-    const long long m = gid / pad;
-    const int c = (int)(gid % pad);
-    float val = 0.f;
-    if (c < 27) {
-        const float* d = viewdirs + 3 * (m / n);
-        if (c < 3) val = d[c];
-        else {
-            int q = c - 3;
-            const bool shifted = q >= 12;
-            if (shifted) q -= 12;
-            const float xb = mul_(d[q % 3], (float)(1 << (q / 3)));
-            val = sinf(shifted ? add_(xb, 1.57079637f) : xb);
-        }
-    }
-    out[m * ld + c] = __float2half_rn(val);
-}
-__global__ void dir_kernel(const float* __restrict__ viewdirs, long long M, int n, float* __restrict__ DE) {
-    const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (gid >= M * 27) return;
-    const long long m = gid / 27;
-    const int c = (int)(gid % 27);
-    const float* d = viewdirs + 3 * (m / n);
-    float val;
-    if (c < 3) val = d[c];
-    else {
-        int q = c - 3;
-        const bool shifted = q >= 12;
-        if (shifted) q -= 12;
-        const float xb = mul_(d[q % 3], (float)(1 << (q / 3)));
-        val = sinf(shifted ? add_(xb, 1.57079637f) : xb);
-    }
-    DE[gid] = val;
+    if (gid >= M * cols) return;
+    const long long m = gid / cols;
+    const int c = (int)(gid % cols);
+    out[m * ld + c] = from_f32<T>(c < kDirEnc ? pos_enc_col(viewdirs + 3 * (m / n), 3, 4, c) : 0.f);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -384,11 +356,9 @@ __global__ void composite_kernel(const float* __restrict__ raw_density, const fl
         const bool ok = k < n;
         float dens = 0.f, dd = 0.f, col[3] = {0.f, 0.f, 0.f};
         if (ok) {
-            const float xs = raw_density[(size_t)b * n + k] - 1.0f;
-            dens = xs > 20.f ? xs : log1pf(expf(xs));
+            dens = softplus_(raw_density[(size_t)b * n + k] - 1.0f);
             dd = (k == n - 1) ? INFINITY : mul_(dens, mul_(sub_(t[k + 1], t[k]), dn));
-            for (int c = 0; c < 3; ++c)
-                col[c] = raw_rgb ? (1.f / (1.f + expf(-raw_rgb[((size_t)b * n + k) * 3 + c]))) * 1.002f - 0.001f : 0.f;
+            for (int c = 0; c < 3; ++c) col[c] = raw_rgb ? rgb_act(raw_rgb[((size_t)b * n + k) * 3 + c]) : 0.f;
         }
         float sc = ok ? ((k == n - 1) ? 0.f : dd) : 0.f;       // cumsum runs over dd[:-1]
 #pragma unroll
@@ -413,104 +383,40 @@ __global__ void composite_kernel(const float* __restrict__ raw_density, const fl
     }
 }
 
-// ---- tensor-core path helpers: out[m][c] = sum_k fp16 h[m][k] * w[c][k] + b[c]  for tiny N (density: 1, rgb: 3) ----
-// HBM-bound (one pass over the activation rows).  8 lanes per row, 4 rows per warp: every load instruction fetches four whole
-// 128-byte lines; the weights sit in shared memory (fp32, read as broadcast float4); 3 shuffles finish a row.
-constexpr int kRowdotIters = 4;          // row groups per warp: 8 warps x 4 rows x 4 = 128 rows per block
-template <int N>
-__global__ void __launch_bounds__(256) rowdot_f16_kernel(const __half* __restrict__ H, long long ld, int K, const float* __restrict__ Wt,
-                                                         const float* __restrict__ b, long long M, float* __restrict__ out) {
-    extern __shared__ __align__(16) float wsm[];          // [N][K]
-    for (int i = threadIdx.x; i < N * K; i += blockDim.x) wsm[i] = Wt[i];
-    __syncthreads();
-    const int lane = threadIdx.x & 31, sub = lane & 7, rsel = lane >> 3, warp = threadIdx.x >> 5;
-    float bias[N];
-#pragma unroll
-    for (int c = 0; c < N; ++c) bias[c] = b[c];
-#pragma unroll 1
-    for (int it = 0; it < kRowdotIters; ++it) {
-        const long long m = (((long long)blockIdx.x * kRowdotIters + it) * 8 + warp) * 4 + rsel;
-        float acc[N];
-#pragma unroll
-        for (int c = 0; c < N; ++c) acc[c] = 0.f;
-        if (m < M) {
-            const __half* h = H + m * ld;
-            for (int k = sub * 8; k < K; k += 64) {
-                const uint4 v = *reinterpret_cast<const uint4*>(h + k);
-                const __half2* hv = reinterpret_cast<const __half2*>(&v);
-                const float2 f0 = __half22float2(hv[0]), f1 = __half22float2(hv[1]), f2 = __half22float2(hv[2]), f3 = __half22float2(hv[3]);
-#pragma unroll
-                for (int c = 0; c < N; ++c) {
-                    const float4 w0 = *reinterpret_cast<const float4*>(wsm + c * K + k), w1 = *reinterpret_cast<const float4*>(wsm + c * K + k + 4);
-                    acc[c] = fmaf(f0.x, w0.x, fmaf(f0.y, w0.y, fmaf(f1.x, w0.z, fmaf(f1.y, w0.w,
-                             fmaf(f2.x, w1.x, fmaf(f2.y, w1.y, fmaf(f3.x, w1.z, fmaf(f3.y, w1.w, acc[c]))))))));
-                }
-            }
-        }
-#pragma unroll
-        for (int c = 0; c < N; ++c) {
-            acc[c] += __shfl_xor_sync(0xffffffffu, acc[c], 1);
-            acc[c] += __shfl_xor_sync(0xffffffffu, acc[c], 2);
-            acc[c] += __shfl_xor_sync(0xffffffffu, acc[c], 4);
-        }
-        if (m < M && sub == 0) {
-#pragma unroll
-            for (int c = 0; c < N; ++c) out[m * N + c] = acc[c] + bias[c];
-        }
-    }
-}
-
 }  // namespace mip
-int launch_rowdot_f16(const void* H, long long ld, int K, const float* W, const float* b, int N, long long M, float* out, cudaStream_t s) {
-    if (M <= 0) return NEO_OK;
-    if ((K % 8) || (ld % 8) || (N != 1 && N != 3)) { set_error("rowdot_f16: K %% 8, ld %% 8 and N in {1, 3} required (K=%d ld=%lld N=%d)", K, ld, N); return NEO_ERR_INVALID; }
-    if (K <= 0 || ld < K || (size_t)N * K * sizeof(float) > 48 * 1024) { set_error("rowdot_f16: need 0 < K <= ld and N*K*4 <= 48 KB (K=%d ld=%lld N=%d)", K, ld, N); return NEO_ERR_INVALID; }
-    if (!H || !W || !b || !out || (reinterpret_cast<uintptr_t>(H) & 15)) { set_error("rowdot_f16: null pointer or H not 16-byte aligned"); return NEO_ERR_INVALID; }
-    const unsigned grid = (unsigned)((M + 8 * 4 * mip::kRowdotIters - 1) / (8 * 4 * mip::kRowdotIters));
-    const size_t smem = (size_t)N * K * sizeof(float);
-    if (N == 1) mip::rowdot_f16_kernel<1><<<grid, 256, smem, s>>>((const __half*)H, ld, K, W, b, M, out);
-    else mip::rowdot_f16_kernel<3><<<grid, 256, smem, s>>>((const __half*)H, ld, K, W, b, M, out);
-    NEO_LAUNCH_CHECK("rowdot_f16_kernel");
-    return NEO_OK;
-}
-// csrc/gemm_tc.cu
-int gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M, int N, int K,
-             int relu, cudaStream_t s);
-int f32_to_f16_pad(const float* in, long long rows, int cols_in, long long ld_in, void* out, int cols_out, long long ld_out, cudaStream_t s);
 }  // namespace neo
 
 using namespace neo;
 
 namespace {
-struct Cv { float* base; size_t used; float* take(size_t n) { n = (n + 63) & ~size_t(63); float* p = base ? base + used : nullptr; used += n; return p; } };
 struct WSM {
     float *s[3], *t, *w[3], *X, *Ha, *Hb, *beta, *DE, *V, *rawd, *rawc;
     // tensor-core path (fp16): two activation buffers [M][width + 512] whose tail columns hold the padded IPE features of buffer 0,
     // [M][256 + 64] = bottleneck | padded direction encoding, [M][128], and the packed weights
-    void *A16[2], *B16, *V16, *W16;
+    __half *A16[2], *B16, *V16, *W16;
 };
 constexpr int kFeatPad = 512, kDirPad = 64;
 size_t tc_weight_halves(int width) {      // fp16 elements of one MLP's packed weights (upper bound: the 8-layer NeRF MLP)
     return (size_t)width * kFeatPad + 6 * (size_t)width * width + (size_t)width * (width + kFeatPad) + 256 * (size_t)width + 128 * (256 + kDirPad);
 }
-size_t carve(Cv& c, int n, const NeoMipCfg* cfg, int width, WSM& w) {
+size_t carve(Carve& c, int n, const NeoMipCfg* cfg, int width, WSM& w) {
     const int ns[3] = {cfg->n_prop, cfg->n_prop, cfg->n_nerf};
     int nmax = cfg->n_prop > cfg->n_nerf ? cfg->n_prop : cfg->n_nerf;
-    for (int l = 0; l < 3; ++l) { w.s[l] = c.take((size_t)n * (ns[l] + 1)); w.w[l] = c.take((size_t)n * ns[l]); }
-    w.t = c.take((size_t)n * (nmax + 1));
+    for (int l = 0; l < 3; ++l) { w.s[l] = c.take<float>((size_t)n * (ns[l] + 1)); w.w[l] = c.take<float>((size_t)n * ns[l]); }
+    w.t = c.take<float>((size_t)n * (nmax + 1));
     const size_t M = (size_t)n * nmax;
     const bool tcp = cfg->precision == NEO_PREC_TC;          // the fp32 activation buffers are not needed on the tensor-core path
-    w.X = c.take(tcp ? 0 : M * mip::kFeat);
-    w.Ha = c.take(tcp ? 0 : M * width); w.Hb = c.take(tcp ? 0 : M * width);
-    w.beta = c.take(tcp ? 0 : M * 256); w.DE = c.take(tcp ? 0 : M * 27); w.V = c.take(tcp ? 0 : M * 128);
-    w.rawd = c.take(M); w.rawc = c.take(M * 3);
+    w.X = c.take<float>(tcp ? 0 : M * mip::kFeat);
+    w.Ha = c.take<float>(tcp ? 0 : M * width); w.Hb = c.take<float>(tcp ? 0 : M * width);
+    w.beta = c.take<float>(tcp ? 0 : M * 256); w.DE = c.take<float>(tcp ? 0 : M * 27); w.V = c.take<float>(tcp ? 0 : M * 128);
+    w.rawd = c.take<float>(M); w.rawc = c.take<float>(M * 3);
     if (cfg->precision == NEO_PREC_TC) {
-        for (int i = 0; i < 2; ++i) w.A16[i] = c.take((M * (size_t)(width + kFeatPad) + 1) / 2);
-        w.B16 = c.take((M * (256 + kDirPad) + 1) / 2);
-        w.V16 = c.take((M * 128 + 1) / 2);
-        w.W16 = c.take((tc_weight_halves(width) + 1) / 2);
+        for (int i = 0; i < 2; ++i) w.A16[i] = c.take<__half>(M * (size_t)(width + kFeatPad));
+        w.B16 = c.take<__half>(M * (256 + kDirPad));
+        w.V16 = c.take<__half>(M * 128);
+        w.W16 = c.take<__half>(tc_weight_halves(width));
     }
-    return c.used * sizeof(float);
+    return c.used;
 }
 int check(const NeoMipCfg* c) {
     if (!c || c->n_prop < 2 || c->n_nerf < 2 || c->n_prop > 160 || c->n_nerf > 160) { set_error("mip: sample counts must be in [2,160]"); return NEO_ERR_INVALID; }
@@ -530,8 +436,8 @@ int gemm(const float* A1, int K1, const float* A2, int K2, const float* W, const
 int mlp_tc(const NeoMipMLPParams& p, const WSM& w, long long M, int n, const float* viewdirs, float* rawd, float* rawc, cudaStream_t s) {
     const int W = p.width, ld = W + kFeatPad;
     if (W % 64) { set_error("mip tc: width must be a multiple of 64 (got %d)", W); return NEO_ERR_UNSUPPORTED; }
-    __half* buf[2] = {(__half*)w.A16[0], (__half*)w.A16[1]};
-    __half* wp = (__half*)w.W16;
+    __half* buf[2] = {w.A16[0], w.A16[1]};
+    __half* wp = w.W16;
     int rc;
     // the IPE features were written by features_kernel as fp16 into the tail columns of buffer 0 (zero padded to 512)
     auto pack = [&](const float* src, int rows, int cols_in, int cols_out) -> __half* {
@@ -563,14 +469,14 @@ int mlp_tc(const NeoMipMLPParams& p, const WSM& w, long long M, int n, const flo
     const __half* h = buf[(p.depth - 1) & 1];
     if ((rc = launch_rowdot_f16(h, ld, W, p.wsig, p.bsig, 1, M, rawd, s))) return rc;
     if (p.wrgb) {
-        __half* B = (__half*)w.B16;
-        __half* V = (__half*)w.V16;
+        __half* B = w.B16;
+        __half* V = w.V16;
         const int ldb = 256 + kDirPad;
         __half* wb = pack(p.wb, 256, W, W);
         if (!wb) return NEO_ERR_CUDA;
         if ((rc = gemm_f16(h, ld, wb, W, p.bb, B, ldb, M, 256, W, 0, s))) return rc;
-        mip::dir16_kernel<<<(unsigned)((M * kDirPad + 255) / 256), 256, 0, s>>>(viewdirs, M, n, B + 256, ldb, kDirPad);
-        NEO_LAUNCH_CHECK("mip dir16_kernel");
+        mip::dir_kernel<<<(unsigned)((M * kDirPad + 255) / 256), 256, 0, s>>>(viewdirs, M, n, B + 256, ldb, kDirPad);
+        NEO_LAUNCH_CHECK("mip dir_kernel");
         __half* wv = wp;
         wp += (size_t)128 * ldb;
         if ((rc = f32_to_f16_pad(p.wv0, 128, 256, 256 + 27, wv, 256, ldb, s))) return rc;
@@ -582,14 +488,9 @@ int mlp_tc(const NeoMipMLPParams& p, const WSM& w, long long M, int n, const flo
 }
 }  // namespace
 
-// Stage-level entry point of rowdot_f16, the tiny-N head of the vanilla NeRF, Mip-NeRF 360 and encoder paths.
-extern "C" int neo_tc_rowdot_f16(const void* H, long long ld, int K, const float* W, const float* b, int N, long long M, float* out, void* stream) {
-    return neo::launch_rowdot_f16(H, ld, K, W, b, N, M, out, (cudaStream_t)stream);
-}
-
 extern "C" size_t neo_mip_workspace_bytes(int n_rays, const NeoMipCfg* cfg, int nerf_width) {
     if (n_rays <= 0 || check(cfg) || nerf_width < 64) return 0;
-    Cv c{nullptr, 0};
+    Carve c{nullptr, 0};
     WSM w;
     return carve(c, n_rays, cfg, nerf_width > 256 ? nerf_width : 256, w);
 }
@@ -607,7 +508,7 @@ extern "C" int neo_mip_render_fwd(const NeoMipMLPParams mlps[3], const float* ra
     }
     cudaStream_t s = (cudaStream_t)stream;
     const int width = mlps[2].width > 256 ? mlps[2].width : 256;
-    Cv c{reinterpret_cast<float*>(workspace), 0};
+    Carve c{static_cast<unsigned char*>(workspace), 0};
     WSM w;
     size_t need = carve(c, n_rays, cfg, width, w);
     if (!workspace || workspace_bytes < need) { set_error("workspace too small: need %zu bytes, got %zu", need, workspace_bytes); return NEO_ERR_WORKSPACE; }
@@ -630,7 +531,7 @@ extern "C" int neo_mip_render_fwd(const NeoMipMLPParams mlps[3], const float* ra
         const long long M = (long long)n_rays * n;
         const bool tcp = cfg->precision == NEO_PREC_TC;
         if (tcp) mip::features16_kernel<<<(unsigned)((M + mip::kFeatSamples - 1) / mip::kFeatSamples), mip::kFeatThreads, 0, s>>>(
-                     rays_o, rays_d, radii, w.t, mlps[lvl].basis, M, n, (__half*)w.A16[0] + mlps[lvl].width, mlps[lvl].width + kFeatPad);
+                     rays_o, rays_d, radii, w.t, mlps[lvl].basis, M, n, w.A16[0] + mlps[lvl].width, mlps[lvl].width + kFeatPad);
         else mip::features_kernel<<<(unsigned)((M + 7) / 8), 256, 0, s>>>(rays_o, rays_d, radii, w.t, mlps[lvl].basis, M, n, w.X);
         NEO_LAUNCH_CHECK("mip features_kernel");
         const NeoMipMLPParams& p = mlps[lvl];
@@ -651,7 +552,7 @@ extern "C" int neo_mip_render_fwd(const NeoMipMLPParams mlps[3], const float* ra
             if ((rc = gemm(src, p.width, nullptr, 0, p.wsig, p.bsig, M, 1, 0, w.rawd, s))) return rc;
                     if (p.wrgb) {
                 if ((rc = gemm(src, p.width, nullptr, 0, p.wb, p.bb, M, 256, 0, w.beta, s))) return rc;
-                mip::dir_kernel<<<(unsigned)((M * 27 + 255) / 256), 256, 0, s>>>(viewdirs, M, n, w.DE);
+                mip::dir_kernel<<<(unsigned)((M * 27 + 255) / 256), 256, 0, s>>>(viewdirs, M, n, w.DE, 27, 27);
                 NEO_LAUNCH_CHECK("mip dir_kernel");
                 if ((rc = gemm(w.beta, 256, w.DE, 27, p.wv0, p.bv0, M, 128, 1, w.V, s))) return rc;
                 if ((rc = gemm(w.V, 128, nullptr, 0, p.wrgb, p.brgb, M, 3, 0, w.rawc, s))) return rc;
@@ -664,8 +565,8 @@ extern "C" int neo_mip_render_fwd(const NeoMipMLPParams mlps[3], const float* ra
         mip::composite_kernel<<<(n_rays + cw - 1) / cw, cw * 32, 0, s>>>(w.rawd, rawc, w.t, rays_d, n_rays, n, out->density[lvl],
                                                                         rawc ? out->rgb_s[lvl] : nullptr, w.w[lvl], out->rgb[lvl]);
         NEO_LAUNCH_CHECK("mip composite_kernel");
-        if (out->sdist[lvl]) NEO_CUDA(cudaMemcpyAsync(out->sdist[lvl], w.s[lvl], (size_t)n_rays * (n + 1) * sizeof(float), cudaMemcpyDeviceToDevice, s));
-        if (out->weights[lvl]) NEO_CUDA(cudaMemcpyAsync(out->weights[lvl], w.w[lvl], (size_t)M * sizeof(float), cudaMemcpyDeviceToDevice, s));
+        if ((rc = copy_out(out->sdist[lvl], w.s[lvl], (size_t)n_rays * (n + 1), s))) return rc;
+        if ((rc = copy_out(out->weights[lvl], w.w[lvl], (size_t)M, s))) return rc;
     }
     return NEO_OK;
 }

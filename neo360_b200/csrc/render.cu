@@ -7,37 +7,26 @@ using namespace neo;
 
 namespace {
 
-struct Carver {
-    float* base;
-    size_t used, cap;
-    float* take(size_t n) {
-        n = (n + 63) & ~size_t(63);          // 256-byte granules
-        float* p = base ? base + used : nullptr;
-        used += n;
-        return p;
-    }
-};
-
 struct WS {
     float *far, *t0[2], *w0[2], *t1[2], *w1[2], *sig[2], *rgb[2];
     float *c[2], *acc[2], *lam, *dep[2];
 };
 
-size_t carve(Carver& cv, int n, int N0, int N1, WS& w) {
-    w.far = cv.take(n);
+size_t carve(Carve& cv, int n, int N0, int N1, WS& w) {
+    w.far = cv.take<float>(n);
     for (int b = 0; b < 2; ++b) {
-        w.t0[b] = cv.take((size_t)n * N0);
-        w.w0[b] = cv.take((size_t)n * N0);
-        w.t1[b] = cv.take((size_t)n * N1);
-        w.w1[b] = cv.take((size_t)n * N1);
-        w.sig[b] = cv.take((size_t)n * N1);
-        w.rgb[b] = cv.take((size_t)n * N1 * 3);
-        w.c[b] = cv.take((size_t)n * 3);
-        w.acc[b] = cv.take(n);
-        w.dep[b] = cv.take(n);
+        w.t0[b] = cv.take<float>((size_t)n * N0);
+        w.w0[b] = cv.take<float>((size_t)n * N0);
+        w.t1[b] = cv.take<float>((size_t)n * N1);
+        w.w1[b] = cv.take<float>((size_t)n * N1);
+        w.sig[b] = cv.take<float>((size_t)n * N1);
+        w.rgb[b] = cv.take<float>((size_t)n * N1 * 3);
+        w.c[b] = cv.take<float>((size_t)n * 3);
+        w.acc[b] = cv.take<float>(n);
+        w.dep[b] = cv.take<float>(n);
     }
-    w.lam = cv.take(n);
-    return cv.used * sizeof(float);
+    w.lam = cv.take<float>(n);
+    return cv.used;
 }
 
 int check_cfg(const NeoCfg* cfg) {
@@ -82,17 +71,11 @@ int field(const NeoScene* sc, const NeoRays* rays, const float* far, const float
     return rc;
 }
 
-int copy_out(float* dst, const float* src, size_t n, cudaStream_t s) {
-    if (!dst || dst == src) return NEO_OK;
-    NEO_CUDA(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, s));
-    return NEO_OK;
-}
-
 }  // namespace
 
 extern "C" size_t neo_render_workspace_bytes(int n_rays, const NeoCfg* cfg) {
     if (n_rays <= 0 || check_cfg(cfg)) return 0;
-    Carver cv{nullptr, 0, 0};
+    Carve cv{nullptr, 0};
     WS w;
     return carve(cv, n_rays, cfg->n_coarse + 1, cfg->n_coarse + 1 + cfg->n_fine, w);
 }
@@ -106,7 +89,7 @@ extern "C" int neo_render_fwd(const NeoScene* sc, const NeoRays* rays, const Neo
     if (!(sc->precision_mask & (1 << cfg->precision))) { set_error("scene not prepared for precision %d", cfg->precision); return NEO_ERR_INVALID; }
     cudaStream_t s = (cudaStream_t)stream;
     const int n = rays->n_rays, N0 = cfg->n_coarse + 1, N1 = N0 + cfg->n_fine;
-    Carver cv{reinterpret_cast<float*>(workspace), 0, 0};
+    Carve cv{static_cast<unsigned char*>(workspace), 0};
     WS w;
     size_t need = carve(cv, n, N0, N1, w);
     if (!workspace || workspace_bytes < need) { set_error("workspace too small: need %zu bytes, got %zu", need, workspace_bytes); return NEO_ERR_WORKSPACE; }

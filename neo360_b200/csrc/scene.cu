@@ -26,12 +26,13 @@ int cuda_fail(cudaError_t e, const char* what) {
 const char* last_error() { return g_err; }
 
 // (n, C, HW) -> (n, HW, C), tiled through shared memory so both sides are coalesced
-__global__ void nchw_to_nhwc_kernel(const float* __restrict__ in, float* __restrict__ out, int C, int HW) {
+template <class T>
+__global__ void nchw_to_nhwc_kernel(const float* __restrict__ in, T* __restrict__ out, int C, int HW) {
     __shared__ float tile[32][33];
     int n = blockIdx.z;
     int c0 = blockIdx.y * 32, p0 = blockIdx.x * 32;
     const float* src = in + (size_t)n * C * HW;
-    float* dst = out + (size_t)n * C * HW;
+    T* dst = out + (size_t)n * C * HW;
     for (int i = threadIdx.y; i < 32; i += blockDim.y) {
         int c = c0 + i, p = p0 + threadIdx.x;
         if (c < C && p < HW) tile[i][threadIdx.x] = src[(size_t)c * HW + p];
@@ -39,9 +40,19 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ in, float* __restr
     __syncthreads();
     for (int i = threadIdx.y; i < 32; i += blockDim.y) {
         int p = p0 + i, c = c0 + threadIdx.x;
-        if (c < C && p < HW) dst[(size_t)p * C + c] = tile[threadIdx.x][i];
+        if (c < C && p < HW) dst[(size_t)p * C + c] = from_f32<T>(tile[threadIdx.x][i]);
     }
 }
+
+template <class T>
+static int nchw_to_nhwc(const float* in, T* out, int n, int C, int HW, cudaStream_t s) {
+    dim3 grid((HW + 31) / 32, (C + 31) / 32, n), block(32, 8);
+    nchw_to_nhwc_kernel<T><<<grid, block, 0, s>>>(in, out, C, HW);
+    NEO_LAUNCH_CHECK("nchw_to_nhwc_kernel");
+    return NEO_OK;
+}
+int launch_nchw_to_nhwc(const float* in, float* out, int n, int C, int HW, cudaStream_t s) { return nchw_to_nhwc(in, out, n, C, HW, s); }
+int launch_nchw_to_nhwc(const float* in, __half* out, int n, int C, int HW, cudaStream_t s) { return nchw_to_nhwc(in, out, n, C, HW, s); }
 
 // (out,in) -> (in,out)
 __global__ void transpose_kernel(const float* __restrict__ w, float* __restrict__ wt, int out_f, int in_f) {
@@ -49,6 +60,13 @@ __global__ void transpose_kernel(const float* __restrict__ w, float* __restrict_
     if (idx >= out_f * in_f) return;
     int o = idx / in_f, i = idx % in_f;
     wt[(size_t)i * out_f + o] = w[idx];
+}
+
+int launch_transpose(const float* w, float* wt, int out_f, int in_f, cudaStream_t s) {
+    int n = out_f * in_f;
+    transpose_kernel<<<(n + 255) / 256, 256, 0, s>>>(w, wt, out_f, in_f);
+    NEO_LAUNCH_CHECK("transpose_kernel");
+    return NEO_OK;
 }
 
 __global__ void view_xform_kernel(const float* __restrict__ poses, int nv, ViewXform* __restrict__ out) {
@@ -142,10 +160,7 @@ int scene_alloc_bytes(NeoScene* sc, void** p, size_t bytes) {
 static int transpose_to(NeoScene* sc, const float* w, int out_f, int in_f, const float** dst, cudaStream_t s) {
     float* t = nullptr;
     int rc = dev_alloc(sc, &t, (size_t)out_f * in_f);
-    if (rc) return rc;
-    int n = out_f * in_f;
-    transpose_kernel<<<(n + 255) / 256, 256, 0, s>>>(w, t, out_f, in_f);
-    NEO_LAUNCH_CHECK("transpose_kernel");
+    if (rc || (rc = launch_transpose(w, t, out_f, in_f, s))) return rc;
     *dst = t;
     return NEO_OK;
 }
@@ -153,10 +168,7 @@ static int transpose_to(NeoScene* sc, const float* w, int out_f, int in_f, const
 static int to_channel_last(NeoScene* sc, const float* src, int n, int C, int HW, const float** dst, cudaStream_t s) {
     float* t = nullptr;
     int rc = dev_alloc(sc, &t, (size_t)n * C * HW);
-    if (rc) return rc;
-    dim3 grid((HW + 31) / 32, (C + 31) / 32, n), block(32, 8);
-    nchw_to_nhwc_kernel<<<grid, block, 0, s>>>(src, t, C, HW);
-    NEO_LAUNCH_CHECK("nchw_to_nhwc_kernel");
+    if (rc || (rc = launch_nchw_to_nhwc(src, t, n, C, HW, s))) return rc;
     *dst = t;
     return NEO_OK;
 }

@@ -40,25 +40,6 @@ __global__ void sample_kernel(const float* __restrict__ o, const float* __restri
     t_out[gid] = t;
 }
 
-template <int ROWS>
-__device__ __forceinline__ void dense(const float* __restrict__ Wt, int ldw, int K, const float* __restrict__ A, int lda, float* acc, int j) {
-    int k = 0;
-    for (; k + 4 <= K; k += 4) {
-        float w0 = __ldg(Wt + (size_t)(k + 0) * ldw + j), w1 = __ldg(Wt + (size_t)(k + 1) * ldw + j);
-        float w2 = __ldg(Wt + (size_t)(k + 2) * ldw + j), w3 = __ldg(Wt + (size_t)(k + 3) * ldw + j);
-#pragma unroll
-        for (int r = 0; r < ROWS; ++r) {
-            float4 a = *reinterpret_cast<const float4*>(A + r * lda + k);
-            acc[r] = fmaf(a.w, w3, fmaf(a.z, w2, fmaf(a.y, w1, fmaf(a.x, w0, acc[r]))));
-        }
-    }
-    for (; k < K; ++k) {
-        float w0 = __ldg(Wt + (size_t)k * ldw + j);
-#pragma unroll
-        for (int r = 0; r < ROWS; ++r) acc[r] = fmaf(A[r * lda + k], w0, acc[r]);
-    }
-}
-
 __global__ void __launch_bounds__(kThreads) field_kernel(NeoVanilla::Mlp m, const float* __restrict__ rays_o,
                                                          const float* __restrict__ viewdirs, const float* __restrict__ tvals,
                                                          int n_rays, int N, float* __restrict__ rgb_out, float* __restrict__ sigma_out) {
@@ -79,31 +60,12 @@ __global__ void __launch_bounds__(kThreads) field_kernel(NeoVanilla::Mlp m, cons
     __syncthreads();
     for (int e = j; e < kP * 64; e += kThreads) {
         int p = e / 64, c = e % 64;
-        float val = 0.f;
-        if (c < 3) val = xp[p][c];
-        else if (c < kEnc) {
-            int q = c - 3;
-            bool shifted = q >= 30;
-            if (shifted) q -= 30;
-            float xb = mul_(xp[p][q % 3], (float)(1 << (q / 3)));
-            val = sinf(shifted ? add_(xb, 1.57079637f) : xb);
-        }
-        X[p][c] = val;
+        X[p][c] = c < kEnc ? pos_enc_col(xp[p], 3, 10, c) : 0.f;
     }
     for (int e = j; e < kP * 28; e += kThreads) {
         int p = e / 28, c = e % 28;
         long long gp = min(tile0 + p, total - 1);
-        const float* d = viewdirs + 3 * (gp / N);
-        float val = 0.f;
-        if (c < 3) val = d[c];
-        else if (c < kDirEnc) {
-            int q = c - 3;
-            bool shifted = q >= 12;
-            if (shifted) q -= 12;
-            float xb = mul_(d[q % 3], (float)(1 << (q / 3)));
-            val = sinf(shifted ? add_(xb, 1.57079637f) : xb);
-        }
-        Dn[p][c] = val;
+        Dn[p][c] = c < kDirEnc ? pos_enc_col(viewdirs + 3 * (gp / N), 3, 4, c) : 0.f;
     }
     __syncthreads();
     float acc[kP];
@@ -112,11 +74,11 @@ __global__ void __launch_bounds__(kThreads) field_kernel(NeoVanilla::Mlp m, cons
     float (*src)[kW + 4] = Ha;
     float (*dst)[kW + 4] = Hb;
     // layer 0
-    init(m.b[0]); dense<kP>(m.wt[0], kW, kEnc, &X[0][0], 64, acc, j); relu_to(Ha); __syncthreads();
+    init(m.b[0]); dense_rows<kP>(m.wt[0], kW, kEnc, &X[0][0], 64, acc, j); relu_to(Ha); __syncthreads();
     for (int l = 1; l < 8; ++l) {
         init(m.b[l]);
-        dense<kP>(m.wt[l], kW, kW, &src[0][0], kW + 4, acc, j);
-        if (l == 5) dense<kP>(m.wt[l] + (size_t)kW * kW, kW, kEnc, &X[0][0], 64, acc, j);      // cat([h, inputs]) after layer 4
+        dense_rows<kP>(m.wt[l], kW, kW, &src[0][0], kW + 4, acc, j);
+        if (l == 5) dense_rows<kP>(m.wt[l] + (size_t)kW * kW, kW, kEnc, &X[0][0], 64, acc, j);      // cat([h, inputs]) after layer 4
         relu_to(dst);
         __syncthreads();
         float (*tmp)[kW + 4] = src; src = dst; dst = tmp;
@@ -130,7 +92,7 @@ __global__ void __launch_bounds__(kThreads) field_kernel(NeoVanilla::Mlp m, cons
         }
     }
     // bottleneck -> dst
-    init(m.bb); dense<kP>(m.wbt, kW, kW, &src[0][0], kW + 4, acc, j);
+    init(m.bb); dense_rows<kP>(m.wbt, kW, kW, &src[0][0], kW + 4, acc, j);
     for (int r = 0; r < kP; ++r) dst[r][j] = acc[r];
     __syncthreads();
     if (j < kP) {
@@ -138,8 +100,7 @@ __global__ void __launch_bounds__(kThreads) field_kernel(NeoVanilla::Mlp m, cons
         if (gp < total) {
             float raw = __ldg(m.bsig);
             for (int w = 0; w < 8; ++w) raw += red[w][j];
-            float xs = raw - 1.0f;
-            sigma_out[gp] = xs > 20.f ? xs : log1pf(expf(xs));
+            sigma_out[gp] = softplus_(raw - 1.0f);
         }
     }
     // view branch: [bottleneck | dir_enc] -> 128 relu  (result into src rows, first 128 columns)
@@ -147,8 +108,8 @@ __global__ void __launch_bounds__(kThreads) field_kernel(NeoVanilla::Mlp m, cons
     if (j < kCond) {
         float v = __ldg(m.bv0 + j);
         for (int r = 0; r < kP; ++r) a2[r] = v;
-        dense<kP>(m.wv0t, kCond, kW, &dst[0][0], kW + 4, a2, j);
-        dense<kP>(m.wv0t + (size_t)kW * kCond, kCond, kDirEnc, &Dn[0][0], 28, a2, j);
+        dense_rows<kP>(m.wv0t, kCond, kW, &dst[0][0], kW + 4, a2, j);
+        dense_rows<kP>(m.wv0t + (size_t)kW * kCond, kCond, kDirEnc, &Dn[0][0], 28, a2, j);
     }
     __syncthreads();
     if (j < kCond) for (int r = 0; r < kP; ++r) src[r][j] = fmaxf(a2[r], 0.f);
@@ -159,7 +120,7 @@ __global__ void __launch_bounds__(kThreads) field_kernel(NeoVanilla::Mlp m, cons
         if (gp < total) {
             float a = __ldg(m.brgb + c);
             for (int k = 0; k < kCond; ++k) a = fmaf(src[p][k], __ldg(m.wrgb + c * kCond + k), a);
-            rgb_out[gp * 3 + c] = (1.f / (1.f + expf(-a))) * 1.002f - 0.001f;
+            rgb_out[gp * 3 + c] = rgb_act(a);
         }
     }
 }
@@ -239,40 +200,29 @@ __global__ void head_act_kernel(const float* __restrict__ raw_sigma, const float
     if (i >= M * 4) return;
     const long long m = i >> 2;
     const int c = (int)(i & 3);
-    if (c == 3) { const float xs = raw_sigma[m] - 1.0f; sigma[m] = xs > 20.f ? xs : log1pf(expf(xs)); }
-    else rgb[m * 3 + c] = (1.f / (1.f + expf(-raw_rgb[m * 3 + c]))) * 1.002f - 0.001f;
+    if (c == 3) sigma[m] = softplus_(raw_sigma[m] - 1.0f);
+    else rgb[m * 3 + c] = rgb_act(raw_rgb[m * 3 + c]);
 }
 
 }  // namespace van
-// csrc/gemm_tc.cu, csrc/mip.cu
-int gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M, int N, int K,
-             int relu, cudaStream_t s);
-int f32_to_f16_pad(const float* in, long long rows, int cols_in, long long ld_in, void* out, int cols_out, long long ld_out, cudaStream_t s);
-int launch_rowdot_f16(const void* H, long long ld, int K, const float* W, const float* b, int N, long long M, float* out, cudaStream_t s);
 }  // namespace neo
 
 using namespace neo;
 
 namespace {
-__global__ void transpose2(const float* __restrict__ w, float* __restrict__ wt, int out_f, int in_f) {
-    int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= out_f * in_f) return;
-    wt[(size_t)(idx % in_f) * out_f + idx / in_f] = w[idx];
-}
-struct Carver2 { float* base; size_t used; float* take(size_t n) { n = (n + 63) & ~size_t(63); float* p = base ? base + used : nullptr; used += n; return p; } };
-struct WSV { float *t0, *w0, *t1, *w1, *sig, *rgb; void *A16[2], *B16, *V16; float *rawd, *rawc; };
+struct WSV { float *t0, *w0, *t1, *w1, *sig, *rgb; __half *A16[2], *B16, *V16; float *rawd, *rawc; };
 constexpr int kLdA = 256 + 64, kLdB = 256 + 64;      // activation rows: [h (256) | padded encoding (64)], [bottleneck (256) | padded direction encoding (64)]
-size_t carve2(Carver2& c, int n, int N0, int N1, WSV& w, int precision) {
-    w.t0 = c.take((size_t)n * N0); w.w0 = c.take((size_t)n * N0); w.t1 = c.take((size_t)n * N1); w.w1 = c.take((size_t)n * N1);
-    w.sig = c.take((size_t)n * N1); w.rgb = c.take((size_t)n * N1 * 3);
+size_t carve(Carve& c, int n, int N0, int N1, WSV& w, int precision) {
+    w.t0 = c.take<float>((size_t)n * N0); w.w0 = c.take<float>((size_t)n * N0); w.t1 = c.take<float>((size_t)n * N1); w.w1 = c.take<float>((size_t)n * N1);
+    w.sig = c.take<float>((size_t)n * N1); w.rgb = c.take<float>((size_t)n * N1 * 3);
     if (precision == NEO_PREC_TC) {
         const size_t M = (size_t)n * N1;
-        for (int i = 0; i < 2; ++i) w.A16[i] = c.take((M * kLdA + 1) / 2);
-        w.B16 = c.take((M * kLdB + 1) / 2);
-        w.V16 = c.take((M * 128 + 1) / 2);
-        w.rawd = c.take(M); w.rawc = c.take(M * 3);
+        for (int i = 0; i < 2; ++i) w.A16[i] = c.take<__half>(M * kLdA);
+        w.B16 = c.take<__half>(M * kLdB);
+        w.V16 = c.take<__half>(M * 128);
+        w.rawd = c.take<float>(M); w.rawc = c.take<float>(M * 3);
     }
-    return c.used * sizeof(float);
+    return c.used;
 }
 int check(const NeoVanillaCfg* c) {
     if (!c || c->n_coarse < 3 || c->n_fine < 1 || c->n_coarse > 4096 || c->n_fine > 4096) { set_error("vanilla: bad sample counts"); return NEO_ERR_INVALID; }
@@ -293,10 +243,8 @@ extern "C" int neo_vanilla_create(const NeoVanillaMLPParams mlps[2], NeoVanilla*
         if (e != cudaSuccess) return cuda_fail(e, "cudaMalloc(vanilla)");
         v->allocations.push_back(q);
         v->bytes += n * sizeof(float);
-        if (out_f > 0) transpose2<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(src, (float*)q, out_f, in_f);
-        else { e = cudaMemcpyAsync(q, src, n * sizeof(float), cudaMemcpyDeviceToDevice, s); if (e != cudaSuccess) return cuda_fail(e, "copy"); }
         *dst = (const float*)q;
-        return NEO_OK;
+        return out_f > 0 ? launch_transpose(src, (float*)q, out_f, in_f, s) : copy_out((float*)q, src, n, s);
     };
     for (int i = 0; i < 2; ++i) {
         const NeoVanillaMLPParams& p = mlps[i];
@@ -356,9 +304,9 @@ extern "C" void neo_vanilla_free(NeoVanilla* v) {
 
 extern "C" size_t neo_vanilla_workspace_bytes(int n_rays, const NeoVanillaCfg* cfg) {
     if (n_rays <= 0 || check(cfg)) return 0;
-    Carver2 c{nullptr, 0};
+    Carve c{nullptr, 0};
     WSV w;
-    return carve2(c, n_rays, cfg->n_coarse + 1, cfg->n_coarse + 1 + cfg->n_fine, w, cfg->precision);
+    return carve(c, n_rays, cfg->n_coarse + 1, cfg->n_coarse + 1 + cfg->n_fine, w, cfg->precision);
 }
 
 extern "C" int neo_vanilla_render_fwd(const NeoVanilla* v, const NeoRays* rays, const NeoVanillaCfg* cfg, NeoVanillaOut* out,
@@ -369,9 +317,9 @@ extern "C" int neo_vanilla_render_fwd(const NeoVanilla* v, const NeoRays* rays, 
     if (rays->n_rays <= 0 || !rays->rays_o || !rays->rays_d || !rays->viewdirs) { set_error("neo_vanilla_render_fwd: empty rays"); return NEO_ERR_INVALID; }
     cudaStream_t s = (cudaStream_t)stream;
     const int n = rays->n_rays, N0 = cfg->n_coarse + 1, N1 = N0 + cfg->n_fine;
-    Carver2 c{reinterpret_cast<float*>(workspace), 0};
+    Carve c{static_cast<unsigned char*>(workspace), 0};
     WSV w;
-    size_t need = carve2(c, n, N0, N1, w, cfg->precision);
+    size_t need = carve(c, n, N0, N1, w, cfg->precision);
     if (!workspace || workspace_bytes < need) { set_error("workspace too small: need %zu bytes, got %zu", need, workspace_bytes); return NEO_ERR_WORKSPACE; }
     for (int lvl = 0; lvl < 2; ++lvl) {
         const int N = lvl ? N1 : N0;
@@ -391,8 +339,8 @@ extern "C" int neo_vanilla_render_fwd(const NeoVanilla* v, const NeoRays* rays, 
             // NeRFMLP (models/vanilla_nerf/model.py:44-125) layer by layer on the tensor cores (csrc/gemm_tc.cu), fp16 activations; the skip concatenation
             // by keeping h4 and the encoding in ONE buffer (layer 5 is a single K = 320 GEMM)
             const NeoVanilla::Mlp& m = v->mlp[lvl];
-            __half* buf[2] = {(__half*)w.A16[0], (__half*)w.A16[1]};
-            __half* B = (__half*)w.B16;
+            __half* buf[2] = {w.A16[0], w.A16[1]};
+            __half* B = w.B16;
             van::enc16_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(rays->rays_o, rays->viewdirs, t, total, N, buf[0] + 256, kLdA, B + 256, kLdB);
             NEO_LAUNCH_CHECK("vanilla enc16_kernel");
             if ((rc = gemm_f16(buf[0] + 256, kLdA, m.w16[0], 64, m.b[0], buf[0], kLdA, total, 256, 64, 1, s))) return rc;
@@ -415,15 +363,10 @@ extern "C" int neo_vanilla_render_fwd(const NeoVanilla* v, const NeoRays* rays, 
         // mode 2: ascending t, last interval 1e10, scaled by |rays_d|, depth nan_to_num(inf)
         if ((rc = launch_composite(w.rgb, w.sig, t, rays->rays_d, nullptr, n, N, cfg->white_bkgd, 2, out->comp_rgb[lvl], out->acc[lvl], wt, nullptr,
                                    out->depth[lvl], s))) return rc;
-        auto cp = [&](float* dst, const float* src, size_t cnt) -> int {
-            if (!dst) return NEO_OK;
-            NEO_CUDA(cudaMemcpyAsync(dst, src, cnt * sizeof(float), cudaMemcpyDeviceToDevice, s));
-            return NEO_OK;
-        };
-        if ((rc = cp(out->t[lvl], t, (size_t)n * N))) return rc;
-        if ((rc = cp(out->sigma[lvl], w.sig, (size_t)n * N))) return rc;
-        if ((rc = cp(out->rgb_s[lvl], w.rgb, (size_t)n * N * 3))) return rc;
-        if ((rc = cp(out->weights[lvl], wt, (size_t)n * N))) return rc;
+        if ((rc = copy_out(out->t[lvl], t, (size_t)n * N, s))) return rc;
+        if ((rc = copy_out(out->sigma[lvl], w.sig, (size_t)n * N, s))) return rc;
+        if ((rc = copy_out(out->rgb_s[lvl], w.rgb, (size_t)n * N * 3, s))) return rc;
+        if ((rc = copy_out(out->weights[lvl], wt, (size_t)n * N, s))) return rc;
     }
     return NEO_OK;
 }

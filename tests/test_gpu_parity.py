@@ -651,29 +651,6 @@ def test_output_side_psnr_and_frames(cuda, tmp_path):
     assert all(os.path.getsize(p) > 0 for p in paths)
 
 
-@pytest.mark.parametrize("M,N,K,relu", [(1000, 1024, 512, 1), (257, 256, 1536, 1), (4096, 128, 320, 1), (130, 64, 64, 0), (70000, 1024, 1024, 1),
-                                          (20001, 256, 128, 0), (19000, 512, 1536, 1), (40000, 256, 256, 1), (19000, 256, 64, 1)])
-def test_tc_dense_vs_torch(cuda, M, N, K, relu):
-    """The fp32 wrapper neo_tc_dense (fp32 -> fp16 staging, gemm_f16, fp16 -> fp32) against a plain PyTorch fp32 reference of the same
-    op on the fp16-rounded operands, ragged M, N = 64 (BN = 64 tiles) and multiples of 128, K up to 1536.  Stated: |err| <= 2e-3 *
-    max|ref| (fp32 accumulation order + the fp16 rounding of the output).  gemm_f16 itself is held to an element-wise bound at its
-    callers' strides and aliasing in test_gpu_tc_kernels.py."""
-    from neo360_b200 import _lib as L
-    lib = L.load()
-    g = torch.Generator().manual_seed(M + N + K)
-    A = torch.randn(M, K, generator=g).to(cuda)
-    W = (torch.randn(N, K, generator=g) / K ** 0.5).to(cuda)
-    b = torch.randn(N, generator=g).to(cuda)
-    out = torch.empty(M, N, device=cuda)
-    L.check(lib.neo_tc_dense(L.ptr(A), L.ptr(W), L.ptr(b), M, N, K, relu, L.ptr(out), torch.cuda.current_stream().cuda_stream))
-    ref = A.half().float() @ W.half().float().T + b
-    if relu:
-        ref = torch.relu(ref)
-    err = float((out - ref).abs().max())
-    print(f"tc dense {M}x{N}x{K}: max err {err:.3e}, max ref {float(ref.abs().max()):.3f}")
-    assert err <= 2e-3 * float(ref.abs().max())
-
-
 def test_scene_cache_is_keyed_by_identity_and_parameter_version(cuda):
     """ADVICE round 1: (1) a new scene whose tensors the caching allocator placed at the SAME addresses as the freed previous scene must
     not be rendered with the previous scene's packed maps; (2) a parameter update after the first render must be picked up (the scene
