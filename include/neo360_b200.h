@@ -255,6 +255,24 @@ size_t neo_vanilla_workspace_bytes(int n_rays, const NeoVanillaCfg* cfg);
 /* NeRF.forward (models/vanilla_nerf/model.py:154-216); rays->chunk is ignored (no cross-ray coupling in this model) */
 int neo_vanilla_render_fwd(const NeoVanilla* v, const NeoRays* rays, const NeoVanillaCfg* cfg, NeoVanillaOut* out,
                            void* workspace, size_t workspace_bytes, void* stream);
+/* Stages of the differentiable NeRF.forward (training, models/vanilla_nerf/model.py:154-216 under autograd; neo360_b200/vanilla.py).
+ * Hand-written: sampling, encodings, compositing forward and backward; the NeRFMLP dense layers are differentiated by the host framework.
+ * The fine level resamples with neo_sample_pdf(rays_o, viewdirs, NULL, t0, weights0, n, n_coarse+1, n_fine, 1, 0, u1, t1, NULL, NULL)
+ * and composites forward with neo_volumetric_rendering(..., in_sphere = 2, ...), the calls neo_vanilla_render_fwd makes. */
+/* helper.py:415-442 along viewdirs (quirk Q15): t_vals (n_rays, n_coarse+1); u_rand (n_rays, n_coarse+1) or NULL = deterministic.
+ * The same kernel as neo_vanilla_render_fwd's level 0: bit-identical t. */
+int neo_vanilla_sample_along_rays(const float* rays_o, const float* viewdirs, int n_rays, int n_coarse, float near_plane, float far_plane,
+                                  const float* u_rand, float* t_vals, void* stream);
+/* fp32 positional encodings (helper.py:445-449 column order) of the points o + t viewdirs: enc (n_rays*N, 63), and of the view
+ * directions: dir_enc (n_rays, 27).  The same arithmetic as the NEO_PREC_FP32 field kernel (bit-identical).  No backward. */
+int neo_vanilla_encode(const float* rays_o, const float* viewdirs, const float* t_vals, int n_rays, int N, float* enc, float* dir_enc,
+                       void* stream);
+/* Backward of neo_volumetric_rendering in mode 2 (helper.py:521-559): upstream gradients of comp_rgb (n,3), acc (n), weights (n,N),
+ * depth (n) -- any may be NULL -- -> d_rgb (n,N,3), d_sigma (n,N).  The depth gradient passes where sum w t was finite (nan_to_num +
+ * clamp, quirk Q10) and is zero elsewhere.  Same rgb / sigma / t / rays_d as the forward call. */
+int neo_vanilla_composite_bwd(const float* rgb, const float* sigma, const float* t_vals, const float* rays_d, int n_rays, int N, int white_bkgd,
+                              const float* g_comp_rgb, const float* g_acc, const float* g_weights, const float* g_depth, float* d_rgb,
+                              float* d_sigma, void* stream);
 
 /* ---- Mip-NeRF 360 (SURVEY.md section 8(a) row a18): models/mipnerf360/model.py:30-365 ---- */
 typedef struct {

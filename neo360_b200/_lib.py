@@ -114,6 +114,9 @@ SYMBOLS = {
     "neo_vanilla_free": (None, [C.c_void_p]),
     "neo_vanilla_workspace_bytes": (C.c_size_t, [C.c_int, C.POINTER(NeoVanillaCfg)]),
     "neo_vanilla_render_fwd": (C.c_int, [C.c_void_p, C.POINTER(NeoRays), C.POINTER(NeoVanillaCfg), C.POINTER(NeoVanillaOut), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "neo_vanilla_sample_along_rays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "neo_vanilla_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "neo_vanilla_composite_bwd": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 3 + [C.c_void_p] * 7),
     "neo_mip_workspace_bytes": (C.c_size_t, [C.c_int, C.POINTER(NeoMipCfg), C.c_int]),
     "neo_mip_render_fwd": (C.c_int, [C.POINTER(NeoMipMLPParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(NeoMipCfg),
                                      C.POINTER(NeoMipOut), C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -409,6 +409,9 @@ int launch_composite(const float* rgb, const float* sigma, const float* t, const
 //   backward : G_i = g_comp.c_i + g_w_i + g_acc + g_depth t_i - white * sum(g_comp)        (dL/dw_i)
 //              S_i = sum_{j>i} G_j w_j + g_lam T_N                                          (everything downstream of factor a_i)
 //              dL/dalpha_i = G_i T_i - S_i / a_i ,   dL/dsigma_i = dL/dalpha_i * delta_i (1 - alpha_i) ,   dL/dc_i = w_i g_comp
+// in_sphere 2 (vanilla NeRF, entry point neo_vanilla_composite_bwd): ascending t, last interval 1e10, every interval times |d|, no far and
+// no g_lam; the forward's depth is nan_to_num(sum w t, inf) clamped to its own chunk-wide min / max (quirk Q10), whose gradient passes
+// where sum w t is finite and is zero where it was substituted.
 // ------------------------------------------------------------------------------------------------
 __global__ void composite_bwd_kernel(const float* __restrict__ rgb, const float* __restrict__ sigma, const float* __restrict__ t,
                                      const float* __restrict__ d, const float* __restrict__ far, int n, int N, int white, int in_sphere,
@@ -426,21 +429,23 @@ __global__ void composite_bwd_kernel(const float* __restrict__ rgb, const float*
     if (in_sphere) {
         const float* dd = d + 3 * b;
         dn = __fsqrt_rn(dot3_(dd, dd));
-        fr = far[b];
+        if (in_sphere == 1) fr = far[b];
     }
     auto dist_of = [&](int k) -> float {
-        if (in_sphere) return mul_(sub_((k + 1 < N) ? tb[k + 1] : fr, tb[k]), dn);
+        if (in_sphere == 1) return mul_(sub_((k + 1 < N) ? tb[k + 1] : fr, tb[k]), dn);
+        if (in_sphere == 2) return mul_((k + 1 < N) ? sub_(tb[k + 1], tb[k]) : 1e10f, dn);
         return (k + 1 < N) ? sub_(tb[k], tb[k + 1]) : 1e10f;
     };
-    float T = 1.f;
+    float T = 1.f, dep = 0.f;
     for (int k = 0; k < N; ++k) {
         ds[k] = T;
         const float alpha = sub_(1.0f, expf(-mul_(sb[k], dist_of(k))));
+        if (in_sphere == 2) dep += alpha * T * tb[k];
         T = mul_(T, add_(sub_(1.0f, alpha), 1e-10f));
     }
     const float gc[3] = {g_comp ? g_comp[b * 3] : 0.f, g_comp ? g_comp[b * 3 + 1] : 0.f, g_comp ? g_comp[b * 3 + 2] : 0.f};
     const float ga = (g_acc ? g_acc[b] : 0.f) - (white ? (gc[0] + gc[1] + gc[2]) : 0.f);
-    const float gd = g_depth ? g_depth[b] : 0.f;
+    const float gd = (g_depth && (in_sphere != 2 || isfinite(dep))) ? g_depth[b] : 0.f;
     float S = (g_lam ? g_lam[b] : 0.f) * T;
     for (int k = N - 1; k >= 0; --k) {
         const float Tk = ds[k];

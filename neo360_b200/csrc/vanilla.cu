@@ -204,6 +204,25 @@ __global__ void head_act_kernel(const float* __restrict__ raw_sigma, const float
     else rgb[m * 3 + c] = rgb_act(raw_rgb[m * 3 + c]);
 }
 
+// Training path (neo360_b200/vanilla.py): the fp32 encodings the field kernel builds in shared memory, written out for the framework's
+// dense layers.  Elements [0, M*63) are point-encoding columns (row = sample, helper.py:445-449 column order), [M*63, M*63 + n*27) are
+// direction-encoding columns (row = ray); the point and pos_enc_col are field_kernel's own arithmetic, so the values are bit-identical.
+__global__ void encode_kernel(const float* __restrict__ rays_o, const float* __restrict__ viewdirs, const float* __restrict__ tvals, int n, int N,
+                              float* __restrict__ enc, float* __restrict__ dir_enc) {
+    const long long M = (long long)n * N, gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid < M * kEnc) {
+        const long long m = gid / kEnc;
+        const int c = (int)(gid % kEnc), b = (int)(m / N);
+        const float t = tvals[m];
+        float x[3];
+        for (int j = 0; j < 3; ++j) x[j] = add_(rays_o[3 * b + j], mul_(t, viewdirs[3 * b + j]));
+        enc[gid] = pos_enc_col(x, 3, 10, c);
+    } else if (gid < M * kEnc + (long long)n * kDirEnc) {
+        const long long e = gid - M * kEnc;
+        dir_enc[e] = pos_enc_col(viewdirs + 3 * (e / kDirEnc), 3, 4, (int)(e % kDirEnc));
+    }
+}
+
 }  // namespace van
 }  // namespace neo
 
@@ -369,4 +388,36 @@ extern "C" int neo_vanilla_render_fwd(const NeoVanilla* v, const NeoRays* rays, 
         if ((rc = copy_out(out->weights[lvl], wt, (size_t)n * N, s))) return rc;
     }
     return NEO_OK;
+}
+
+// ---- stage-level entry points of the training path (neo360_b200/vanilla.py): sampling and encodings have no backward; the compositing
+// backward is composite_bwd_kernel in mode 2 (csrc/sampling.cu); the dense layers are differentiated by the host framework ----
+extern "C" int neo_vanilla_sample_along_rays(const float* rays_o, const float* viewdirs, int n_rays, int n_coarse, float near_plane, float far_plane,
+                                             const float* u_rand, float* t_vals, void* stream) {
+    if (!rays_o || !viewdirs || !t_vals || n_rays <= 0 || n_coarse < 1) { set_error("neo_vanilla_sample_along_rays: bad arguments"); return NEO_ERR_INVALID; }
+    const long long total = (long long)n_rays * (n_coarse + 1);
+    van::sample_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(rays_o, viewdirs, n_rays, n_coarse, near_plane, far_plane,
+                                                                                          u_rand, t_vals);
+    NEO_LAUNCH_CHECK("vanilla sample_kernel");
+    return NEO_OK;
+}
+
+extern "C" int neo_vanilla_encode(const float* rays_o, const float* viewdirs, const float* t_vals, int n_rays, int N, float* enc, float* dir_enc,
+                                  void* stream) {
+    if (!rays_o || !viewdirs || !t_vals || !enc || !dir_enc || n_rays <= 0 || N < 1) { set_error("neo_vanilla_encode: bad arguments"); return NEO_ERR_INVALID; }
+    const long long total = (long long)n_rays * N * van::kEnc + (long long)n_rays * kDirEnc;
+    van::encode_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(rays_o, viewdirs, t_vals, n_rays, N, enc, dir_enc);
+    NEO_LAUNCH_CHECK("vanilla encode_kernel");
+    return NEO_OK;
+}
+
+extern "C" int neo_vanilla_composite_bwd(const float* rgb, const float* sigma, const float* t_vals, const float* rays_d, int n_rays, int N, int white_bkgd,
+                                         const float* g_comp_rgb, const float* g_acc, const float* g_weights, const float* g_depth, float* d_rgb,
+                                         float* d_sigma, void* stream) {
+    if (!rgb || !sigma || !t_vals || !rays_d || !d_rgb || !d_sigma || n_rays <= 0 || N < 1) {
+        set_error("neo_vanilla_composite_bwd: bad arguments");
+        return NEO_ERR_INVALID;
+    }
+    return launch_composite_bwd(rgb, sigma, t_vals, rays_d, nullptr, n_rays, N, white_bkgd, 2, g_comp_rgb, g_acc, g_weights, nullptr, g_depth,
+                                d_rgb, d_sigma, (cudaStream_t)stream);
 }

@@ -109,41 +109,48 @@ class _LookupMaps(torch.autograd.Function):
 
 
 class _Composite(torch.autograd.Function):
-    """volumetric_rendering (helper.py:128-171): (rgb (B,N,3), sigma (B,N,1), t (B,N)) -> comp, acc, weights, bg_lambda, depth."""
+    """volumetric_rendering (helper.py:128-171): (rgb (B,N,3), sigma (B,N,1), t (B,N)) -> comp, acc, weights, bg_lambda, depth.
+    `mode`: True / 1 = NeO-360 fg (reads far), False / 0 = NeO-360 bg, 2 = vanilla NeRF (models/vanilla_nerf/helper.py:521-559; far is
+    None, bg_lambda is zeros, backward through neo_vanilla_composite_bwd)."""
 
     @staticmethod
-    def forward(ctx, rgb, sigma, t, d, far, white, in_sphere):
+    def forward(ctx, rgb, sigma, t, d, far, white, mode):
         lib = L.load()
+        mode = int(mode)
         rgb_c, sig_c = rgb.detach().contiguous().float(), sigma.detach().reshape(sigma.shape[0], -1).contiguous().float()
-        t_c, d_c, far_c = t.detach().contiguous().float(), d.detach().contiguous().float(), far.detach().reshape(-1).contiguous().float()
+        t_c, d_c = t.detach().contiguous().float(), d.detach().contiguous().float()
+        far_c = far.detach().reshape(-1).contiguous().float() if far is not None else None
         n, N = t_c.shape
         dev = t_c.device
         comp, acc = torch.empty(n, 3, device=dev), torch.empty(n, device=dev)
         w, depth = torch.empty(n, N, device=dev), torch.empty(n, device=dev)
-        lam = torch.empty(n, 1, device=dev)
+        lam = torch.empty(n, 1, device=dev) if mode == 1 else torch.zeros(n, 1, device=dev)
         with torch.cuda.device(dev):
             L.check(lib.neo_volumetric_rendering(L.ptr(rgb_c), L.ptr(sig_c), L.ptr(t_c), L.ptr(d_c), L.ptr(far_c), n, N, int(bool(white)),
-                                                 int(bool(in_sphere)), L.ptr(comp), L.ptr(acc), L.ptr(w), L.ptr(lam) if in_sphere else None,
+                                                 mode, L.ptr(comp), L.ptr(acc), L.ptr(w), L.ptr(lam) if mode == 1 else None,
                                                  L.ptr(depth), _stream()))
         ctx.save_for_backward(rgb_c, sig_c, t_c, d_c, far_c)
-        ctx.flags = (int(bool(white)), int(bool(in_sphere)))
-        if not in_sphere:
-            lam = torch.zeros(n, 1, device=dev)
+        ctx.flags = (int(bool(white)), mode)
         return comp, acc, w, lam, depth
 
     @staticmethod
     def backward(ctx, g_comp, g_acc, g_w, g_lam, g_depth):
         lib = L.load()
         rgb_c, sig_c, t_c, d_c, far_c = ctx.saved_tensors
-        white, in_sphere = ctx.flags
+        white, mode = ctx.flags
         n, N = t_c.shape
         dev = t_c.device
         d_rgb, d_sig = torch.empty(n, N, 3, device=dev), torch.empty(n, N, device=dev)
         f = lambda g: None if g is None else g.contiguous().float()
-        gs = [f(g_comp), f(g_acc), f(g_w), f(g_lam) if in_sphere else None, f(g_depth)]
         with torch.cuda.device(dev):
-            L.check(lib.neo_volumetric_rendering_bwd(L.ptr(rgb_c), L.ptr(sig_c), L.ptr(t_c), L.ptr(d_c), L.ptr(far_c), n, N, white, in_sphere,
-                                                     *[L.ptr(g) for g in gs], L.ptr(d_rgb), L.ptr(d_sig), _stream()))
+            if mode == 2:
+                gs = [f(g_comp), f(g_acc), f(g_w), f(g_depth)]
+                L.check(lib.neo_vanilla_composite_bwd(L.ptr(rgb_c), L.ptr(sig_c), L.ptr(t_c), L.ptr(d_c), n, N, white,
+                                                      *[L.ptr(g) for g in gs], L.ptr(d_rgb), L.ptr(d_sig), _stream()))
+            else:
+                gs = [f(g_comp), f(g_acc), f(g_w), f(g_lam) if mode else None, f(g_depth)]
+                L.check(lib.neo_volumetric_rendering_bwd(L.ptr(rgb_c), L.ptr(sig_c), L.ptr(t_c), L.ptr(d_c), L.ptr(far_c), n, N, white, mode,
+                                                         *[L.ptr(g) for g in gs], L.ptr(d_rgb), L.ptr(d_sig), _stream()))
         return d_rgb, d_sig.reshape(n, N, 1), None, None, None, None, None
 
 

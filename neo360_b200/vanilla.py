@@ -3,7 +3,13 @@
 `NeRF.forward(rays, randomized, white_bkgd, near, far)` returns the reference's `list[2]` of `(comp_rgb, acc, depth)`
 (model.py:214).  Parameter names and shapes equal the reference's (`coarse_mlp.pts_linears.0.weight`, ...), so its checkpoints
 load.  Arithmetic (csrc/vanilla.cu): `self.precision = "fp32"` (default) runs the layers on fp32 CUDA cores in the reference
-formulation; `"tc"` runs them as fp16 wgmma GEMMs with fp32 accumulation (csrc/gemm_tc.cu).  CUDA only, no CPU fallback."""
+formulation; `"tc"` runs them as fp16 wgmma GEMMs with fp32 accumulation (csrc/gemm_tc.cu).  CUDA only, no CPU fallback.
+
+Training: with autograd on, the module in train mode and parameters that require grad, `NeRF.forward` returns the same tuples
+differentiable w.r.t. every MLP parameter (LitNeRF.training_step, model.py:273-299).  Sampling, encodings and compositing forward and
+backward are hand-written CUDA; the dense layers are framework fp32 GEMMs under autograd.  `precision` applies to inference only: training
+runs fp32 whatever it is set to.  After an optimiser step the next inference call re-packs the weights (`_ensure` keys on each
+parameter's storage and version)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -11,8 +17,10 @@ from typing import Dict, List
 
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 
 from . import _lib as L
+from .training import _Composite
 
 
 class NeRFMLP(nn.Module):
@@ -50,6 +58,25 @@ class NeRFMLP(nn.Module):
 
     def forward(self, *a, **k):
         raise RuntimeError("NeRFMLP is evaluated inside the CUDA path; call NeRF.forward")
+
+
+def _mlp_train(m: NeRFMLP, enc: torch.Tensor, denc: torch.Tensor, n: int, N: int):
+    """NeRFMLP.forward (model.py:100-125) as framework GEMMs on the module's parameters: enc (n*N, 63), denc (n, 27) -> raw rgb (n, N, 3),
+    raw sigma (n, N, 1).  views_linear.0 sees [bottleneck | dir_enc]; its dir_enc columns are applied once per ray and broadcast over the
+    ray's N samples (the same sum, re-associated)."""
+    lin = lambda layer, x: F.linear(x, layer.weight, layer.bias)
+    x = enc
+    for i in range(8):
+        x = torch.relu(lin(m.pts_linears[i], x))
+        if i == 4:
+            x = torch.cat([x, enc], -1)
+    raw_sigma = lin(m.density_layer, x)
+    beta = lin(m.bottleneck_layer, x)
+    v = m.views_linear[0]
+    kb = beta.shape[-1]
+    y = F.linear(beta, v.weight[:, :kb], v.bias).reshape(n, N, -1) + F.linear(denc, v.weight[:, kb:])[:, None, :]
+    raw_rgb = lin(m.rgb_layer, torch.relu(y))
+    return raw_rgb, raw_sigma.reshape(n, N, 1)
 
 
 class NeRF(nn.Module):
@@ -91,7 +118,7 @@ class NeRF(nn.Module):
 
     def forward(self, rays: Dict[str, torch.Tensor], randomized: bool, white_bkgd: bool, near, far, debug: bool = False) -> List[tuple]:
         if torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters()):
-            raise NotImplementedError("backward through the CUDA path is not built yet; call under torch.no_grad() / .eval()")
+            return self._forward_train(rays, randomized, white_bkgd, near, far, debug)
         o = rays["rays_o"].contiguous().float()
         d = rays["rays_d"].contiguous().float()
         vd = rays["viewdirs"].contiguous().float()
@@ -135,3 +162,47 @@ class NeRF(nn.Module):
         if debug:
             self.last_debug = T
         return [(T["comp_rgb"][lvl], T["acc"][lvl], T["depth"][lvl]) for lvl in range(2)]
+
+    def _forward_train(self, rays: Dict[str, torch.Tensor], randomized: bool, white_bkgd: bool, near, far, debug: bool = False) -> List[tuple]:
+        """NeRF.forward under autograd (what LitNeRF.training_step calls, models/vanilla_nerf/model.py:273-299): the same tuples,
+        differentiable w.r.t. every parameter of coarse_mlp and fine_mlp.  Sampling, encodings and compositing (forward and backward) are
+        the library's stages; the NeRFMLP layers are framework GEMMs (`F.linear`) on the modules' own parameters, in fp32 whatever
+        `self.precision` is.  `debug=True` keeps each level's sample positions and (detached) weights in `self.last_debug`."""
+        o = rays["rays_o"].contiguous().float()
+        d = rays["rays_d"].contiguous().float()
+        vd = rays["viewdirs"].contiguous().float()
+        if not o.is_cuda:
+            raise RuntimeError("neo360_b200 needs CUDA tensors (no CPU fallback)")
+        lib = L.load()
+        n, dev = o.shape[0], o.device
+        nc, nf = self.num_coarse_samples, self.num_fine_samples
+        u = [None, None]
+        if randomized:
+            u = rays.get("_uniforms") or [torch.rand((n, nc + 1), device=dev), torch.rand((n, nf), device=dev)]   # helper.py:438, 587
+            u = [x.contiguous().float() for x in u]
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        ret, t, w = [], None, None
+        dbg = {"t": [], "weights": []}
+        for lvl, mlp in enumerate((self.coarse_mlp, self.fine_mlp)):
+            with torch.cuda.device(dev):
+                if lvl == 0:
+                    t = torch.empty(n, nc + 1, device=dev)
+                    L.check(lib.neo_vanilla_sample_along_rays(L.ptr(o), L.ptr(vd), n, nc, float(near), float(far), L.ptr(u[0]), L.ptr(t), stream))
+                else:       # bins = mids(t), weights[1:-1] of the DETACHED level-0 weights (helper.py:613)
+                    t1 = torch.empty(n, t.shape[1] + nf, device=dev)
+                    L.check(lib.neo_sample_pdf(L.ptr(o), L.ptr(vd), None, L.ptr(t), L.ptr(w.detach().contiguous()), n, t.shape[1], nf, 1, 0.0,
+                                               L.ptr(u[1]), L.ptr(t1), None, None, stream))
+                    t = t1
+                N = t.shape[1]
+                enc, denc = torch.empty(n * N, 63, device=dev), torch.empty(n, 27, device=dev)
+                L.check(lib.neo_vanilla_encode(L.ptr(o), L.ptr(vd), L.ptr(t), n, N, L.ptr(enc), L.ptr(denc), stream))
+            raw_rgb, raw_sigma = _mlp_train(mlp, enc, denc, n, N)
+            rgb = torch.sigmoid(raw_rgb) * (1 + 2 * 0.001) - 0.001              # model.py:197-205
+            sigma = F.softplus(raw_sigma - 1.0)
+            comp, acc, w, _, depth = _Composite.apply(rgb, sigma, t, d, None, white_bkgd, 2)
+            ret.append((comp, acc, depth))
+            dbg["t"].append(t)
+            dbg["weights"].append(w.detach())
+        if debug:
+            self.last_debug = dbg
+        return ret
