@@ -305,6 +305,33 @@ size_t neo_mip_workspace_bytes(int n_rays, const NeoMipCfg* cfg, int nerf_width)
 int neo_mip_render_fwd(const NeoMipMLPParams mlps[3], const float* rays_o, const float* rays_d, const float* viewdirs,
                        const float* radii, int n_rays, const NeoMipCfg* cfg, NeoMipOut* out, void* workspace,
                        size_t workspace_bytes, void* stream);
+/* Stages of the differentiable MipNeRF360.forward (training, LitMipNeRF360.training_step, models/mipnerf360/model.py:427-456 under autograd;
+ * neo360_b200/mip.py).  Hand-written: resampling, IPE features and direction encoding (no backward: sdist is detached, model.py:309-310, and
+ * contract returns detached values, helper.py:63-66), compositing forward and backward; the MLP dense layers are differentiated by the host
+ * framework.  Each launches the same kernel as neo_mip_render_fwd's NEO_PREC_FP32 path, so training and eval share their arithmetic. */
+/* One level of max_dilate_weights + annealed logits + sample_intervals + s_to_t (model.py:262-312): sdist, tdist (n_rays, n_new+1).
+ * level 0 reads no previous level (sdist_prev / weights_prev may be NULL); level 1 or 2 reads the previous level's sdist (n_rays, n_prev+1)
+ * and weights (n_rays, n_prev).  The dilation is 0.0025 + 0.5 / n_prev^level (both proposal levels take num_prop_samples).  n_new in
+ * [2,160], n_prev in [1,160]; jitter (n_rays) or NULL = deterministic.  Bit-identical to neo_mip_render_fwd's resampling of that level. */
+int neo_mip_resample(const float* sdist_prev, const float* weights_prev, int n_rays, int n_prev, int level, int n_new, float near_plane,
+                     float far_plane, float train_frac, const float* jitter, float* sdist, float* tdist, void* stream);
+/* fp32 integrated positional encoding of the conical frustums of tdist (n_rays, N+1) (cast_rays + contract + lift_and_diagonalize +
+ * integrated_pos_enc): feats (n_rays*N, 504); and the direction encoding of viewdirs, one row per ray: dir_enc (n_rays, 27).  basis is
+ * pos_basis_t (3,21).  The NEO_PREC_FP32 path's own kernels (bit-identical).  No backward. */
+int neo_mip_encode(const float* rays_o, const float* rays_d, const float* viewdirs, const float* radii, const float* tdist, const float* basis,
+                   int n_rays, int N, float* feats, float* dir_enc, void* stream);
+/* Head activations + compute_alpha_weights(opaque_background) + volumetric_rendering with a white background (helper.py:234-274) of raw
+ * density (n_rays,N) and raw rgb (n_rays,N,3) at tdist (n_rays,N+1): rgb (n_rays,3), weights (n_rays,N), density (n_rays,N), rgb_s
+ * (n_rays,N,3).  raw_rgb NULL = a proposal level (rgb_s is written as zeros).  Outputs may be NULL.  The eval path's compositing kernel. */
+int neo_mip_composite(const float* raw_density, const float* raw_rgb, const float* tdist, const float* rays_d, int n_rays, int N, float* rgb,
+                      float* weights, float* density, float* rgb_s, void* stream);
+/* Backward of neo_mip_composite: upstream gradients of rgb (n,3), weights (n,N), density (n,N), rgb_s (n,N,3) -- any may be NULL -- ->
+ * d_raw_density (n,N) and, unless raw_rgb is NULL, d_raw_rgb (n,N,3).  Same raw_density / raw_rgb / tdist / rays_d as the forward call.
+ * The gradient of clip(1 - acc, min=0) passes where 1 - acc >= 0 of this call's own fp32 acc; the last (infinite) interval has no
+ * density gradient through the weights. */
+int neo_mip_composite_bwd(const float* raw_density, const float* raw_rgb, const float* tdist, const float* rays_d, int n_rays, int N,
+                          const float* g_rgb, const float* g_weights, const float* g_density, const float* g_rgb_s, float* d_raw_density,
+                          float* d_raw_rgb, void* stream);
 
 /* ---- tri-plane builder, dense part (SURVEY.md section 8(f1)): models/neo360/encoder_tp_fusion_conv.py:472-597 between the ResNet feature
  * extractor and the floor-plan conv stacks (both stay in the host framework).  64^3 world grid x nv views: latent lookup, DepthPillarEncoder

@@ -120,6 +120,11 @@ SYMBOLS = {
     "neo_mip_workspace_bytes": (C.c_size_t, [C.c_int, C.POINTER(NeoMipCfg), C.c_int]),
     "neo_mip_render_fwd": (C.c_int, [C.POINTER(NeoMipMLPParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(NeoMipCfg),
                                      C.POINTER(NeoMipOut), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "neo_mip_resample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_void_p]),
+    "neo_mip_encode": (C.c_int, [C.c_void_p] * 6 + [C.c_int] * 2 + [C.c_void_p] * 3),
+    "neo_mip_composite": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 2 + [C.c_void_p] * 5),
+    "neo_mip_composite_bwd": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 2 + [C.c_void_p] * 7),
     "neo_grid_encoder_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "neo_grid_encoder_dense": (C.c_int, [C.POINTER(NeoGridEncoderParams), C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                          C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

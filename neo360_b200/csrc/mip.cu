@@ -383,6 +383,92 @@ __global__ void composite_kernel(const float* __restrict__ raw_density, const fl
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// backward of composite_kernel w.r.t. the raw density and raw rgb (sample positions carry no gradient: model.py:309-310)  (one warp per ray)
+//   x_k = softplus(r_k - 1) delta_k (x_{N-1} = inf),  T_k = exp(-sum_{j<k} x_j),  w_k = (1 - e^{-x_k}) T_k,  rgb = sum w c + clip(1 - acc, 0)
+//   G_k = g_w_k + g_rgb . c_k - m sum(g_rgb),   m = [1 - acc >= 0]   (the gradient clip passes, decided on this kernel's own fp32 acc)
+//   dL/dx_k = G_k e^{-x_k} T_k - sum_{j>k} G_j w_j  (0 for the last, infinite, interval)
+//   d_raw_density_k = (delta_k dL/dx_k + g_density_k) softplus'(r_k - 1),   d_raw_rgb_k = (w_k g_rgb + g_rgb_s_k) 1.002 s (1 - s)
+// Pass 1 repeats composite_kernel's operations for w and acc and keeps the exclusive scan in the d_raw_density
+// row; pass 2 walks the chunks backwards with a suffix scan of G w.
+// ------------------------------------------------------------------------------------------------
+__global__ void composite_bwd_kernel(const float* __restrict__ raw_density, const float* __restrict__ raw_rgb, const float* __restrict__ tdist,
+                                     const float* __restrict__ rays_d, int n_rays, int n, const float* __restrict__ g_rgb,
+                                     const float* __restrict__ g_w, const float* __restrict__ g_density, const float* __restrict__ g_rgb_s,
+                                     float* __restrict__ d_raw_density, float* __restrict__ d_raw_rgb) {
+    const int warps = blockDim.x / 32, wid = threadIdx.x / 32, lane = threadIdx.x % 32;
+    const int b = blockIdx.x * warps + wid;
+    if (b >= n_rays) return;
+    const float* dd3 = rays_d + 3 * b;
+    const float dn = __fsqrt_rn(dot3_(dd3, dd3));
+    const float* t = tdist + (size_t)b * (n + 1);
+    const float* rd = raw_density + (size_t)b * n;
+    float* gd = d_raw_density + (size_t)b * n;
+    auto x_of = [&](int k, float& delta) -> float {
+        delta = mul_(sub_(t[k + 1], t[k]), dn);
+        return (k == n - 1) ? INFINITY : mul_(softplus_(rd[k] - 1.0f), delta);
+    };
+    float carry = 0.f, acc = 0.f;
+    for (int base = 0; base < n; base += 32) {
+        const int k = base + lane;
+        const bool ok = k < n;
+        float delta, dd = ok ? x_of(k, delta) : 0.f;
+        float sc = ok ? ((k == n - 1) ? 0.f : dd) : 0.f;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { float nb = __shfl_up_sync(0xffffffffu, sc, o); if (lane >= o) sc = add_(sc, nb); }
+        const float incl = add_(sc, carry);
+        float excl = __shfl_up_sync(0xffffffffu, incl, 1);
+        if (lane == 0) excl = carry;
+        if (ok) {
+            gd[k] = excl;
+            acc += (1.f - expf(-dd)) * expf(-excl);
+        }
+        carry = __shfl_sync(0xffffffffu, incl, 31);
+    }
+    acc = warp_sum(acc);
+    const float gc[3] = {g_rgb ? g_rgb[3 * b] : 0.f, g_rgb ? g_rgb[3 * b + 1] : 0.f, g_rgb ? g_rgb[3 * b + 2] : 0.f};
+    const float gbg = (1.f - acc >= 0.f) ? gc[0] + gc[1] + gc[2] : 0.f;
+    float S = 0.f;                                              // sum_{j >= next chunk} G_j w_j
+    for (int base = ((n - 1) / 32) * 32; base >= 0; base -= 32) {
+        const int k = base + lane;
+        const bool ok = k < n;
+        float v = 0.f, dx = 0.f, delta = 0.f, w = 0.f, T = 0.f, e = 0.f, s[3] = {0.f, 0.f, 0.f};
+        if (ok) {
+            const float dd = x_of(k, delta);
+            T = expf(-gd[k]);
+            e = expf(-dd);
+            w = (1.f - e) * T;
+            float G = (g_w ? g_w[(size_t)b * n + k] : 0.f) - gbg;
+            if (raw_rgb)
+                for (int c = 0; c < 3; ++c) {
+                    s[c] = raw_rgb[((size_t)b * n + k) * 3 + c];
+                    G += gc[c] * rgb_act(s[c]);
+                }
+            v = G * w;
+            dx = G * e * T;
+        }
+        float incl = v;                                         // suffix scan within the chunk
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { float nb = __shfl_down_sync(0xffffffffu, incl, o); if (lane + o < 32) incl += nb; }
+        float after = __shfl_down_sync(0xffffffffu, incl, 1);
+        if (lane == 31) after = 0.f;
+        const float chunk = __shfl_sync(0xffffffffu, incl, 0);
+        if (ok) {
+            dx = (k == n - 1) ? 0.f : dx - (after + S);
+            const float z = rd[k] - 1.0f;
+            const float sp = z > 20.f ? 1.f : 1.f / (1.f + expf(-z));            // softplus'(z), threshold 20 as F.softplus
+            gd[k] = (delta * dx + (g_density ? g_density[(size_t)b * n + k] : 0.f)) * sp;
+            if (raw_rgb)
+                for (int c = 0; c < 3; ++c) {
+                    const float q = expf(-fabsf(s[c]));                           // s (1 - s) = q / (1 + q)^2 without cancellation
+                    const float up = w * gc[c] + (g_rgb_s ? g_rgb_s[((size_t)b * n + k) * 3 + c] : 0.f);
+                    d_raw_rgb[((size_t)b * n + k) * 3 + c] = up * (1.002f * (q / ((1.f + q) * (1.f + q))));
+                }
+        }
+        S += chunk;
+    }
+}
+
 }  // namespace mip
 }  // namespace neo
 
@@ -424,6 +510,23 @@ int check(const NeoMipCfg* c) {
     if (c->precision != NEO_PREC_FP32 && c->precision != NEO_PREC_TC) { set_error("mip: bad precision %d", c->precision); return NEO_ERR_INVALID; }
     return NEO_OK;
 }
+// One level of proposal resampling (max_dilate_weights + annealed logits + sample_intervals + s_to_t): sdist / tdist (n_rays, n + 1).
+// Level 0 reads no previous level; level l > 0 reads the (n_rays, n_prev + 1) sdist and (n_rays, n_prev) weights of level l - 1.
+// dilation = 0.0025 + 0.5 / prod(sample counts of the levels before), model.py:265-272.
+int launch_resample(const float* s_prev, const float* w_prev, int n_rays, int n_prev, int level, float dilation, float anneal, int n, float near,
+                    float far, const float* jitter, float* s_out, float* t_out, cudaStream_t s) {
+    int p2 = 2;
+    while (p2 < 3 * n_prev + 1 || p2 < n + 1) p2 <<= 1;
+    const int warps = 4;
+    const size_t smem = (size_t)warps * (3 * p2 + 3 * n_prev) * sizeof(float);
+    if (smem > 48 * 1024) NEO_CUDA(cudaFuncSetAttribute(mip::resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    mip::resample_kernel<<<(n_rays + warps - 1) / warps, warps * 32, smem, s>>>(s_prev, w_prev, n_rays, n_prev, level, dilation, anneal, n, near, far,
+                                                                               jitter, s_out, t_out, p2);
+    NEO_LAUNCH_CHECK("mip resample_kernel");
+    return NEO_OK;
+}
+float anneal_of(float train_frac) { return (10.f * train_frac) / (9.f * train_frac + 1.f); }     // bias(train_frac, anneal_slope=10)
+constexpr int kCompWarps = 8;
 int gemm(const float* A1, int K1, const float* A2, int K2, const float* W, const float* b, long long M, int N, int relu, float* out, cudaStream_t s) {
     dim3 grid((unsigned)((M + 63) / 64), (unsigned)((N + 63) / 64));
     mip::sgemm_kernel<<<grid, 256, 0, s>>>(A1, K1, A2, K2, W, b, M, N, relu, out);
@@ -513,21 +616,14 @@ extern "C" int neo_mip_render_fwd(const NeoMipMLPParams mlps[3], const float* ra
     size_t need = carve(c, n_rays, cfg, width, w);
     if (!workspace || workspace_bytes < need) { set_error("workspace too small: need %zu bytes, got %zu", need, workspace_bytes); return NEO_ERR_WORKSPACE; }
     const int ns[3] = {cfg->n_prop, cfg->n_prop, cfg->n_nerf};
-    const float anneal = (10.f * cfg->train_frac) / (9.f * cfg->train_frac + 1.f);      // bias(train_frac, anneal_slope=10)
+    const float anneal = anneal_of(cfg->train_frac);
     long long prod = 1;
     for (int lvl = 0; lvl < 3; ++lvl) {
         const int n = ns[lvl], n_prev = lvl ? ns[lvl - 1] : 1;
         const float dilation = 0.0025f + 0.5f / (float)prod;
         prod *= n;
-        int p2 = 2;
-        while (p2 < 3 * n_prev + 1 || p2 < n + 1) p2 <<= 1;
-        const int warps = 4;
-        const size_t smem = (size_t)warps * (3 * p2 + 3 * n_prev) * sizeof(float);
-        if (smem > 48 * 1024) NEO_CUDA(cudaFuncSetAttribute(mip::resample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        mip::resample_kernel<<<(n_rays + warps - 1) / warps, warps * 32, smem, s>>>(lvl ? w.s[lvl - 1] : nullptr, lvl ? w.w[lvl - 1] : nullptr, n_rays,
-                                                                                   n_prev, lvl, dilation, anneal, n, cfg->near_plane, cfg->far_plane,
-                                                                                   cfg->jitter[lvl], w.s[lvl], w.t, p2);
-        NEO_LAUNCH_CHECK("mip resample_kernel");
+        if ((rc = launch_resample(lvl ? w.s[lvl - 1] : nullptr, lvl ? w.w[lvl - 1] : nullptr, n_rays, n_prev, lvl, dilation, anneal, n, cfg->near_plane,
+                                  cfg->far_plane, cfg->jitter[lvl], w.s[lvl], w.t, s))) return rc;
         const long long M = (long long)n_rays * n;
         const bool tcp = cfg->precision == NEO_PREC_TC;
         if (tcp) mip::features16_kernel<<<(unsigned)((M + mip::kFeatSamples - 1) / mip::kFeatSamples), mip::kFeatThreads, 0, s>>>(
@@ -561,12 +657,67 @@ extern "C" int neo_mip_render_fwd(const NeoMipMLPParams mlps[3], const float* ra
                 if (out->rgb_s[lvl]) NEO_CUDA(cudaMemsetAsync(out->rgb_s[lvl], 0, (size_t)M * 3 * sizeof(float), s));     // disable_rgb: zeros
             }
         }
-        const int cw = 8;
+        const int cw = kCompWarps;
         mip::composite_kernel<<<(n_rays + cw - 1) / cw, cw * 32, 0, s>>>(w.rawd, rawc, w.t, rays_d, n_rays, n, out->density[lvl],
                                                                         rawc ? out->rgb_s[lvl] : nullptr, w.w[lvl], out->rgb[lvl]);
         NEO_LAUNCH_CHECK("mip composite_kernel");
         if ((rc = copy_out(out->sdist[lvl], w.s[lvl], (size_t)n_rays * (n + 1), s))) return rc;
         if ((rc = copy_out(out->weights[lvl], w.w[lvl], (size_t)M, s))) return rc;
     }
+    return NEO_OK;
+}
+
+// ---- stage-level entry points of the training path (neo360_b200/mip.py): resampling and encodings have no backward (the sample positions
+// are detached, model.py:309-310, and contract returns detached values, helper.py:63-66); compositing forward is composite_kernel itself and
+// its backward composite_bwd_kernel; the dense layers are differentiated by the host framework ----
+extern "C" int neo_mip_resample(const float* sdist_prev, const float* weights_prev, int n_rays, int n_prev, int level, int n_new, float near_plane,
+                                float far_plane, float train_frac, const float* jitter, float* sdist, float* tdist, void* stream) {
+    if (level < 0 || level > 2) { set_error("neo_mip_resample: level must be 0, 1 or 2 (got %d)", level); return NEO_ERR_INVALID; }
+    if (!sdist || !tdist || n_rays <= 0 || n_new < 2 || n_new > 160 || (level > 0 && (!sdist_prev || !weights_prev || n_prev < 1 || n_prev > 160))) {
+        set_error("neo_mip_resample: bad arguments");
+        return NEO_ERR_INVALID;
+    }
+    if (!(near_plane > 0.f) || !(far_plane > near_plane)) { set_error("neo_mip_resample: need 0 < near < far"); return NEO_ERR_INVALID; }
+    // levels 0 and 1 both take num_prop_samples, so the sample counts before level l multiply to n_prev^l
+    float prod = 1.f;
+    for (int l = 0; l < level; ++l) prod *= (float)n_prev;
+    return launch_resample(level ? sdist_prev : nullptr, level ? weights_prev : nullptr, n_rays, level ? n_prev : 1, level, 0.0025f + 0.5f / prod,
+                           anneal_of(train_frac), n_new, near_plane, far_plane, jitter, sdist, tdist, (cudaStream_t)stream);
+}
+
+extern "C" int neo_mip_encode(const float* rays_o, const float* rays_d, const float* viewdirs, const float* radii, const float* tdist, const float* basis,
+                              int n_rays, int N, float* feats, float* dir_enc, void* stream) {
+    if (!rays_o || !rays_d || !viewdirs || !radii || !tdist || !basis || !feats || !dir_enc || n_rays <= 0 || N < 1) {
+        set_error("neo_mip_encode: bad arguments");
+        return NEO_ERR_INVALID;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    const long long M = (long long)n_rays * N;
+    mip::features_kernel<<<(unsigned)((M + 7) / 8), 256, 0, s>>>(rays_o, rays_d, radii, tdist, basis, M, N, feats);
+    NEO_LAUNCH_CHECK("mip features_kernel");
+    mip::dir_kernel<<<(unsigned)(((long long)n_rays * kDirEnc + 255) / 256), 256, 0, s>>>(viewdirs, (long long)n_rays, 1, dir_enc, kDirEnc, kDirEnc);
+    NEO_LAUNCH_CHECK("mip dir_kernel");
+    return NEO_OK;
+}
+
+extern "C" int neo_mip_composite(const float* raw_density, const float* raw_rgb, const float* tdist, const float* rays_d, int n_rays, int N, float* rgb,
+                                 float* weights, float* density, float* rgb_s, void* stream) {
+    if (!raw_density || !tdist || !rays_d || n_rays <= 0 || N < 1) { set_error("neo_mip_composite: bad arguments"); return NEO_ERR_INVALID; }
+    mip::composite_kernel<<<(n_rays + kCompWarps - 1) / kCompWarps, kCompWarps * 32, 0, (cudaStream_t)stream>>>(raw_density, raw_rgb, tdist, rays_d,
+                                                                                                              n_rays, N, density, rgb_s, weights, rgb);
+    NEO_LAUNCH_CHECK("mip composite_kernel");
+    return NEO_OK;
+}
+
+extern "C" int neo_mip_composite_bwd(const float* raw_density, const float* raw_rgb, const float* tdist, const float* rays_d, int n_rays, int N,
+                                     const float* g_rgb, const float* g_weights, const float* g_density, const float* g_rgb_s, float* d_raw_density,
+                                     float* d_raw_rgb, void* stream) {
+    if (!raw_density || !tdist || !rays_d || !d_raw_density || (raw_rgb && !d_raw_rgb) || n_rays <= 0 || N < 1) {
+        set_error("neo_mip_composite_bwd: bad arguments");
+        return NEO_ERR_INVALID;
+    }
+    mip::composite_bwd_kernel<<<(n_rays + kCompWarps - 1) / kCompWarps, kCompWarps * 32, 0, (cudaStream_t)stream>>>(
+        raw_density, raw_rgb, tdist, rays_d, n_rays, N, g_rgb, g_weights, g_density, g_rgb_s, d_raw_density, d_raw_rgb);
+    NEO_LAUNCH_CHECK("mip composite_bwd_kernel");
     return NEO_OK;
 }

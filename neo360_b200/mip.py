@@ -3,7 +3,15 @@
 `MipNeRF360.forward(batch, train_frac, randomized, is_train, near, far)` returns the reference's
 `(renderings: list[3] of {"rgb"}, ray_history: list[3] of {"density","rgb","sdist","weights"})` (model.py:359-365).  Parameter and
 buffer names equal the reference's (`mlps.{0,1,2}.pts_linear.{i}`, `density_layer`, `bottleneck_layer`, `views_linear.0`,
-`rgb_layer`, `pos_basis_t`).  Arithmetic: fp32 CUDA cores in the reference formulation (csrc/mip.cu); CUDA only."""
+`rgb_layer`, `pos_basis_t`).  Arithmetic (csrc/mip.cu): `precision = "fp32"` (default) runs the MLPs as fp32 CUDA-core SGEMMs in the
+reference formulation; `"tc"` runs every dense layer on the tensor cores (fp16 operands).  CUDA only, no CPU fallback.
+
+Training: with autograd on, the module in train mode and parameters that require grad, `MipNeRF360.forward` returns the same
+`(renderings, ray_history)` differentiable w.r.t. every MLP parameter (LitMipNeRF360.training_step, model.py:427-456): `density`, `rgb`
+and `weights` of every level and each level's rendered `rgb` carry gradients, `sdist` is detached (model.py:309-310) and the proposal
+levels' `rgb` are zeros.  Resampling, IPE features, direction encoding and compositing forward and backward are hand-written CUDA; the
+dense layers are framework fp32 GEMMs under autograd.  `precision` applies to inference only: training runs fp32 whatever it is set to.
+`training_loss` is the reference's training loss on those outputs."""
 from __future__ import annotations
 
 import ctypes as C
@@ -11,9 +19,11 @@ from typing import Dict, List, Tuple
 
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 
 from . import _lib as L
 from .mip_basis import POS_BASIS_T
+from .training import distortion_loss
 
 
 class MipNeRF360MLP(nn.Module):
@@ -74,7 +84,7 @@ class MipNeRF360(nn.Module):
 
     def forward(self, batch: Dict[str, torch.Tensor], train_frac: float, randomized: bool, is_train: bool, near, far) -> Tuple[List[dict], List[dict]]:
         if torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters()):
-            raise NotImplementedError("backward through the CUDA path is not built yet; call under torch.no_grad() / .eval()")
+            return self._forward_train(batch, train_frac, randomized, near, far)
         o = batch["rays_o"].contiguous().float()
         if not o.is_cuda:
             raise RuntimeError("neo360_b200 needs CUDA tensors (no CPU fallback)")
@@ -113,3 +123,128 @@ class MipNeRF360(nn.Module):
             L.check(lib.neo_mip_render_fwd(arr, L.ptr(o), L.ptr(d), L.ptr(vd), L.ptr(radii), n, C.byref(cfg), C.byref(out), self._ws.data_ptr(),
                                            self._ws.numel(), torch.cuda.current_stream().cuda_stream))
         return ren, hist
+
+    def _forward_train(self, batch: Dict[str, torch.Tensor], train_frac: float, randomized: bool, near, far) -> Tuple[List[dict], List[dict]]:
+        """MipNeRF360.forward under autograd (what LitMipNeRF360.training_step calls, model.py:427-456).  Per level: `neo_mip_resample` on the
+        detached previous weights, `neo_mip_encode`, the MLP as `F.linear` on the modules' own parameters (fp32 whatever `self.precision`
+        is), then `_MipComposite` (the eval path's compositing kernel forward, `neo_mip_composite_bwd` backward)."""
+        o = batch["rays_o"].contiguous().float()
+        if not o.is_cuda:
+            raise RuntimeError("neo360_b200 needs CUDA tensors (no CPU fallback)")
+        d, vd = batch["rays_d"].contiguous().float(), batch["viewdirs"].contiguous().float()
+        radii = batch["radii"].reshape(-1).contiguous().float()
+        lib = L.load()
+        n, dev = o.shape[0], o.device
+        jit = [None] * 3
+        if randomized:
+            jit = batch.get("_uniforms") or [torch.rand((n, 1), device=dev) for _ in range(3)]     # helper.py:361 (single_jitter)
+            jit = [j.reshape(-1).contiguous().float() for j in jit]
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        ns = (self.num_prop_samples, self.num_prop_samples, self.num_nerf_samples)
+        ren, hist = [], []
+        sdist = w = None
+        for lvl, mlp in enumerate(self.mlps):
+            N = ns[lvl]
+            with torch.cuda.device(dev):
+                s1, t1 = torch.empty(n, N + 1, device=dev), torch.empty(n, N + 1, device=dev)
+                wp = w.detach().contiguous() if lvl else None
+                L.check(lib.neo_mip_resample(L.ptr(sdist), L.ptr(wp), n, ns[lvl - 1] if lvl else 1, lvl, N, float(near), float(far),
+                                             float(train_frac), L.ptr(jit[lvl]), L.ptr(s1), L.ptr(t1), stream))
+                sdist = s1
+                feats, denc = torch.empty(n * N, 504, device=dev), torch.empty(n, 27, device=dev)
+                basis = mlp.pos_basis_t.to(dev).contiguous().float()
+                L.check(lib.neo_mip_encode(L.ptr(o), L.ptr(d), L.ptr(vd), L.ptr(radii), L.ptr(t1), L.ptr(basis), n, N, L.ptr(feats), L.ptr(denc),
+                                           stream))
+            raw_density, raw_rgb = _mlp_train(mlp, feats, denc, n, N)
+            rgb, w, density, rgb_s = _MipComposite.apply(raw_density, raw_rgb, t1, d)
+            ren.append({"rgb": rgb})
+            hist.append({"density": density, "rgb": rgb_s, "sdist": sdist, "weights": w})
+        return ren, hist
+
+
+def _mlp_train(m: MipNeRF360MLP, feats: torch.Tensor, denc: torch.Tensor, n: int, N: int):
+    """MipNeRF360MLP.forward (model.py:111-173) up to the activations, as framework GEMMs on the module's parameters: feats (n*N, 504),
+    denc (n, 27) -> raw density (n, N), raw rgb (n, N, 3) or None (PropMLP).  The skip concatenation follows layer 4 (model.py:122-126);
+    views_linear.0 sees [bottleneck | dir_enc], and its dir_enc columns are applied once per ray and broadcast over the ray's N samples
+    (the same sum, re-associated)."""
+    lin = lambda layer, x: F.linear(x, layer.weight, layer.bias)
+    x = feats
+    for i in range(m.netdepth):
+        x = torch.relu(lin(m.pts_linear[i], x))
+        if i % 4 == 0 and i > 0:
+            x = torch.cat([x, feats], -1)
+    raw_density = lin(m.density_layer, x).reshape(n, N)
+    if m.disable_rgb:
+        return raw_density, None
+    beta = lin(m.bottleneck_layer, x)
+    v = m.views_linear[0]
+    kb = beta.shape[-1]
+    y = F.linear(beta, v.weight[:, :kb], v.bias).reshape(n, N, -1) + F.linear(denc, v.weight[:, kb:])[:, None, :]
+    return raw_density, lin(m.rgb_layer, torch.relu(y))
+
+
+class _MipComposite(torch.autograd.Function):
+    """Head activations + compute_alpha_weights(opaque_background) + volumetric_rendering, white background (helper.py:234-274):
+    raw density (n,N), raw rgb (n,N,3) or None (proposal level), tdist (n,N+1), rays_d (n,3) -> rgb (n,3), weights (n,N), density (n,N),
+    rgb_s (n,N,3) (zeros for a proposal level).  Forward `neo_mip_composite` (the eval path's kernel), backward `neo_mip_composite_bwd`."""
+
+    @staticmethod
+    def forward(ctx, raw_density, raw_rgb, tdist, rays_d):
+        lib = L.load()
+        rd = raw_density.detach().contiguous().float()
+        rc = raw_rgb.detach().contiguous().float() if raw_rgb is not None else None
+        t, d = tdist.detach().contiguous().float(), rays_d.detach().contiguous().float()
+        n, N = rd.shape
+        dev = rd.device
+        rgb, w, dens, rgb_s = torch.empty(n, 3, device=dev), torch.empty(n, N, device=dev), torch.empty(n, N, device=dev), torch.empty(n, N, 3, device=dev)
+        with torch.cuda.device(dev):
+            L.check(lib.neo_mip_composite(L.ptr(rd), L.ptr(rc), L.ptr(t), L.ptr(d), n, N, L.ptr(rgb), L.ptr(w), L.ptr(dens), L.ptr(rgb_s),
+                                          torch.cuda.current_stream(dev).cuda_stream))
+        ctx.save_for_backward(rd, rc, t, d)
+        if rc is None:
+            ctx.mark_non_differentiable(rgb_s)
+        return rgb, w, dens, rgb_s
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_w, g_dens, g_rgb_s):
+        lib = L.load()
+        rd, rc, t, d = ctx.saved_tensors
+        n, N = rd.shape
+        dev = rd.device
+        d_rd = torch.empty(n, N, device=dev)
+        d_rc = torch.empty(n, N, 3, device=dev) if rc is not None else None
+        f = lambda g: None if g is None else g.contiguous().float()
+        with torch.cuda.device(dev):
+            L.check(lib.neo_mip_composite_bwd(L.ptr(rd), L.ptr(rc), L.ptr(t), L.ptr(d), n, N, L.ptr(f(g_rgb)), L.ptr(f(g_w)), L.ptr(f(g_dens)),
+                                              L.ptr(f(g_rgb_s) if rc is not None else None), L.ptr(d_rd), L.ptr(d_rc),
+                                              torch.cuda.current_stream(dev).cuda_stream))
+        return d_rd, d_rc, None, None
+
+
+def _outer_weights(t: torch.Tensor, t_env: torch.Tensor, w_env: torch.Tensor) -> torch.Tensor:
+    """w_outer of helper.inner_outer (helper.py:117-134): the envelope mass over each interval of t.  The reference's mask-based
+    searchsorted (helper.py:108-113) is torch.searchsorted(t_env, t, right=True) = r, lo = max(r - 1, 0), hi = min(r, len(t_env) - 1)."""
+    r = torch.searchsorted(t_env.contiguous(), t.contiguous(), right=True)
+    lo, hi = (r - 1).clamp(min=0), r.clamp(max=t_env.shape[-1] - 1)
+    cy = torch.cat([torch.zeros_like(w_env[..., :1]), torch.cumsum(w_env, -1)], -1)
+    return torch.gather(cy, -1, hi)[..., 1:] - torch.gather(cy, -1, lo)[..., :-1]
+
+
+def training_loss(renderings: List[dict], ray_history: List[dict], target: torch.Tensor, charb_padding: float = 0.001,
+                  interlevel_mult: float = 1.0, distortion_mult: float = 0.01) -> torch.Tensor:
+    """LitMipNeRF360.training_step's loss (model.py:442-449): sqrt(mse + charb_padding^2) of the last rendering, plus the interlevel loss
+    (lossfun_outer of every proposal level against the detached NeRF-level sdist / weights, model.py:725-734, helper.py:138-141), plus
+    distortion_mult times the distortion loss of the NeRF level (model.py:736-741, helper.py:145-152; `training.distortion_loss` is the same
+    functional in O(N) form for ascending sdist)."""
+    mse = ((renderings[-1]["rgb"] - target) ** 2).mean()
+    loss = torch.sqrt(mse + charb_padding ** 2)
+    last = ray_history[-1]
+    c, w = last["sdist"].detach(), last["weights"].detach()
+    eps = 1.1920929e-07                                                           # helper.py:18
+    inter = 0.0
+    for h in ray_history[:-1]:
+        w_outer = _outer_weights(c, h["sdist"], h["weights"])
+        inter = inter + (torch.clip(w - w_outer, min=0) ** 2 / (w + eps)).mean()
+    s, wl = last["sdist"], last["weights"]
+    dist = distortion_loss(wl, 0.5 * (s[..., 1:] + s[..., :-1]), s[..., 1:] - s[..., :-1])
+    return loss + interlevel_mult * inter + distortion_mult * dist
