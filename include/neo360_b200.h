@@ -335,8 +335,11 @@ int neo_mip_composite_bwd(const float* raw_density, const float* raw_rgb, const 
 
 /* ---- tri-plane builder, dense part (SURVEY.md section 8(f1)): models/neo360/encoder_tp_fusion_conv.py:472-597 between the ResNet feature
  * extractor and the floor-plan conv stacks (both stay in the host framework).  64^3 world grid x nv views: latent lookup, DepthPillarEncoder
- * 518->512->512->512, three pillar aggregators (513->512->1, softmax along one grid axis), softmax-weighted pillar sums.  Every dense layer
- * runs on tcgen05 (csrc/gemm_tc.cu, fp16 weights / activations, fp32 accumulation).  nn.Linear layout (out,in) fp32 device pointers. ---- */
+ * 518->512->512->512, three pillar aggregators (513->512->1, softmax along one grid axis), softmax-weighted pillar sums.  At inference
+ * (neo_grid_encoder_dense) every dense layer runs on wgmma through gemm_f16 (csrc/gemm_tc.cu, fp16 weights / activations, fp32
+ * accumulation); nn.Linear layout (out,in) fp32 device pointers.  Training uses the four fp32 stage entry points below around the host
+ * framework's dense layers.  Grid rows: row = v*64^3 + cell, cell = (ix*64 + iy)*64 + iz; axis 0 / 1 / 2 = the yz / xz / xy floor plan
+ * (the pillar runs along x / y / z). ---- */
 typedef struct {
     const float* fc_w[3];   /* depth_fc.common_branch.0 (512,518), depth_fc.common_branch.2 (512,512), depth_fc.depth_encoder (512,512) */
     const float* fc_b[3];
@@ -350,6 +353,25 @@ size_t neo_grid_encoder_workspace_bytes(int nv, int lat_h, int lat_w);
 int neo_grid_encoder_dense(const NeoGridEncoderParams* params, const float* latent, int nv, int lat_h, int lat_w, int img_w, int img_h,
                            const float* src_poses, float focal, float cx, float cy, float* floor_xz, float* floor_xy, float* floor_yz,
                            void* workspace, size_t workspace_bytes, void* stream);
+/* Training path, fp32, caller-owned buffers, asynchronous on `stream`, nothing allocated.  All four return NEO_ERR_INVALID before any
+ * launch on a NULL buffer, nv < 1, lat_h or lat_w < 2, img_w or img_h <= 0, or a stride / alignment the kernels cannot address.
+ * Lookup rows: latent_cl (nv,lat_h,lat_w,512) channel-last (16-byte aligned) -> X (nv*64^3, ldx) rows
+ * [bilinear latent lookup 512 | cam xyz 3 | masked unit direction 3 | 0 ...] = the input of depth_fc; 518 <= ldx <= 640, ldx % 4 == 0,
+ * X 16-byte aligned (so X[:, :518] of a 520-wide buffer is a strided GEMM operand). */
+int neo_grid_encoder_features(const float* latent_cl, int nv, int lat_h, int lat_w, int img_w, int img_h, const float* src_poses, float focal,
+                              float cx, float cy, float* X, int ldx, void* stream);
+/* Adjoint of the lookup columns: g_latent_cl (nv,lat_h,lat_w,512) channel-last, caller-zeroed, 16-byte aligned += sum over rows of the
+ * tap weights times g_X[row][0..512) (16-byte vector atomics; the order of the additions is not fixed).  g_X row stride ldg >= 512 and
+ * even, 8-byte aligned; columns >= 512 are not read (poses do not train).  The taps are the forward's, bit for bit. */
+int neo_grid_encoder_features_bwd(int nv, int lat_h, int lat_w, int img_w, int img_h, const float* src_poses, float focal, float cx, float cy,
+                                  const float* g_X, long long ldg, float* g_latent_cl, void* stream);
+/* Softmax pillar sums: lat (nv*64^3, 512) row-major, 16-byte aligned, logits (3, nv*64^3) by axis -> floor plans (nv,512,64,64) NCHW. */
+int neo_grid_encoder_pool(const float* lat, const float* logits, int nv, float* floor_xz, float* floor_xy, float* floor_yz, void* stream);
+/* Backward of neo_grid_encoder_pool: upstream g_xz / g_xy / g_yz (nv,512,64,64), each may be NULL (zero) -> d_lat (nv*64^3, 512) = the
+ * sum of the three axes' contributions and d_logits (3, nv*64^3) = s (g.lat - sum_pillar s (g.lat)); every element written, no
+ * floating-point atomics (two calls give bit-identical results). */
+int neo_grid_encoder_pool_bwd(const float* lat, const float* logits, int nv, const float* g_xz, const float* g_xy, const float* g_yz,
+                              float* d_lat, float* d_logits, void* stream);
 
 /* bench support: CUDA events around every field-kernel launch on the launching stream + launch accounting.
  * neo_profile(1) resets and enables, neo_profile(0) resets and disables; neo_profile_read synchronises. */

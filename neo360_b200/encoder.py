@@ -11,7 +11,12 @@
                                                                    DepthPillarEncoder, three pillar aggregators, softmax-weighted pillar sums
                                                                    (2.7 TFLOP per scene) -- runs in hand-written CUDA on the tensor cores
                                                                    (`neo_grid_encoder_dense`, csrc/encoder.cu + csrc/gemm_tc.cu) when no
-                                                                   gradient is required; under autograd the same algebra runs as framework ops.
+                                                                   gradient is required.  Under autograd on CUDA tensors (`dense_train`) the
+                                                                   grid lookup and the softmax pillar sums run forward and backward in
+                                                                   hand-written fp32 CUDA (`neo_grid_encoder_features(_bwd)`,
+                                                                   `neo_grid_encoder_pool(_bwd)`) and the dense layers as framework fp32
+                                                                   GEMMs; under autograd on the CPU the same algebra runs as framework ops
+                                                                   (`dense_torch`).
 """
 from __future__ import annotations
 
@@ -97,6 +102,67 @@ def _floorplan_convnet():
         nn.Conv2d(128, 128, 3, padding=1))
 
 
+def _stream():
+    return torch.cuda.current_stream().cuda_stream
+
+
+class _Features(torch.autograd.Function):
+    """Grid lookup rows: latent_cl (NV,Hl,Wl,512) channel-last -> X (NV*G^3, 518) = [latent lookup | cam xyz | masked unit direction], the
+    input of depth_fc.  Returned as a view of a 520-wide buffer (16-byte rows); the gradient flows to the latent only (poses do not train)."""
+
+    @staticmethod
+    def forward(ctx, latent_cl, poses, focal, cx, cy, W, H):
+        lib = L.load()
+        lat = latent_cl.detach().contiguous().float()
+        nv, lh, lw, _ = lat.shape
+        pose_c = poses.detach().contiguous().float()
+        X = torch.empty(nv * GridEncoder.GRID ** 3, 520, device=lat.device)
+        geo = (nv, lh, lw, int(W), int(H))
+        with torch.cuda.device(lat.device):
+            L.check(lib.neo_grid_encoder_features(L.ptr(lat), *geo, L.ptr(pose_c), focal, cx, cy, L.ptr(X), X.shape[1], _stream()))
+        ctx.save_for_backward(pose_c)
+        ctx.geo, ctx.cam = geo, (focal, cx, cy)
+        return X[:, :518]
+
+    @staticmethod
+    def backward(ctx, g_X):
+        lib = L.load()
+        (pose_c,) = ctx.saved_tensors
+        nv, lh, lw, _, _ = ctx.geo
+        g = g_X.contiguous().float()
+        g_lat = torch.zeros(nv, lh, lw, 512, device=g.device)
+        with torch.cuda.device(g.device):
+            L.check(lib.neo_grid_encoder_features_bwd(*ctx.geo, L.ptr(pose_c), *ctx.cam, L.ptr(g), g.stride(0), L.ptr(g_lat), _stream()))
+        return g_lat, None, None, None, None, None, None
+
+
+class _Pool(torch.autograd.Function):
+    """Softmax pillar sums: lat (NV*G^3, 512), logits (3, NV*G^3) by axis (yz, xz, xy) -> floor plans xz, xy, yz (NV,512,G,G)."""
+
+    @staticmethod
+    def forward(ctx, lat, logits):
+        lib = L.load()
+        lat_c, lg = lat.detach().contiguous().float(), logits.detach().contiguous().float()
+        G = GridEncoder.GRID
+        nv = lat_c.shape[0] // G ** 3
+        out = [torch.empty(nv, 512, G, G, device=lat_c.device) for _ in range(3)]
+        with torch.cuda.device(lat_c.device):
+            L.check(lib.neo_grid_encoder_pool(L.ptr(lat_c), L.ptr(lg), nv, *[L.ptr(t) for t in out], _stream()))
+        ctx.save_for_backward(lat_c, lg)
+        return tuple(out)
+
+    @staticmethod
+    def backward(ctx, g_xz, g_xy, g_yz):
+        lib = L.load()
+        lat_c, lg = ctx.saved_tensors
+        nv = lat_c.shape[0] // GridEncoder.GRID ** 3
+        d_lat, d_logits = torch.empty_like(lat_c), torch.empty_like(lg)
+        gs = [None if g is None else g.contiguous().float() for g in (g_xz, g_xy, g_yz)]
+        with torch.cuda.device(lat_c.device):
+            L.check(lib.neo_grid_encoder_pool_bwd(L.ptr(lat_c), L.ptr(lg), nv, *[L.ptr(g) for g in gs], L.ptr(d_lat), L.ptr(d_logits), _stream()))
+        return d_lat, d_logits
+
+
 class GridEncoder(nn.Module):
     GRID = 64
 
@@ -142,6 +208,33 @@ class GridEncoder(nn.Module):
         fp = lambda t: t.permute(0, 3, 1, 2)
         return fp((lat * w_xz).sum(2)), fp((lat * w_xy).sum(3)), fp((lat * w_yz).sum(1))      # xz, xy, yz: (NV, 512, 64, 64)
 
+    # ---- the dense part for training on CUDA: hand-written lookup and pillar sums (forward and backward), framework fp32 GEMMs ----
+    def dense_train(self, latent, poses, focal, c, W, H):
+        """The algebra of `dense_torch`, differentiable with respect to `latent` and every parameter of depth_fc and the three aggregators.
+        The dense layers are fp32 `F.linear` on the modules' own parameters (TF32 when torch.backends.cuda.matmul.allow_tf32 is set); each
+        aggregator's coordinate input (column 512) is applied as a rank-1 term over the grid axis it depends on."""
+        if not latent.is_cuda:
+            raise RuntimeError("neo360_b200 needs CUDA tensors (no CPU fallback)")
+        G, NV = self.GRID, latent.shape[0]
+        lin = lambda m, x: F.linear(x, m.weight, m.bias)
+        X = _Features.apply(latent.permute(0, 2, 3, 1), poses, float(focal[0]), float(c[0, 0]), float(c[0, 1]), W, H)
+        fc = self.depth_fc
+        h = torch.relu_(lin(fc.common_branch[0], X))
+        h = torch.relu_(lin(fc.common_branch[2], h))
+        lat = lin(fc.depth_encoder, h)                                                    # (NV*G^3, 512)
+        ax = [torch.linspace(-1, 1, G, device=latent.device), torch.linspace(-1, 1, G, device=latent.device),
+              torch.linspace(0, 1, G, device=latent.device)]
+        logits = []
+        for axis, name in enumerate(("yz", "xz", "xy")):
+            agg = getattr(self, f"pillar_aggregator_{name}")
+            w0 = agg[0].weight
+            shape = [1, 1, 1, 1]
+            shape[1 + axis] = G
+            a = F.linear(lat, w0[:, :512], agg[0].bias)
+            a.view(NV, G, G, G, -1).add_(ax[axis].reshape(*shape, 1) * w0[:, 512])           # + coordinate (x, y or z) times column 512
+            logits.append(lin(agg[2], torch.relu_(a)).reshape(-1))
+        return _Pool.apply(lat, torch.stack(logits))
+
     # ---- the dense part, hand-written CUDA (wgmma) ----
     def dense_cuda(self, latent, poses, focal, c, W, H):
         if not latent.is_cuda:
@@ -175,9 +268,11 @@ class GridEncoder(nn.Module):
         """images (NV,3,H,W), poses (NV,4,4) camera-to-world, focal (NV,), c (NV,2) -> scene_grid_xz, scene_grid_xy, scene_grid_yz (NV,128,120,160)."""
         NV, _, H, W = images.shape
         latent = self.spatial_encoder(images)
-        needs_grad = torch.is_grad_enabled() and (latent.requires_grad or any(q.requires_grad for q in self.depth_fc.parameters()))
+        trained = [self.depth_fc, self.pillar_aggregator_xz, self.pillar_aggregator_yz, self.pillar_aggregator_xy]
+        needs_grad = torch.is_grad_enabled() and (latent.requires_grad or any(q.requires_grad for m in trained for q in m.parameters()))
         if needs_grad:
-            fxz, fxy, fyz = self.dense_torch(latent, poses.float(), focal.float(), c.float(), W, H)
+            dense = self.dense_train if latent.is_cuda else self.dense_torch
+            fxz, fxy, fyz = dense(latent, poses.float(), focal.float(), c.float(), W, H)
         else:
             fxz, fxy, fyz = self.dense_cuda(latent, poses, focal, c, W, H)
         return self.floorplan_convnet_xz(fxz), self.floorplan_convnet_xy(fxy), self.floorplan_convnet_yz(fyz)

@@ -385,13 +385,15 @@ def bench_train(args, rank, world, local, dev, dist, pk, base, sampler, timed):
                         "batch_rays": per * world, "rays_per_rank": per, "samples": "128+64",
                         "precision": "fp32 (reference formulation)" + ("; framework GEMMs / convolutions in TF32 (the reference's torch-1.11 default)" if tf32 else ""),
                         "parallelism": f"data parallel x{world}: one all-reduce over a flat {state['grad_elems']}-element gradient slab per step",
-                        "encoder": "GridEncoder inside the step (framework ops under autograd), its gradients in the all-reduced slab" if with_encoder
+                        "encoder": "GridEncoder inside the step (dense_train: grid lookup and softmax pillar sums forward / backward in hand-written "
+                                   "CUDA, dense layers as framework GEMMs; ResNet and conv stacks framework), its gradients in the all-reduced slab"
+                                   if with_encoder
                                    else "frozen / absent: encoder outputs are leaf tensors (finetune mode, model.py:969-979)",
                         "batch": "pix_inds drawn on the host as the reference dataset does, rays + targets of the sampled pixels generated on the device "
                                  "from 20 resident target views (neo_sample_rays)",
                         "formulation": "projected maps: [W0_map; W3_map] applied to the 0.4 M map texels once per step under autograd, lookups of 2x256 projected "
                                        "channels, K=63|84 input layers (exact re-association)" if net.train_projected
                                        else "reference: row-by-row K=703/831 input layers on the looked-up 640 raw channels",
-                        "hand_written": "pixel sampling, ray sampling, lookups fwd/bwd, compositing fwd/bwd", "library": "dense layers and encoder (autograd), Adam"},
+                        "hand_written": "pixel sampling, ray sampling, lookups fwd/bwd, compositing fwd/bwd", "library": "dense layers, encoder GEMMs and convolutions (autograd), Adam"},
                 e2e={"value": rays / (ms * 1e-3), "unit": "rays/s", "h2d_bytes_per_step": per * 8, "d2h_bytes_per_step": 4},
                 final_loss=loss, clocks=sampler.result() if sampler else None)
