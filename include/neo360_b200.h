@@ -168,11 +168,15 @@ int neo_sample_rays(int n, const long long* pix_inds, int n_views, int H, int W,
 int neo_intersect_sphere(const float* rays_o, const float* rays_d, int n_rays, float* far, int* err_flag,
                          void* stream);
 /* models/neo360/helper.py:24-75.  in_sphere=1: t (n,N+1), pts (n,N+1,3).  in_sphere=0: t=s (n,N+1) descending,
- * pts (n,N+1,4), pts_linear (n,N+1,3).  u_rand NULL = deterministic. */
+ * pts (n,N+1,4), pts_linear (n,N+1,3).  u_rand NULL = deterministic.  far (n) and t_vals are always read / written, rays_o / rays_d
+ * when pts or pts_linear is given; a NULL one of these, or in_sphere other than 0 / 1, is NEO_ERR_INVALID. */
 int neo_sample_along_rays(const float* rays_o, const float* rays_d, const float* far, int n_rays, int num_samples,
                           int in_sphere, float far_uncontracted, const float* u_rand, float* t_vals, float* pts,
                           float* pts_linear, void* stream);
-/* models/neo360/helper.py:218-249 (sorted_piecewise_constant_pdf 174-215 inside): bins=mids(t_old), weights[1:-1]. */
+/* models/neo360/helper.py:218-249 (sorted_piecewise_constant_pdf 174-215 inside): bins=mids(t_old), weights[1:-1].  t_old / weights
+ * (n,n_old), n_old >= 4; t_vals (n,n_old+num_samples), ascending for in_sphere=1, descending for 0 (bg s).  far is not read (the bg
+ * lookup points use the sphere intersection of rays_o / rays_d) and may be NULL; rays_o / rays_d are read only for pts / pts_linear.
+ * NULL t_old / weights / t_vals, pts or pts_linear without rays_o / rays_d, or in_sphere other than 0 / 1 is NEO_ERR_INVALID. */
 int neo_sample_pdf(const float* rays_o, const float* rays_d, const float* far, const float* t_old,
                    const float* weights, int n_rays, int n_old, int num_samples, int in_sphere,
                    float far_uncontracted, const float* u_rand, float* t_vals, float* pts, float* pts_linear,

@@ -118,8 +118,13 @@ __global__ void resample_kernel(const float* __restrict__ s_prev, const float* _
     }
     if (lane == 0) { cw[0] = 0.f; cw[ns - 1] = 1.0f; }
     __syncwarp();
+    // quirk Q18: a NaN logit (anneal 0 on an empty-weight, non-empty interval: 0 * log 0) or all logits -inf make the reference's
+    // softmax NaN; cumsum and clip keep the NaN and sorted_interp's min then puts every centre on the first knot.  With one weight the
+    // reference cdf is [0, 1] whatever the softmax, so the ordinary path below already agrees.  (se is warp-uniform.)
+    const bool collapse = (se != se) && nw >= 2;
     // centres = sorted_interp(u, cw, td) ; reuse wd for the centres
     for (int k = lane; k < n_new; k += 32) {
+        if (collapse) { wd[k] = td[0]; continue; }
         float u;
         if (jitter) {
             const float u_max = kEps + (1.f - kEps) / (float)n_new;

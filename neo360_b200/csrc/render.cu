@@ -173,12 +173,22 @@ extern "C" int neo_intersect_sphere(const float* o, const float* d, int n, float
 extern "C" int neo_sample_along_rays(const float* o, const float* d, const float* far, int n, int num_samples, int in_sphere,
                                      float far_unc, const float* u_rand, float* t, float* pts, float* pts_lin, void* stream) {
     if (n <= 0 || num_samples < 1) { set_error("neo_sample_along_rays: bad sizes"); return NEO_ERR_INVALID; }
+    if (in_sphere < 0 || in_sphere > 1) { set_error("neo_sample_along_rays: in_sphere must be 0 or 1 (got %d)", in_sphere); return NEO_ERR_INVALID; }
+    if (!far || !t || ((pts || pts_lin) && (!o || !d))) {
+        set_error("neo_sample_along_rays: null far / t_vals, or pts / pts_linear without rays_o / rays_d");
+        return NEO_ERR_INVALID;
+    }
     return launch_sample_coarse(o, d, far, n, num_samples, in_sphere, far_unc, u_rand, t, pts, pts_lin, (cudaStream_t)stream);
 }
 extern "C" int neo_sample_pdf(const float* o, const float* d, const float* far, const float* t_old, const float* weights, int n,
                               int n_old, int num_samples, int in_sphere, float far_unc, const float* u_rand, float* t, float* pts,
                               float* pts_lin, void* stream) {
     if (n <= 0) { set_error("neo_sample_pdf: n_rays <= 0"); return NEO_ERR_INVALID; }
+    if (in_sphere < 0 || in_sphere > 1) { set_error("neo_sample_pdf: in_sphere must be 0 or 1 (got %d)", in_sphere); return NEO_ERR_INVALID; }
+    if (!t_old || !weights || !t || ((pts || pts_lin) && (!o || !d))) {
+        set_error("neo_sample_pdf: null t_old / weights / t_vals, or pts / pts_linear without rays_o / rays_d");
+        return NEO_ERR_INVALID;
+    }
     return launch_resample(o, d, far, t_old, weights, n, n_old, num_samples, in_sphere, far_unc, u_rand, t, pts, pts_lin, (cudaStream_t)stream);
 }
 extern "C" int neo_volumetric_rendering(const float* rgb, const float* sigma, const float* t, const float* d, const float* far, int n,

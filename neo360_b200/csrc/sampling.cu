@@ -246,9 +246,11 @@ __global__ void resample_kernel(const float* __restrict__ o, const float* __rest
     __syncwarp();
     // sort buffer: old values then new samples, padded with +inf
     for (int j = lane; j < p2; j += 32) srt[j] = (j < n_old) ? tb[j] : INFINITY;
+    __syncwarp();   // lane j % 32 pads srt[j] and lane q % 32 writes srt[n_old + q]: the padding must land first
     for (int q = lane; q < m; q += 32) {
         float u = u_rand ? u_rand[(long long)b * m + q] : linspace01(q, m);   // linspace(0, 1-2^-32, m): end == 1.0f (Q7)
-        // idx = last j with cdf[j] <= u   (cdf non-decreasing, cdf[0] = 0 <= u)
+        // a j with cdf[j] <= u < cdf[j+1] (the last such j while the fp32 cdf is non-decreasing; where two lanes rounded a zero-weight
+        // bin differently it can step back one ulp, and the search then returns one valid bracket of the several)
         int lo = 0, hi = K;               // invariant: cdf[lo] <= u, (hi == K or cdf[hi] > u)
         while (hi - lo > 1) {
             int mid = (lo + hi) >> 1;
