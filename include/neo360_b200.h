@@ -203,6 +203,19 @@ int neo_index_local(const NeoScene* scene, const float* pts, int M, float* out, 
 /* Output side (models/interface.py:53-61, LitModel.psnr_each): *out_sum (device double) = sum_i (clip(pred_i,0,1) - clip(gt_i,0,1))^2 over n
  * floats; PSNR = -10 log10(out_sum / n). */
 int neo_clipped_sq_err(const float* pred, const float* gt, long long n, double* out_sum, void* stream);
+/* Object PSNR (models/utils.py:102-109 get_obj_rgbs_from_segmap, then psnr_each): pred / gt (n_pix, 3), mask (n_pix) one byte per pixel,
+ * non-zero = selected.  *out_sum (device double) = the same sum over the values of the selected pixels only, *out_count (device) = their
+ * number (3 per pixel); object PSNR = -10 log10(out_sum / out_count), NaN when out_count is 0.  The kernel of neo_clipped_sq_err. */
+int neo_clipped_sq_err_masked(const float* pred, const float* gt, const uint8_t* mask, long long n_pix, double* out_sum,
+                              unsigned long long* out_count, void* stream);
+/* SSIM as LitModel.ssim_each computes it with piqa's SSIM() at its defaults (models/interface.py:101-111; definition in
+ * csrc/metrics.cu): pred / gt (n, H, W, 3) fp32 channel-last, clipped to [0, 1] inside.  ssim (n) device doubles, one per frame;
+ * ss_map (n, H-10, W-10, 3) fp32 or NULL.  Workspace: neo_ssim_workspace_bytes(n, H, W) bytes, 8-byte aligned, caller-owned (0 = invalid
+ * sizes).  NULL pred / gt / ssim / workspace, n < 1, H or W < 11, or a size past int64 elements is NEO_ERR_INVALID before any launch.
+ * No floating-point atomics: two calls are bit-identical, and a frame gives the same bits alone or inside any batch. */
+size_t neo_ssim_workspace_bytes(int n, int H, int W);
+int neo_ssim(const float* pred, const float* gt, int n, int H, int W, double* ssim, float* ss_map, void* workspace, size_t workspace_bytes,
+             void* stream);
 
 /* ---- backward of the hand-written stages (training: models/neo360/model.py:697-820 differentiates through this path) ----
  * The field's backward is split: the lookups' scatter and the compositing backward are the entry points below; the dense layers of

@@ -106,6 +106,9 @@ SYMBOLS = {
     "neo_index_grid": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "neo_index_local": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "neo_clipped_sq_err": (C.c_int, [C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p]),
+    "neo_clipped_sq_err_masked": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "neo_ssim_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "neo_ssim": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "neo_volumetric_rendering_bwd": (C.c_int, [C.c_void_p] * 5 + [C.c_int] * 4 + [C.c_void_p] * 8),
     "neo_index_grid_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_index_local_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),

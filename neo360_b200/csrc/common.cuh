@@ -287,7 +287,9 @@ int launch_composite_bwd(const float* rgb, const float* sigma, const float* t, c
 int launch_combine(int n, int N, const float* fg_c, const float* bg_c, const float* lam, const float* fg_depth,
                    const float* bg_depth, const float* fg_t, const float* bg_s, float* comp, float* depth,
                    float* fg_sdist, float* bg_sdist, cudaStream_t s);
-int launch_clipped_sq_err(const float* a, const float* b, long long n, double* out, cudaStream_t s);
+// mask NULL: every value; otherwise one byte per (pixel, 3) value triple, and *count = the number of values summed
+int launch_clipped_sq_err(const float* a, const float* b, const unsigned char* mask, long long n, double* out, unsigned long long* count,
+                          cudaStream_t s);
 int launch_sample_rays(int n, const long long* pix, int T, int H, int W, float focal, const float* c2w, const float* images,
                        float* o, float* vd, float* rd, float* radii, float* target, int* err, cudaStream_t s);
 int launch_get_rays(int H, int W, float focal, const float* c2w, float* o, float* vd, float* rd, float* radii,

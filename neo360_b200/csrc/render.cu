@@ -204,7 +204,15 @@ extern "C" int neo_volumetric_rendering(const float* rgb, const float* sigma, co
 }
 extern "C" int neo_clipped_sq_err(const float* pred, const float* gt, long long n, double* out_sum, void* stream) {
     if (n <= 0 || !pred || !gt || !out_sum) { set_error("neo_clipped_sq_err: bad arguments"); return NEO_ERR_INVALID; }
-    return launch_clipped_sq_err(pred, gt, n, out_sum, (cudaStream_t)stream);
+    return launch_clipped_sq_err(pred, gt, nullptr, n, out_sum, nullptr, (cudaStream_t)stream);
+}
+extern "C" int neo_clipped_sq_err_masked(const float* pred, const float* gt, const uint8_t* mask, long long n_pix, double* out_sum,
+                                         unsigned long long* out_count, void* stream) {
+    if (n_pix <= 0 || n_pix > (1LL << 61) || !pred || !gt || !mask || !out_sum || !out_count) {
+        set_error("neo_clipped_sq_err_masked: bad arguments (NULL buffer or n_pix %lld outside [1, 2^61])", n_pix);
+        return NEO_ERR_INVALID;
+    }
+    return launch_clipped_sq_err(pred, gt, mask, 3 * n_pix, out_sum, out_count, (cudaStream_t)stream);
 }
 extern "C" int neo_volumetric_rendering_bwd(const float* rgb, const float* sigma, const float* t, const float* d, const float* far, int n, int N,
                                             int white, int in_sphere, const float* g_comp, const float* g_acc, const float* g_w,

@@ -522,16 +522,36 @@ int launch_combine(int n, int N, const float* fg_c, const float* bg_c, const flo
 // ------------------------------------------------------------------------------------------------
 // output side (SURVEY.md 8(f4)): sum of squared differences of two images after clipping to [0,1] -- the reduction under
 // LitModel.psnr_each (models/interface.py:53-61).  Grid-stride, warp + block reduction, one double atomicAdd per block.
+// MASKED: the object PSNR of get_obj_rgbs_from_segmap (models/utils.py:102-109): only the values of pixels whose mask byte is non-zero
+// (mask has one byte per pixel, the values are (pixel, 3) channel-last) enter the sum, and *count receives their number.
 // ------------------------------------------------------------------------------------------------
-__global__ void clipped_sq_err_kernel(const float* __restrict__ a, const float* __restrict__ b, long long n, double* __restrict__ out) {
+template <bool MASKED>
+__global__ void clipped_sq_err_kernel(const float* __restrict__ a, const float* __restrict__ b, const unsigned char* __restrict__ mask,
+                                      long long n, double* __restrict__ out, unsigned long long* __restrict__ count) {
     double acc = 0.0;
+    unsigned long long cnt = 0;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        if (MASKED) {
+            if (!mask[i / 3]) continue;
+            ++cnt;
+        }
         const float x = fminf(fmaxf(a[i], 0.f), 1.f) - fminf(fmaxf(b[i], 0.f), 1.f);
         acc += (double)(x * x);
     }
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
     __shared__ double red[8];
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+    if (MASKED) {
+        for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+        __shared__ unsigned long long red_cnt[8];
+        if ((threadIdx.x & 31) == 0) red_cnt[threadIdx.x >> 5] = cnt;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            unsigned long long c = 0;
+            for (int w = 0; w < (int)(blockDim.x >> 5); ++w) c += red_cnt[w];
+            atomicAdd(count, c);
+        }
+    }
     __syncthreads();
     if (threadIdx.x == 0) {
         double t = 0.0;
@@ -539,10 +559,15 @@ __global__ void clipped_sq_err_kernel(const float* __restrict__ a, const float* 
         atomicAdd(out, t);
     }
 }
-int launch_clipped_sq_err(const float* a, const float* b, long long n, double* out, cudaStream_t s) {
+int launch_clipped_sq_err(const float* a, const float* b, const unsigned char* mask, long long n, double* out, unsigned long long* count,
+                          cudaStream_t s) {
     NEO_CUDA(cudaMemsetAsync(out, 0, sizeof(double), s));
+    if (mask) NEO_CUDA(cudaMemsetAsync(count, 0, sizeof(unsigned long long), s));
     const int blocks = (int)((n + 255) / 256 < 592 ? (n + 255) / 256 : 592);
-    clipped_sq_err_kernel<<<blocks > 0 ? blocks : 1, 256, 0, s>>>(a, b, n, out);
+    if (mask)
+        clipped_sq_err_kernel<true><<<blocks > 0 ? blocks : 1, 256, 0, s>>>(a, b, mask, n, out, count);
+    else
+        clipped_sq_err_kernel<false><<<blocks > 0 ? blocks : 1, 256, 0, s>>>(a, b, nullptr, n, out, nullptr);
     NEO_LAUNCH_CHECK("clipped_sq_err_kernel");
     return NEO_OK;
 }
