@@ -196,6 +196,23 @@ int neo_index_maps(const NeoScene* scene, const float* pts, int M, int C, const 
  * and gradient maps must be 16-byte aligned (float4 reductions). */
 int neo_index_maps_bwd(const NeoScene* scene, const float* pts, int M, int C, const float* g_local, const float* g_world,
                        float* g_latent_cl, float* g_xz_cl, float* g_xy_cl, float* g_yz_cl, void* stream);
+/* Deterministic form of neo_index_maps_bwd, the same contract (accumulates into caller-zeroed maps, the same NULL and alignment rules) plus a
+ * caller-owned workspace (16-byte aligned) of at least neo_index_maps_bwd_det_workspace_bytes(scene, M, C) bytes (0 = bad arguments or a
+ * CUDA error).  No floating-point atomics: two calls are bit-identical.  neo_index_grid_bwd is this call with g_world and C = 128,
+ * neo_index_local_bwd with g_local and C = 512.  Algorithm (csrc/det.cu): one entry per (view, point, tap, map), taps bit for bit the
+ * forward's; a stable radix sort of (texel key, entry id); then each touched texel is written once, map = map + w * g summed in sorted order
+ * as fp32 round-to-nearest multiply then add.
+ * With rows = nv*M, the entries are:  local (if g_local) e = r*4 + tap, row r of g_local;  world (if g_world) e = E_local + r*12 + plane*4 + tap,
+ * row r of g_world (planes xz, xy, yz), E_local = 4 rows if g_local else 0.  E = the entry count.  Texel keys: latent (if g_local)
+ * v*lat_h*lat_w + texel, then plane p of view v at T_lat + (p*nv + v)*plane_h*plane_w + texel; T = the texel count; a zero-weight tap has
+ * the key T and is not summed.  Workspace blocks, in this order, each at the next multiple of 256 bytes from the workspace start:
+ * keys (E u32, entry order), sorted keys (E u32), entry ids (E u32), sorted entry ids (E u32), weights (E f32, entry order), segment
+ * starts (T + 1 u32: the first sorted position with key >= k), sort scratch.  The sorted entries (texel, row, weight) are
+ * (sorted key[i], row of sorted id[i], weight[sorted id[i]]).  Any entry past 2^31 - 2, or texel count, is NEO_ERR_INVALID. */
+size_t neo_index_maps_bwd_det_workspace_bytes(const NeoScene* scene, int M, int C);
+int neo_index_maps_bwd_det(const NeoScene* scene, const float* pts, int M, int C, const float* g_local, const float* g_world,
+                           float* g_latent_cl, float* g_xz_cl, float* g_xy_cl, float* g_yz_cl, void* workspace, size_t workspace_bytes,
+                           void* stream);
 /* encoder_tp_fusion_conv.py:122-209: pts (M,3) world -> (nv*M,128), rows ordered (view, point). */
 int neo_index_grid(const NeoScene* scene, const float* pts, int M, float* out, void* stream);
 /* model.py:239-264 (get_local_feats): pts (M,3) world -> (nv*M,512). */
@@ -382,6 +399,14 @@ int neo_grid_encoder_features(const float* latent_cl, int nv, int lat_h, int lat
  * even, 8-byte aligned; columns >= 512 are not read (poses do not train).  The taps are the forward's, bit for bit. */
 int neo_grid_encoder_features_bwd(int nv, int lat_h, int lat_w, int img_w, int img_h, const float* src_poses, float focal, float cx, float cy,
                                   const float* g_X, long long ldg, float* g_latent_cl, void* stream);
+/* Deterministic form of neo_grid_encoder_features_bwd, the same geometry, contract and argument rules plus a caller-owned 16-byte aligned
+ * workspace of neo_grid_encoder_features_bwd_det_workspace_bytes(nv, lat_h, lat_w) bytes (0 = bad sizes or a CUDA error).  The order-fixed
+ * scatter of neo_index_maps_bwd_det: entries e = row*4 + tap (row of g_X), keys v*lat_h*lat_w + texel (T = nv*lat_h*lat_w for a zero weight),
+ * the same workspace layout with E = 4 nv 64^3.  g_X is read as float2 pairs.  Two calls are bit-identical. */
+size_t neo_grid_encoder_features_bwd_det_workspace_bytes(int nv, int lat_h, int lat_w);
+int neo_grid_encoder_features_bwd_det(int nv, int lat_h, int lat_w, int img_w, int img_h, const float* src_poses, float focal, float cx,
+                                      float cy, const float* g_X, long long ldg, float* g_latent_cl, void* workspace, size_t workspace_bytes,
+                                      void* stream);
 /* Softmax pillar sums: lat (nv*64^3, 512) row-major, 16-byte aligned, logits (3, nv*64^3) by axis -> floor plans (nv,512,64,64) NCHW. */
 int neo_grid_encoder_pool(const float* lat, const float* logits, int nv, float* floor_xz, float* floor_xy, float* floor_yz, void* stream);
 /* Backward of neo_grid_encoder_pool: upstream g_xz / g_xy / g_yz (nv,512,64,64), each may be NULL (zero) -> d_lat (nv*64^3, 512) = the
@@ -389,6 +414,30 @@ int neo_grid_encoder_pool(const float* lat, const float* logits, int nv, float* 
  * floating-point atomics (two calls give bit-identical results). */
 int neo_grid_encoder_pool_bwd(const float* lat, const float* logits, int nv, const float* g_xz, const float* g_xy, const float* g_yz,
                               float* d_lat, float* d_logits, void* stream);
+
+/* ---- per-ray training losses and the encoder's upsampling adjoint, for training under torch.use_deterministic_algorithms (csrc/det.cu):
+ * one warp per ray with fixed-order sums, every output written once, no floating-point atomics; two calls are bit-identical.  All return
+ * NEO_ERR_INVALID before any launch on a NULL buffer they read or write or a size out of range. ---- */
+/* training.distortion_loss per ray: loss[r] = 1/3 sum_i I_i w_i^2 + 2 sum_k (w_k m_k W_<k - w_k (wm)_<k), W_<k = sum_{i<k} w_i, exactly as
+ * written (for descending m this is minus sum w_i w_j |m_i - m_j|, as the reference's eff_distloss gives).  w, m (n,N); interval (n,N) or
+ * NULL = interval_scalar for every sample.  The caller takes the mean over rays. */
+int neo_distortion_loss(const float* w, const float* m, const float* interval, float interval_scalar, int n, int N, float* loss, void* stream);
+/* d_w (n,N) = g_loss[r] * d loss[r] / d w (m and interval carry no gradient). */
+int neo_distortion_loss_bwd(const float* w, const float* m, const float* interval, float interval_scalar, int n, int N, const float* g_loss,
+                            float* d_w, void* stream);
+/* One proposal level of the Mip-NeRF 360 interlevel loss per ray (helper.py:117-141 lossfun_outer): sdist (n,Nc+1), weights (n,Nc) of the
+ * NeRF level, sdist_env (n,Np+1), weights_env (n,Np) of the proposal level.  r_i = the number of sdist_env knots <= sdist_i (searchsorted
+ * right=True), lo_i = max(r_i - 1, 0), hi_i = min(r_i, Np); w_outer_j = sum of weights_env over [lo_j, hi_{j+1}) in ascending order;
+ * loss[r] = sum_j clip(w_j - w_outer_j, 0)^2 / (w_j + 1.1920929e-07) / Nc.  1 <= Nc <= 1024. */
+int neo_interlevel_loss(const float* sdist, const float* weights, const float* sdist_env, const float* weights_env, int n, int Nc, int Np,
+                        float* loss, void* stream);
+/* d_weights_env (n,Np) = g_loss[r] * d loss[r] / d weights_env. */
+int neo_interlevel_loss_bwd(const float* sdist, const float* weights, const float* sdist_env, const float* weights_env, int n, int Nc, int Np,
+                            const float* g_loss, float* d_weights_env, void* stream);
+/* Adjoint of F.interpolate(mode="bilinear", align_corners=True) on NCHW fp32: g_out (planes, H_out, W_out) -> g_in (planes, H_in, W_in),
+ * every element written once as a gather over the output rows / columns whose taps reach it, with the tap weights of ATen's
+ * upsample_bilinear2d forward (source index scale * o in fp32, scale = (in-1)/(out-1)). */
+int neo_upsample_bilinear_bwd(const float* g_out, long long planes, int H_in, int W_in, int H_out, int W_out, float* g_in, void* stream);
 
 /* bench support: CUDA events around every field-kernel launch on the launching stream + launch accounting.
  * neo_profile(1) resets and enables, neo_profile(0) resets and disables; neo_profile_read synchronises. */

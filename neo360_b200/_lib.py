@@ -98,6 +98,8 @@ SYMBOLS = {
     "neo_index_maps": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_index_maps_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_void_p]),
+    "neo_index_maps_bwd_det_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int, C.c_int]),
+    "neo_index_maps_bwd_det": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 7 + [C.c_size_t, C.c_void_p]),
     "neo_get_rays": (C.c_int, [C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_intersect_sphere": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_sample_along_rays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -135,6 +137,14 @@ SYMBOLS = {
                                             C.c_void_p, C.c_int, C.c_void_p]),
     "neo_grid_encoder_features_bwd": (C.c_int, [C.c_int] * 5 + [C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_longlong, C.c_void_p,
                                                                 C.c_void_p]),
+    "neo_grid_encoder_features_bwd_det_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "neo_grid_encoder_features_bwd_det": (C.c_int, [C.c_int] * 5 + [C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_longlong,
+                                                                    C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "neo_distortion_loss": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "neo_distortion_loss_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "neo_interlevel_loss": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 3 + [C.c_void_p, C.c_void_p]),
+    "neo_interlevel_loss_bwd": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 3 + [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "neo_upsample_bilinear_bwd": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "neo_grid_encoder_pool": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 4),
     "neo_grid_encoder_pool_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 6),
     "neo_profile": (C.c_int, [C.c_int]),

@@ -305,6 +305,29 @@ int launch_index_maps_bwd(const NeoScene* sc, const float* pts, int M, int C, co
                           float* g_xy, float* g_yz, cudaStream_t s);
 int launch_index_bwd(const NeoScene* sc, const float* pts, int M, int local, const float* g_out, float* g_lat, float* g_xz, float* g_xy,
                      float* g_yz, cudaStream_t s);
+// det.cu: order-fixed scatter (deterministic adjoint of the lookups).  The caller's entry kernel writes, for entry e in [0, E), keys[e]
+// (texel key in [0, T), or T for a zero-weight tap), ids[e] = e and wts[e]; det_sort_reduce sorts and reduces.  Workspace blocks, in
+// this order and each starting on a 256-byte boundary of the workspace: keys, keys_sorted, ids, ids_sorted (E u32 each), wts (E f32),
+// starts (T + 1 u32), sort scratch.
+struct DetBuffers {
+    unsigned *keys, *keys_sorted, *ids, *ids_sorted;
+    float* wts;
+    unsigned* starts;
+    void* scratch;
+    size_t scratch_bytes, total;     // total = 0: the sort's scratch query failed (neo_last_error says why)
+};
+DetBuffers det_carve(void* ws, long long E, long long T);
+// Entry e belongs to source s = (e >= e0[1]), row (e - e0[s]) / taps[s] of g[s] (row stride ld[s] floats).
+struct DetSrc { const float* g[2]; long long ld[2]; unsigned e0[2]; int taps[2]; };
+// Keys [key0[m], key0[m+1]) address map m (channel-last rows of C floats); unused maps repeat the last key0.
+constexpr int kDetMaps = 4;
+struct DetDst { float* map[kDetMaps]; long long key0[kDetMaps]; };
+// vec = 4: rows and maps are read as float4 (C % 4 == 0, 16-byte aligned); 2: float2 (C, ld even, 8-byte aligned)
+int det_sort_reduce(const DetBuffers& b, long long E, long long T, int C, int vec, const DetSrc& src, const DetDst& dst, cudaStream_t s);
+int launch_index_maps_bwd_det(const NeoScene* sc, const float* pts, int M, int C, const float* g_local, const float* g_world, float* g_lat,
+                              float* g_xz, float* g_xy, float* g_yz, const DetBuffers& b, cudaStream_t s);
+// E and T of neo_index_maps_bwd_det for the maps that receive a gradient
+void index_det_sizes(const NeoScene* sc, int M, bool local, bool world, long long& E, long long& T);
 // field_tc.cu
 int tc_scene_create(NeoScene* sc, const NeoMLPParams mlps[4], cudaStream_t s);
 void tc_scene_free(NeoScene* sc);

@@ -113,6 +113,25 @@ __global__ void __launch_bounds__(128) grid_gather_bwd_kernel(int lh, int lw, co
     }
 }
 
+// entries of the same adjoint for the order-fixed scatter (csrc/det.cu): e = row*4 + tap, key = v*lh*lw + texel, or T for a zero weight
+__global__ void grid_gather_entries_kernel(long long rows, int lh, int lw, const float* __restrict__ poses, float focal, float cx, float cy,
+                                           float sx, float sy, unsigned T, unsigned* __restrict__ keys, unsigned* __restrict__ ids,
+                                           float* __restrict__ wts) {
+    const long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (row >= rows) return;
+    CellView cv;
+    cell_view(row, lh, lw, poses, focal, cx, cy, sx, sy, cv);
+    const unsigned base = (unsigned)(row / kNC) * lh * lw;
+#pragma unroll
+    for (int tp = 0; tp < 4; ++tp) {
+        const unsigned e = (unsigned)row * 4 + tp;
+        const float w = cv.t.w[tp];
+        keys[e] = w != 0.f ? base + cv.t.idx[tp] : T;
+        ids[e] = e;
+        wts[e] = w;
+    }
+}
+
 // column 512 of every row = the world coordinate of its cell along `axis` (the aggregator's extra input); columns 513.. = 0
 __global__ void coord_col_kernel(__half* __restrict__ L, long long rows, int axis) {
     const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -382,6 +401,53 @@ extern "C" int neo_grid_encoder_features_bwd(int nv, int lat_h, int lat_w, int i
                                                                                               ldg, g_latent_cl);
     NEO_LAUNCH_CHECK("grid_gather_bwd_kernel");
     return NEO_OK;
+}
+
+// E = nv * 64^3 * 4 entries, T = nv * lat_h * lat_w texels
+static bool features_det_sizes(const char* who, int nv, int lat_h, int lat_w, long long& E, long long& T) {
+    E = 4LL * nv * enc::kNC;
+    T = (long long)nv * lat_h * lat_w;
+    if (nv < 1 || lat_h < 2 || lat_w < 2 || E >= (1LL << 31) - 1 || T >= (1LL << 31) - 1) {
+        set_error("%s: bad sizes (nv %d, latent %dx%d) or more than 2^31 - 2 entries", who, nv, lat_h, lat_w);
+        return false;
+    }
+    return true;
+}
+
+extern "C" size_t neo_grid_encoder_features_bwd_det_workspace_bytes(int nv, int lat_h, int lat_w) {
+    long long E, T;
+    if (!features_det_sizes("neo_grid_encoder_features_bwd_det_workspace_bytes", nv, lat_h, lat_w, E, T)) return 0;
+    return det_carve(nullptr, E, T).total;
+}
+
+extern "C" int neo_grid_encoder_features_bwd_det(int nv, int lat_h, int lat_w, int img_w, int img_h, const float* src_poses, float focal, float cx,
+                                                 float cy, const float* g_X, long long ldg, float* g_latent_cl, void* workspace,
+                                                 size_t workspace_bytes, void* stream) {
+    using namespace enc;
+    if (!enc_geometry_ok("neo_grid_encoder_features_bwd_det", nv, lat_h, lat_w, img_w, img_h, src_poses)) return NEO_ERR_INVALID;
+    if (!g_X || !g_latent_cl || !workspace || ldg < kLat || ldg % 2 || !aligned(g_X, 8) || !aligned(g_latent_cl, 16) || !aligned(workspace, 16)) {
+        set_error("neo_grid_encoder_features_bwd_det: NULL buffer, g_X not 8-byte aligned with an even row stride >= 512 (got %lld), or the "
+                  "gradient map / workspace not 16-byte aligned", ldg);
+        return NEO_ERR_INVALID;
+    }
+    long long E, T;
+    if (!features_det_sizes("neo_grid_encoder_features_bwd_det", nv, lat_h, lat_w, E, T)) return NEO_ERR_INVALID;
+    const DetBuffers b = det_carve(workspace, E, T);
+    if (!b.total) return NEO_ERR_CUDA;
+    if (workspace_bytes < b.total) {
+        set_error("neo_grid_encoder_features_bwd_det: workspace of %zu bytes, %zu needed", workspace_bytes, b.total);
+        return NEO_ERR_INVALID;
+    }
+    float sx, sy;
+    lat_scale(lat_h, lat_w, img_w, img_h, sx, sy);
+    cudaStream_t s = (cudaStream_t)stream;
+    const long long rows = (long long)nv * kNC;
+    grid_gather_entries_kernel<<<(unsigned)((rows + 127) / 128), 128, 0, s>>>(rows, lat_h, lat_w, src_poses, focal, cx, cy, sx, sy, (unsigned)T,
+                                                                             b.keys, b.ids, b.wts);
+    NEO_LAUNCH_CHECK("grid_gather_entries_kernel");
+    const DetSrc src{{g_X, g_X}, {ldg, ldg}, {0u, 0xffffffffu}, {4, 4}};
+    const DetDst dst{{g_latent_cl, g_latent_cl, g_latent_cl, g_latent_cl}, {0, T, T, T}};
+    return det_sort_reduce(b, E, T, kLat, 2, src, dst, s);
 }
 
 extern "C" int neo_grid_encoder_pool(const float* lat, const float* logits, int nv, float* floor_xz, float* floor_xy, float* floor_yz, void* stream) {

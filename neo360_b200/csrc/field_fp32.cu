@@ -368,4 +368,64 @@ int launch_index_maps_bwd(const NeoScene* sc, const float* pts, int M, int C, co
     return NEO_OK;
 }
 
+// ---- deterministic backward (csrc/det.cu): the entries of the scatter that index_bwd_kernel does with atomics ----
+// Row r = v*M + m.  Local entries e = r*4 + tap, key = v*Hl*Wl + texel; world entries e = e0 + r*12 + plane*4 + tap,
+// key = key0 + (plane*nv + v)*Hp*Wp + texel (planes xz, xy, yz).  A zero-weight tap gets the key `T` and is never reduced.
+__global__ void index_entries_kernel(SceneDev sc, const float* __restrict__ pts, int M, int local, unsigned e0, unsigned key0, unsigned T,
+                                     unsigned* __restrict__ keys, unsigned* __restrict__ ids, float* __restrict__ wts) {
+    const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= (long long)sc.nv * M) return;
+    const int v = (int)(r / M), m = (int)(r % M);
+    float c[3];
+    to_camera(sc.views[v], pts + 3 * (size_t)m, c);
+    auto put = [&](unsigned e, unsigned key, float w) { keys[e] = w != 0.f ? key : T; ids[e] = e; wts[e] = w; };
+    if (local) {
+        float gx, gy;
+        Taps t;
+        local_grid_coords(sc, c, gx, gy);
+        bilinear_taps(gx, gy, sc.lat_w, sc.lat_h, t);
+        const unsigned base = key0 + (unsigned)v * sc.lat_h * sc.lat_w;
+        for (int tp = 0; tp < 4; ++tp) put(e0 + (unsigned)r * 4 + tp, base + t.idx[tp], t.w[tp]);
+    } else {
+        const float ga[3] = {c[0], c[0], c[1]}, gb[3] = {c[2], c[1], c[2]};
+        const unsigned hw = (unsigned)sc.plane_h * sc.plane_w;
+        for (int pi = 0; pi < 3; ++pi) {
+            Taps t;
+            bilinear_taps(ga[pi], gb[pi], sc.plane_w, sc.plane_h, t);
+            const unsigned base = key0 + ((unsigned)pi * sc.nv + v) * hw;
+            for (int tp = 0; tp < 4; ++tp) put(e0 + (unsigned)r * 12 + pi * 4 + tp, base + t.idx[tp], t.w[tp]);
+        }
+    }
+}
+
+void index_det_sizes(const NeoScene* sc, int M, bool local, bool world, long long& E, long long& T) {
+    const long long rows = (long long)sc->dev.nv * M;
+    E = (local ? 4 * rows : 0) + (world ? 12 * rows : 0);
+    T = (local ? (long long)sc->dev.nv * sc->dev.lat_h * sc->dev.lat_w : 0) + (world ? 3LL * sc->dev.nv * sc->dev.plane_h * sc->dev.plane_w : 0);
+}
+
+int launch_index_maps_bwd_det(const NeoScene* sc, const float* pts, int M, int C, const float* g_local, const float* g_world, float* g_lat,
+                              float* g_xz, float* g_xy, float* g_yz, const DetBuffers& b, cudaStream_t s) {
+    long long E, T;
+    index_det_sizes(sc, M, g_local != nullptr, g_world != nullptr, E, T);
+    const long long rows = (long long)sc->dev.nv * M;
+    const unsigned grid = (unsigned)((rows + 127) / 128);
+    const long long T_lat = g_local ? (long long)sc->dev.nv * sc->dev.lat_h * sc->dev.lat_w : 0;
+    const unsigned e_world = g_local ? (unsigned)(4 * rows) : 0u;
+    if (g_local) {
+        index_entries_kernel<<<grid, 128, 0, s>>>(sc->dev, pts, M, 1, 0u, 0u, (unsigned)T, b.keys, b.ids, b.wts);
+        NEO_LAUNCH_CHECK("index_entries_kernel(local)");
+    }
+    if (g_world) {
+        index_entries_kernel<<<grid, 128, 0, s>>>(sc->dev, pts, M, 0, e_world, (unsigned)T_lat, (unsigned)T, b.keys, b.ids, b.wts);
+        NEO_LAUNCH_CHECK("index_entries_kernel(world)");
+    }
+    const long long hw = (long long)sc->dev.nv * sc->dev.plane_h * sc->dev.plane_w;
+    DetSrc src{{g_local ? g_local : g_world, g_world}, {C, C}, {0u, g_local && g_world ? e_world : 0xffffffffu}, {g_local ? 4 : 12, 12}};
+    DetDst dst{{g_local ? g_lat : g_xz, g_xz, g_xy, g_yz}, {0, T_lat, T_lat + hw, T_lat + 2 * hw}};
+    if (!g_local) dst = DetDst{{g_xz, g_xy, g_yz, g_yz}, {0, hw, 2 * hw, 3 * hw}};
+    else if (!g_world) dst = DetDst{{g_lat, g_lat, g_lat, g_lat}, {0, T, T, T}};
+    return det_sort_reduce(b, E, T, C, 4, src, dst, s);
+}
+
 }  // namespace neo

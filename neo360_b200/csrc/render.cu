@@ -255,6 +255,49 @@ extern "C" int neo_index_maps_bwd(const NeoScene* sc, const float* pts, int M, i
     }
     return launch_index_maps_bwd(sc, pts, M, C, g_local, g_world, g_latent_cl, g_xz_cl, g_xy_cl, g_yz_cl, (cudaStream_t)stream);
 }
+namespace {
+// entry ids and keys are 32-bit; the sort's item count is an int
+bool det_sizes_ok(const char* who, long long E, long long T) {
+    if (E >= (1LL << 31) - 1 || T >= (1LL << 31) - 1) { set_error("%s: %lld entries / %lld texels exceed 2^31 - 2", who, E, T); return false; }
+    return true;
+}
+}  // namespace
+extern "C" size_t neo_index_maps_bwd_det_workspace_bytes(const NeoScene* sc, int M, int C) {
+    if (!sc || M <= 0 || C < 4 || (C % 4)) { set_error("neo_index_maps_bwd_det_workspace_bytes: bad arguments"); return 0; }
+    size_t need = 0;
+    for (int which = 1; which <= 3; ++which) {             // local only, world only, both: the largest layout
+        long long E, T;
+        index_det_sizes(sc, M, which & 1, which & 2, E, T);
+        if (!det_sizes_ok("neo_index_maps_bwd_det_workspace_bytes", E, T)) return 0;
+        const DetBuffers b = det_carve(nullptr, E, T);
+        if (!b.total) return 0;
+        need = b.total > need ? b.total : need;
+    }
+    return need;
+}
+extern "C" int neo_index_maps_bwd_det(const NeoScene* sc, const float* pts, int M, int C, const float* g_local, const float* g_world, float* g_latent_cl,
+                                      float* g_xz_cl, float* g_xy_cl, float* g_yz_cl, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!sc || M <= 0 || !pts || C < 4 || (C % 4) || (g_local && !g_latent_cl) || (g_world && !(g_xz_cl && g_xy_cl && g_yz_cl)) || !(g_local || g_world) ||
+        !workspace) {
+        set_error("neo_index_maps_bwd_det: bad arguments");
+        return NEO_ERR_INVALID;
+    }
+    if (!aligned16(g_local) || !aligned16(g_world) || !aligned16(g_latent_cl) || !aligned16(g_xz_cl) || !aligned16(g_xy_cl) || !aligned16(g_yz_cl) ||
+        !aligned16(workspace)) {
+        set_error("neo_index_maps_bwd_det: row gradients, gradient maps and the workspace must be 16-byte aligned");
+        return NEO_ERR_INVALID;
+    }
+    long long E, T;
+    index_det_sizes(sc, M, g_local != nullptr, g_world != nullptr, E, T);
+    if (!det_sizes_ok("neo_index_maps_bwd_det", E, T)) return NEO_ERR_INVALID;
+    const DetBuffers b = det_carve(workspace, E, T);
+    if (!b.total) return NEO_ERR_CUDA;
+    if (workspace_bytes < b.total) {
+        set_error("neo_index_maps_bwd_det: workspace of %zu bytes, %zu needed", workspace_bytes, b.total);
+        return NEO_ERR_INVALID;
+    }
+    return launch_index_maps_bwd_det(sc, pts, M, C, g_local, g_world, g_latent_cl, g_xz_cl, g_xy_cl, g_yz_cl, b, (cudaStream_t)stream);
+}
 extern "C" int neo_index_grid(const NeoScene* sc, const float* pts, int M, float* out, void* stream) {
     if (!sc || M <= 0 || !sc->dev.planes_cl[0]) { set_error("neo_index_grid: needs a scene prepared with NEO_PREC_FP32"); return NEO_ERR_INVALID; }
     return launch_index_grid(sc, pts, M, out, (cudaStream_t)stream);

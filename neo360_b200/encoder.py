@@ -22,6 +22,7 @@ from __future__ import annotations
 
 import ctypes as C
 import functools
+import math
 
 import torch
 import torch.nn as nn
@@ -50,6 +51,48 @@ class _ResNet34Trunk(nn.Module):
         self.layer1, self.layer2, self.layer3 = net.layer1, net.layer2, net.layer3
 
 
+class _UpsampleBilinear(torch.autograd.Function):
+    """F.interpolate(x, size, mode="bilinear", align_corners=True) with the gather adjoint neo_upsample_bilinear_bwd as its backward (every
+    input element written once, no atomics).  The forward is F.interpolate itself, so values are bit-identical."""
+
+    @staticmethod
+    def forward(ctx, x, size):
+        ctx.in_shape = x.shape
+        return F.interpolate(x, size, mode="bilinear", align_corners=True)
+
+    @staticmethod
+    def backward(ctx, g):
+        lib = L.load()
+        n, c, hi, wi = ctx.in_shape
+        gc = g.contiguous().float()
+        g_in = torch.empty(ctx.in_shape, device=gc.device)
+        with torch.cuda.device(gc.device):
+            L.check(lib.neo_upsample_bilinear_bwd(L.ptr(gc), n * c, hi, wi, gc.shape[-2], gc.shape[-1], L.ptr(g_in), _stream()))
+        return g_in, None
+
+
+def upsample_bilinear(x, size):
+    """F.interpolate(x, size, mode="bilinear", align_corners=True).  Under torch.use_deterministic_algorithms, where the framework's backward
+    of this op raises, a CUDA input that needs a gradient goes through `_UpsampleBilinear`."""
+    if torch.are_deterministic_algorithms_enabled() and x.is_cuda and torch.is_grad_enabled() and x.requires_grad:
+        return _UpsampleBilinear.apply(x, tuple(int(v) for v in size))
+    return F.interpolate(x, size, mode="bilinear", align_corners=True)
+
+
+class _Upsample(nn.Upsample):
+    """nn.Upsample(mode="bilinear", align_corners=True) that differentiates through `upsample_bilinear` (no parameters or buffers, so the
+    state dict is nn.Upsample's)."""
+
+    def forward(self, x):
+        if torch.are_deterministic_algorithms_enabled() and x.is_cuda and torch.is_grad_enabled() and x.requires_grad:
+            if self.size is not None:
+                size = self.size
+            else:
+                size = [int(math.floor(d * self.scale_factor)) for d in x.shape[-2:]]
+            return upsample_bilinear(x, size)
+        return super().forward(x)
+
+
 class SpatialEncoder(nn.Module):
     """encoder_pn.py:32-210 with the reference's defaults as GridEncoder passes them (resnet34, 4 layers, bilinear, zeros padding)."""
 
@@ -70,7 +113,7 @@ class SpatialEncoder(nn.Module):
         x = self.model.layer3(x)
         feats.append(x)
         size = feats[0].shape[-2:]
-        self.latent = torch.cat([F.interpolate(f, size, mode="bilinear", align_corners=True) for f in feats], 1)
+        self.latent = torch.cat([upsample_bilinear(f, size) for f in feats], 1)
         ls = torch.tensor([self.latent.shape[-1], self.latent.shape[-2]], dtype=torch.float32, device=self.latent.device)
         self.latent_scaling = ls / (ls - 1) * 2.0
         return self.latent
@@ -96,9 +139,9 @@ def _floorplan_convnet():
         nn.Conv2d(512, 256, 3, stride=2, padding=1), nn.BatchNorm2d(256), nn.ReLU(inplace=True),
         nn.Conv2d(256, 128, 3, stride=2, padding=1), nn.BatchNorm2d(128), nn.ReLU(inplace=True),
         nn.Conv2d(128, 128, 3, stride=1, padding=1), nn.BatchNorm2d(128), nn.ReLU(inplace=True),
-        nn.Upsample(scale_factor=2, mode="bilinear", align_corners=True),
+        _Upsample(scale_factor=2, mode="bilinear", align_corners=True),
         nn.Conv2d(128, 128, 3, padding=1), nn.BatchNorm2d(128), nn.ReLU(inplace=True),
-        nn.Upsample(size=(120, 160), mode="bilinear", align_corners=True),
+        _Upsample(size=(120, 160), mode="bilinear", align_corners=True),
         nn.Conv2d(128, 128, 3, padding=1))
 
 
@@ -122,6 +165,7 @@ class _Features(torch.autograd.Function):
             L.check(lib.neo_grid_encoder_features(L.ptr(lat), *geo, L.ptr(pose_c), focal, cx, cy, L.ptr(X), X.shape[1], _stream()))
         ctx.save_for_backward(pose_c)
         ctx.geo, ctx.cam = geo, (focal, cx, cy)
+        ctx.det = torch.are_deterministic_algorithms_enabled()
         return X[:, :518]
 
     @staticmethod
@@ -132,7 +176,15 @@ class _Features(torch.autograd.Function):
         g = g_X.contiguous().float()
         g_lat = torch.zeros(nv, lh, lw, 512, device=g.device)
         with torch.cuda.device(g.device):
-            L.check(lib.neo_grid_encoder_features_bwd(*ctx.geo, L.ptr(pose_c), *ctx.cam, L.ptr(g), g.stride(0), L.ptr(g_lat), _stream()))
+            if ctx.det:                 # order-fixed scatter: bit-reproducible
+                need = lib.neo_grid_encoder_features_bwd_det_workspace_bytes(nv, lh, lw)
+                if need == 0:
+                    L.check(-1)
+                ws = torch.empty(need, dtype=torch.uint8, device=g.device)
+                L.check(lib.neo_grid_encoder_features_bwd_det(*ctx.geo, L.ptr(pose_c), *ctx.cam, L.ptr(g), g.stride(0), L.ptr(g_lat), L.ptr(ws),
+                                                              need, _stream()))
+            else:
+                L.check(lib.neo_grid_encoder_features_bwd(*ctx.geo, L.ptr(pose_c), *ctx.cam, L.ptr(g), g.stride(0), L.ptr(g_lat), _stream()))
         return g_lat, None, None, None, None, None, None
 
 

@@ -230,19 +230,55 @@ def _outer_weights(t: torch.Tensor, t_env: torch.Tensor, w_env: torch.Tensor) ->
     return torch.gather(cy, -1, hi)[..., 1:] - torch.gather(cy, -1, lo)[..., :-1]
 
 
+class _Interlevel(torch.autograd.Function):
+    """One proposal level of the interlevel loss per ray (neo_interlevel_loss, backward neo_interlevel_loss_bwd): sdist (n,Nc+1), weights
+    (n,Nc) of the NeRF level (no gradient), sdist_env (n,Np+1), weights_env (n,Np) of the proposal level -> (n,); the gradient flows to
+    weights_env.  Fixed-order sums, no atomics."""
+
+    @staticmethod
+    def forward(ctx, c, w, t_env, w_env):
+        lib = L.load()
+        ts = [x.detach().contiguous().float() for x in (c, w, t_env, w_env)]
+        n, Nc = ts[1].shape
+        Np = ts[3].shape[1]
+        out = torch.empty(n, device=ts[0].device)
+        with torch.cuda.device(out.device):
+            L.check(lib.neo_interlevel_loss(*[L.ptr(x) for x in ts], n, Nc, Np, L.ptr(out), torch.cuda.current_stream(out.device).cuda_stream))
+        ctx.save_for_backward(*ts)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        lib = L.load()
+        ts = ctx.saved_tensors
+        n, Nc = ts[1].shape
+        Np = ts[3].shape[1]
+        d_we = torch.empty_like(ts[3])
+        with torch.cuda.device(d_we.device):
+            L.check(lib.neo_interlevel_loss_bwd(*[L.ptr(x) for x in ts], n, Nc, Np, L.ptr(g.contiguous().float()), L.ptr(d_we),
+                                                torch.cuda.current_stream(d_we.device).cuda_stream))
+        return None, None, None, d_we
+
+
 def training_loss(renderings: List[dict], ray_history: List[dict], target: torch.Tensor, charb_padding: float = 0.001,
                   interlevel_mult: float = 1.0, distortion_mult: float = 0.01) -> torch.Tensor:
     """LitMipNeRF360.training_step's loss (model.py:442-449): sqrt(mse + charb_padding^2) of the last rendering, plus the interlevel loss
     (lossfun_outer of every proposal level against the detached NeRF-level sdist / weights, model.py:725-734, helper.py:138-141), plus
     distortion_mult times the distortion loss of the NeRF level (model.py:736-741, helper.py:145-152; `training.distortion_loss` is the same
-    functional in O(N) form for ascending sdist)."""
+    functional in O(N) form for ascending sdist).  Under torch.use_deterministic_algorithms on CUDA tensors the interlevel terms come from
+    neo_interlevel_loss (the same searchsorted / lo / hi semantics as `_outer_weights`, without its cumulative sums)."""
     mse = ((renderings[-1]["rgb"] - target) ** 2).mean()
     loss = torch.sqrt(mse + charb_padding ** 2)
     last = ray_history[-1]
     c, w = last["sdist"].detach(), last["weights"].detach()
     eps = 1.1920929e-07                                                           # helper.py:18
     inter = 0.0
+    det = torch.are_deterministic_algorithms_enabled() and c.is_cuda           # torch.cumsum raises in deterministic mode
     for h in ray_history[:-1]:
+        if det:
+            inter = inter + _Interlevel.apply(c.reshape(-1, c.shape[-1]), w.reshape(-1, w.shape[-1]), h["sdist"].reshape(-1, h["sdist"].shape[-1]),
+                                              h["weights"].reshape(-1, h["weights"].shape[-1])).mean()
+            continue
         w_outer = _outer_weights(c, h["sdist"], h["weights"])
         inter = inter + (torch.clip(w - w_outer, min=0) ** 2 / (w + eps)).mean()
     s, wl = last["sdist"], last["weights"]

@@ -16,6 +16,8 @@ What runs where
     differentiates through the projection, so the map-column weights and the encoder outputs get exactly the reference's gradients (to
     fp32 re-association).  `train_projected = False` keeps the reference formulation row by row.
   * NCCL: ONE all-reduce over the flat gradient slab of the four MLPs per step (`allreduce_flat`), as the reference's DDP does.
+  * under torch.use_deterministic_algorithms(True) the lookups' backward is the order-fixed `neo_index_maps_bwd_det` (sort + segmented
+    reduction, bit-reproducible) and the distortion loss comes from `neo_distortion_loss`; with the flag off the code above runs unchanged.
 There is no CPU fallback: every op raises on CPU tensors.
 """
 from __future__ import annotations
@@ -37,6 +39,19 @@ def _stream():
     return torch.cuda.current_stream().cuda_stream
 
 
+def _index_maps_bwd_det(sc, p, M, Cc, g_local, g_world, g_lat, g_pl):
+    """neo_index_maps_bwd_det (no floating-point atomics, bit-reproducible) with a workspace of the queried size; a None row gradient skips
+    its maps."""
+    lib = L.load()
+    need = lib.neo_index_maps_bwd_det_workspace_bytes(sc.handle, M, Cc)
+    if need == 0:
+        L.check(-1)
+    ws = torch.empty(need, dtype=torch.uint8, device=p.device)
+    f = lambda g: None if g is None else g.contiguous().float()
+    L.check(lib.neo_index_maps_bwd_det(sc.handle, L.ptr(p), M, Cc, L.ptr(f(g_local)), L.ptr(f(g_world)), L.ptr(g_lat), *[L.ptr(t) for t in g_pl],
+                                       L.ptr(ws), need, _stream()))
+
+
 class _Lookup(torch.autograd.Function):
     """index_grid + get_local_feats (encoder_tp_fusion_conv.py:122-209, model.py:239-264) of world points (M,3):
     -> world (NV*M,128), local (NV*M,512); gradients flow to the three tri-planes and the latent image."""
@@ -55,6 +70,7 @@ class _Lookup(torch.autograd.Function):
         ctx.save_for_backward(p)
         ctx.net, ctx.scene = net, sc
         ctx.shapes = (planes_xz.shape, latent.shape)
+        ctx.det = torch.are_deterministic_algorithms_enabled()
         return world, local
 
     @staticmethod
@@ -67,9 +83,13 @@ class _Lookup(torch.autograd.Function):
         g_planes = [torch.zeros(nv, hp, wp, cw, device=p.device) for _ in range(3)]
         g_lat = torch.zeros(nv, hl, wl, cl, device=p.device)
         with torch.cuda.device(p.device):
-            L.check(lib.neo_index_grid_bwd(sc.handle, L.ptr(p), M, L.ptr(g_world.contiguous().float()), L.ptr(g_planes[0]), L.ptr(g_planes[1]),
-                                           L.ptr(g_planes[2]), _stream()))
-            L.check(lib.neo_index_local_bwd(sc.handle, L.ptr(p), M, L.ptr(g_local.contiguous().float()), L.ptr(g_lat), _stream()))
+            if ctx.det:
+                _index_maps_bwd_det(sc, p, M, cw, None, g_world, None, g_planes)
+                _index_maps_bwd_det(sc, p, M, cl, g_local, None, g_lat, [None] * 3)
+            else:
+                L.check(lib.neo_index_grid_bwd(sc.handle, L.ptr(p), M, L.ptr(g_world.contiguous().float()), L.ptr(g_planes[0]),
+                                               L.ptr(g_planes[1]), L.ptr(g_planes[2]), _stream()))
+                L.check(lib.neo_index_local_bwd(sc.handle, L.ptr(p), M, L.ptr(g_local.contiguous().float()), L.ptr(g_lat), _stream()))
         nchw = lambda t: t.permute(0, 3, 1, 2)
         return None, nchw(g_planes[0]), nchw(g_planes[1]), nchw(g_planes[2]), nchw(g_lat), None
 
@@ -92,6 +112,7 @@ class _LookupMaps(torch.autograd.Function):
         ctx.save_for_backward(p)
         ctx.scene, ctx.C = sc, Cc
         ctx.shapes = (lat_cl.shape, xz_cl.shape)
+        ctx.det = torch.are_deterministic_algorithms_enabled()
         return local, world
 
     @staticmethod
@@ -103,8 +124,12 @@ class _LookupMaps(torch.autograd.Function):
         g_lat = torch.zeros(ctx.shapes[0], device=p.device)
         g_pl = [torch.zeros(ctx.shapes[1], device=p.device) for _ in range(3)]
         with torch.cuda.device(p.device):
-            L.check(lib.neo_index_maps_bwd(sc.handle, L.ptr(p), M, Cc, L.ptr(g_local.contiguous().float()), L.ptr(g_world.contiguous().float()),
-                                           L.ptr(g_lat), L.ptr(g_pl[0]), L.ptr(g_pl[1]), L.ptr(g_pl[2]), _stream()))
+            if ctx.det:
+                _index_maps_bwd_det(sc, p, M, Cc, g_local, g_world, g_lat, g_pl)
+            else:
+                L.check(lib.neo_index_maps_bwd(sc.handle, L.ptr(p), M, Cc, L.ptr(g_local.contiguous().float()),
+                                               L.ptr(g_world.contiguous().float()), L.ptr(g_lat), L.ptr(g_pl[0]), L.ptr(g_pl[1]), L.ptr(g_pl[2]),
+                                               _stream()))
         return None, g_lat, g_pl[0], g_pl[1], g_pl[2], None
 
 
@@ -276,9 +301,40 @@ def render_train(net, rays: Dict[str, Tensor], planes: List[Tensor], latent: Ten
     return ret
 
 
+class _Distortion(torch.autograd.Function):
+    """Per-ray distortion regulariser (neo_distortion_loss, backward neo_distortion_loss_bwd): w, m, interval (n,N) -> (n,).  Fixed-order
+    sums, no atomics; m and interval carry no gradient."""
+
+    @staticmethod
+    def forward(ctx, w, m, interval):
+        lib = L.load()
+        wc, mc, ic = (t.detach().contiguous().float() for t in (w, m, interval))
+        n, N = wc.shape
+        out = torch.empty(n, device=wc.device)
+        with torch.cuda.device(wc.device):
+            L.check(lib.neo_distortion_loss(L.ptr(wc), L.ptr(mc), L.ptr(ic), 0.0, n, N, L.ptr(out), _stream()))
+        ctx.save_for_backward(wc, mc, ic)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        lib = L.load()
+        wc, mc, ic = ctx.saved_tensors
+        n, N = wc.shape
+        d_w = torch.empty_like(wc)
+        with torch.cuda.device(wc.device):
+            L.check(lib.neo_distortion_loss_bwd(L.ptr(wc), L.ptr(mc), L.ptr(ic), 0.0, n, N, L.ptr(g.contiguous().float()), L.ptr(d_w), _stream()))
+        return d_w, None, None
+
+
 def distortion_loss(w: Tensor, m: Tensor, interval: Tensor) -> Tensor:
     """The O(N) form of the regulariser the reference applies through `eff_distloss` (models/neo360/model.py:1246-1260; same functional
-    as the in-tree O(N^2) lossfun_distortion, helper.py:111-118):  1/3 sum_i interval_i w_i^2 + 2 sum_i w_i (m_i W_{<i} - (wm)_{<i})."""
+    as the in-tree O(N^2) lossfun_distortion, helper.py:111-118):  1/3 sum_i interval_i w_i^2 + 2 sum_i w_i (m_i W_{<i} - (wm)_{<i}).
+    Under torch.use_deterministic_algorithms on CUDA tensors (where torch.cumsum raises) the per-ray values come from neo_distortion_loss."""
+    if torch.are_deterministic_algorithms_enabled() and w.is_cuda:
+        N = w.shape[-1]
+        flat = lambda t: t.expand_as(w).reshape(-1, N)
+        return _Distortion.apply(w.reshape(-1, N), flat(m), flat(interval)).mean()
     loss_uni = (1.0 / 3.0) * (interval * w.pow(2)).sum(-1).mean()
     wm = w * m
     w_cum, wm_cum = w.cumsum(-1), wm.cumsum(-1)
