@@ -84,7 +84,33 @@ struct Params {
     float* rgb_out;
     float* sigma_out;
     int* trap;          // host-mapped int[8]: who timed out on the weight-load mbarrier
+#ifdef NEO_FIELD_PHASES
+    int phase_slot;     // row of g_phase_cycles this launch adds to
+#endif
 };
+
+// Phase clocks (diagnostic build only, -DNEO_FIELD_PHASES; read by tools/field_phases.py): thread 0 of every warpgroup adds the
+// clock64() cycles between consecutive marks to its phase, and at the end of the kernel the warpgroup's sums (and its tile count) go
+// into the launch's row of g_phase_cycles.  The marks bound the phases as the compiler scheduled them, which is close to, but not
+// exactly, the source order.  Without the macro the kernel has no marks at all.
+#ifdef NEO_FIELD_PHASES
+constexpr int kPhases = 8;          // tile setup | camera + encodings | tap table | blend P0 | layers 0-2 | blend P3 | layer 3 + head | colour head + stores
+constexpr uint32_t kPhaseBytes = kWarpgroups * (kPhases + 1) * 8;        // per-warpgroup sums in shared memory
+constexpr int kPhaseSlots = 64;
+__device__ unsigned long long g_phase_cycles[kPhaseSlots][kPhases + 1];    // [launch][phase], column kPhases: tiles
+static int g_phase_launches = 0;
+#define FIELD_PHASE_INIT() long long ph_t = clock64()
+#define FIELD_PHASE(p)                                   \
+    do {                                                 \
+        const long long now_ = clock64();                \
+        if (wt == 0) ph_acc[wg][p] += now_ - ph_t;       \
+        ph_t = now_;                                     \
+    } while (0)
+#else
+constexpr uint32_t kPhaseBytes = 0;
+#define FIELD_PHASE_INIT() do {} while (0)
+#define FIELD_PHASE(p) do {} while (0)
+#endif
 
 // ------------------------------------------------------------------------------------------------
 // per-scene preparation kernels
@@ -310,37 +336,61 @@ __device__ __forceinline__ void seed_bias(float (&d)[NC / 2], const float* b, in
 // descriptor of k-step ks of a 128-byte-swizzled K-major weight tile whose 64-column slabs are `slab` bytes apart
 __device__ __forceinline__ uint64_t wdesc(uint32_t base, int ks, uint32_t slab) { return desc_sw128(base + (uint32_t)(ks >> 2) * slab + (uint32_t)(ks & 3) * 32u); }
 
+// Tap table of one (tile, view), per warpgroup in shared memory: for every point n of the tile and map m (latent, xz, xy, yz), the
+// texel indices (view included) of the four taps {nw, ne, sw, se} and their bilinear weights.  Split in two arrays of 16-byte
+// entries [m][n], so that the 8 points a warp reads at once fall on distinct banks.
+struct TapTable {
+    int4 tex[4][kTilePts];
+    float4 w[4][kTilePts];
+};
+__device__ __forceinline__ int comp4(const int4& x, int k) { return k == 0 ? x.x : k == 1 ? x.y : k == 2 ? x.z : x.w; }
+__device__ __forceinline__ float comp4(const float4& x, int k) { return k == 0 ? x.x : k == 1 ? x.y : k == 2 ? x.z : x.w; }
+
+// entry (point n, map m) of the tap table from the camera-frame lookup point cl: grid_sample(bilinear, align_corners=True, zeros)
+// taps of the map in source view v.  A tap out of range has weight 0, which the blend skips, and index 0, so that every index in the
+// table is a texel of the map.
+__device__ __forceinline__ void tap_entry(TapTable& tab, const SceneDev& sc, const float (&cl)[3], int v, int n, int m) {
+    float gx, gy;
+    int mw, mh;
+    if (m == 0) {
+        local_grid_coords(sc, cl, gx, gy);
+        mw = sc.lat_w; mh = sc.lat_h;
+    } else {
+        gx = (m == 3) ? cl[1] : cl[0];
+        gy = (m == 2) ? cl[1] : cl[2];          // xz, xy, yz
+        mw = sc.plane_w; mh = sc.plane_h;
+    }
+    TapQuad tq;
+    tap_quad(gx, gy, mw, mh, tq);
+    int tx[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) tx[k] = tq.w[k] == 0.f ? 0 : (v * mh + tq.y0 + (k >> 1)) * mw + tq.x0 + (k & 1);
+    tab.tex[m][n] = make_int4(tx[0], tx[1], tx[2], tx[3]);
+    tab.w[m][n] = make_float4(tq.w[0], tq.w[1], tq.w[2], tq.w[3]);
+}
+
 // acc[4 j + 2 i + e] += bilinear blend (grid_sample, align_corners=True, zeros) of channel 8 j + 2 t + e of half HALF of [P0 | P3]
-// over the four maps, at this thread's two points (camera-frame lookup points cl[i]) in source view v; fp32 blend of fp16 texels
+// over the four maps, at this thread's two points (rows r0, r0 + 8 of the tile); fp32 blend of fp16 texels.
+// The taps' geometry comes from the tap table; the taps are still fetched one at a time: each tap's four 16-byte loads sit behind
+// its zero-weight skip, and the FMAs that use them follow.  (Issuing a map's four taps ahead of their FMAs needs the skip replaced
+// by masking, 64 more live registers and the FMAs of out-of-range taps; measured on H100 that made the field launches 10 % slower
+// than this form, see DESIGN.md §5.)
 template <int HALF>
-__device__ __forceinline__ void blend_maps(float (&acc)[64], const Params& P, const float (&cl)[2][3], int v, int t) {
-    const SceneDev& sc = P.sc;
+__device__ __forceinline__ void blend_maps(float (&acc)[64], const Params& P, const TapTable& tab, int r0, int t) {
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
 #pragma unroll 1
         for (int m = 0; m < 4; ++m) {
-            float gx, gy;
-            int mw, mh;
-            if (m == 0) {
-                local_grid_coords(sc, cl[i], gx, gy);
-                mw = sc.lat_w; mh = sc.lat_h;
-            } else {
-                gx = (m == 3) ? cl[i][1] : cl[i][0];
-                gy = (m == 2) ? cl[i][1] : cl[i][2];          // xz, xy, yz
-                mw = sc.plane_w; mh = sc.plane_h;
-            }
-            TapQuad tq;
-            tap_quad(gx, gy, mw, mh, tq);
-            const __half* base = P.mlp.pmap[m] + (size_t)v * mh * mw * 256 + HALF * 128 + t * 32;
+            const int4 tx = tab.tex[m][r0 + 8 * i];
+            const float4 wv = tab.w[m][r0 + 8 * i];
+            const uint4* base = reinterpret_cast<const uint4*>(P.mlp.pmap[m] + HALF * 128 + t * 32);
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
-                const float w = tq.w[k];
-                if (w == 0.f) continue;                        // out-of-range tap (zeros padding): its texel index may be invalid
-                const int x = tq.x0 + (k & 1), y = tq.y0 + (k >> 1);
-                const uint4* p = reinterpret_cast<const uint4*>(base + ((size_t)y * mw + x) * 256);
+                const float w = comp4(wv, k);
+                if (w == 0.f) continue;                                // out-of-range tap (zeros padding): no contribution
                 uint4 q[4];
 #pragma unroll
-                for (int u = 0; u < 4; ++u) q[u] = __ldg(p + u);
+                for (int u = 0; u < 4; ++u) q[u] = __ldg(base + (size_t)comp4(tx, k) * 32 + u);   // 32 uint4 per texel
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
                     const uint32_t wd[4] = {q[u].x, q[u].y, q[u].z, q[u].w};
@@ -360,7 +410,9 @@ __device__ __forceinline__ void blend_maps(float (&acc)[64], const Params& P, co
 template <int KE>
 struct SmemMap {
     static constexpr uint32_t HEAD = trunk_bytes(KE), BIAS = HEAD + WH_BYTES, VIEWS = BIAS + BIAS_BYTES,
-                              PTS = VIEWS + kMaxViews * 64, BAR = PTS + kWarpgroups * kTilePts * (uint32_t)sizeof(PtsRow), TOTAL = BAR + 16;
+                              PTS = VIEWS + kMaxViews * 64, TAPS = PTS + kWarpgroups * kTilePts * (uint32_t)sizeof(PtsRow),
+                              BAR = TAPS + kWarpgroups * (uint32_t)sizeof(TapTable), PHASES = BAR + 16, TOTAL = PHASES + kPhaseBytes;
+    static_assert(TOTAL + 1024 <= 227u * 1024u, "field kernel shared memory exceeds the 227 KB an sm_90 CTA can have");
 };
 
 template <int ICH>
@@ -388,16 +440,22 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
         const float* vsrc = reinterpret_cast<const float*>(P.sc.views);
         for (int i = threadIdx.x; i < P.nv * 16; i += kThreads) vsm[i] = __ldg(vsrc + i);
     }
+#ifdef NEO_FIELD_PHASES
+    auto ph_acc = reinterpret_cast<unsigned long long (*)[kPhases + 1]>(sgen + SM::PHASES);
+    if (threadIdx.x < kWarpgroups * (kPhases + 1)) (&ph_acc[0][0])[threadIdx.x] = 0ull;
+#endif
     __syncthreads();
     if (!mbar_wait_bounded(bar, 0)) load_timeout(P.trap, bar);
 
     const int wg = threadIdx.x >> 7, wt = threadIdx.x & 127, warp = wt >> 5, lane = threadIdx.x & 31, t = lane & 3;
     PtsRow* pts = reinterpret_cast<PtsRow*>(sgen + SM::PTS) + wg * kTilePts;
+    TapTable* tab = reinterpret_cast<TapTable*>(sgen + SM::TAPS) + wg;
     const ViewXform* vxs = reinterpret_cast<const ViewXform*>(sgen + SM::VIEWS);
     const float* sb = reinterpret_cast<const float*>(sgen + SM::BIAS);
     const uint32_t sW = sbase, sH = sbase + SM::HEAD;
     const int nv = P.nv, N = P.N;
     const int r0 = warp * 16 + (lane >> 2);          // this thread's accumulator rows (points) r0, r0 + 8
+    FIELD_PHASE_INIT();
 
     for (int tile = blockIdx.x * kWarpgroups + wg; tile < P.n_tiles; tile += gridDim.x * kWarpgroups) {
         const int g = tile / P.sg, q = tile % P.sg;
@@ -424,19 +482,21 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
             pts[n] = pr;
         }
         asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+#ifdef NEO_FIELD_PHASES
+        if (wt == 0) ph_acc[wg][kPhases] += 1ull;
+#endif
+        FIELD_PHASE(0);
 
         float hacc[40];                                 // folded head: [q (64) | sigma | pad], summed over the views
 #pragma unroll
         for (int i = 0; i < 40; ++i) hacc[i] = 0.f;
 #pragma unroll 1
         for (int v = 0; v < nv; ++v) {
-            float ce[2][4], cl[2][3];
+            float ce[2][4];
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
                 const PtsRow& pr = pts[r0 + 8 * i];
                 to_camera(vxs[v], pr.xe, ce[i]);
-                if (IS_BG) to_camera(vxs[v], pr.xl, cl[i]);
-                else { cl[i][0] = ce[i][0]; cl[i][1] = ce[i][1]; cl[i][2] = ce[i][2]; }      // foreground: the lookup point IS the encoded point
                 ce[i][3] = pr.tv;
             }
             uint32_t enc[KS][4];
@@ -449,12 +509,25 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
                         const int c = 16 * ks + 8 * h + 2 * t;
                         enc[ks][2 * h + i] = pack_h2(enc_value<ICH>(ce[i], c), enc_value<ICH>(ce[i], c + 1));
                     }
+            FIELD_PHASE(1);
+            // tap table of this view, built once for both halves: thread wt does point wt % 64, maps 2 (wt / 64) and 2 (wt / 64) + 1
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // the previous view's table has been read
+            {
+                const int n = wt & (kTilePts - 1), m0 = 2 * (wt >> 6);
+                float cl[3];
+                to_camera(vxs[v], pts[n].xl, cl);               // foreground: xl == xe, the lookup point IS the encoded point
+                tap_entry(*tab, P.sc, cl, v, n, m0);
+                tap_entry(*tab, P.sc, cl, v, n, m0 + 1);
+            }
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+            FIELD_PHASE(2);
             float acc[64];
             uint32_t a[8][4];
             // layer 0: blend of P0 + W0enc . enc (b0 on the constant-one column)
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-            blend_maps<0>(acc, P, cl, v, t);
+            blend_maps<0>(acc, P, *tab, r0, t);
+            FIELD_PHASE(3);
             wgmma_fence();
 #pragma unroll
             for (int ks = 0; ks < KS; ++ks) wgmma_rs_n128(acc, enc[ks], wdesc(sW + trunk_off(KE, 0), ks, SLAB));
@@ -475,7 +548,9 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
             // layer 3: blend of P3 + W3h . h2 + W3enc . enc (b3 on the constant-one column)
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-            blend_maps<1>(acc, P, cl, v, t);
+            FIELD_PHASE(4);
+            blend_maps<1>(acc, P, *tab, r0, t);
+            FIELD_PHASE(5);
             wgmma_fence();
 #pragma unroll
             for (int ks = 0; ks < 8; ++ks) wgmma_rs_n128(acc, a[ks], wdesc(sW + trunk_off(KE, 3), ks, SLAB));
@@ -490,6 +565,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
             for (int ks = 0; ks < 8; ++ks) wgmma_rs_n80(hacc, a[ks], wdesc(sH + WH_H, ks, 80 * 128));
             wgmma_commit();
             wgmma_wait<0>();
+            FIELD_PHASE(6);
         }
         // direction term: hacc += mean_v(dir_enc_v) . Whead_dir^T   (K = 32: 27 columns + zero padding)
         {
@@ -578,7 +654,12 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
                 }
             }
         }
+        FIELD_PHASE(7);
     }
+#ifdef NEO_FIELD_PHASES
+    if (wt == 0)
+        for (int p = 0; p <= kPhases; ++p) atomicAdd(&g_phase_cycles[P.phase_slot][p], ph_acc[wg][p]);
+#endif
 }
 
 }  // namespace tc
@@ -628,6 +709,10 @@ int tc_scene_create(NeoScene* sc, const NeoMLPParams mlps[4], cudaStream_t s) {
         }
     } tmp;
     tmp.s = s;
+    if ((long long)d.nv * d.lat_h * d.lat_w > 0x7fffffffLL || (long long)d.nv * d.plane_h * d.plane_w > 0x7fffffffLL) {
+        set_error("feature maps too large: the tap table holds 32-bit texel indices");
+        return NEO_ERR_UNSUPPORTED;
+    }
     __half** feat16 = tmp.feat16;
     __half*& wsel = tmp.wsel;
     {
@@ -717,6 +802,9 @@ int launch_field_tc(const NeoScene* sc, const NeoRays* rays, const float* far, c
     P.rgb_out = rgb; P.sigma_out = sigma;
     { int rc0 = trap_buffer(); if (rc0) return rc0; }
     P.trap = g_trap_dev;
+#ifdef NEO_FIELD_PHASES
+    P.phase_slot = g_phase_launches++ % kPhaseSlots;
+#endif
     const long long ctas = (n_tiles + kWarpgroups - 1) / kWarpgroups;
     const int grid = (int)(ctas < n_sm ? ctas : n_sm);
     auto launch = [&](auto kern, size_t smem) -> int {
@@ -743,3 +831,21 @@ extern "C" int neo_tc_enc_column(int in_ch, int col) {
     return (in_ch == 3) ? enc_col_ref_index<3>(col) : enc_col_ref_index<4>(col);
 }
 extern "C" const char* neo_tc_trap_info(void) { return neo::tc_trap_info(); }
+
+#ifdef NEO_FIELD_PHASES
+// diagnostic build only (not part of include/neo360_b200.h): zero the phase clocks, and read them back after a synchronise as
+// [launch][kPhases + 1] (cycles per phase, then tiles), one row per field launch since the reset; returns the number of launches
+extern "C" int neo_field_phases_reset(void) {
+    neo::tc::g_phase_launches = 0;
+    void* p = nullptr;
+    if (cudaGetSymbolAddress(&p, neo::tc::g_phase_cycles) != cudaSuccess) return -1;
+    return cudaMemset(p, 0, sizeof(neo::tc::g_phase_cycles)) == cudaSuccess ? 0 : -1;
+}
+extern "C" int neo_field_phases_read(unsigned long long* out, int max_launches) {
+    using namespace neo::tc;
+    if (g_phase_launches > kPhaseSlots) return -1;          // rows have wrapped
+    const int n = g_phase_launches < max_launches ? g_phase_launches : max_launches;
+    if (n > 0 && cudaMemcpyFromSymbol(out, g_phase_cycles, sizeof(unsigned long long) * n * (kPhases + 1)) != cudaSuccess) return -1;
+    return n;
+}
+#endif

@@ -1,0 +1,88 @@
+"""Where the tensor-core field kernel spends its cycles: phase clocks of one bench.py frame.
+
+Builds a copy of the library with -DNEO_FIELD_PHASES (clock64() marks in field_tc_kernel, see csrc/field_tc.cu) into a temporary
+directory, loads it through NEO360_B200_LIB, renders the headline frame of bench.py (same scene, rays, img_wh block order and chunk)
+once to warm up and once measured, and prints for each field launch the cycles per tile (64 points, all views) of every phase,
+summed over the warpgroups.  Usage on a GPU box:
+
+  python tools/field_phases.py [--lib PATH]      (--lib: an instrumented library built beforehand, e.g. from another source tree)
+"""
+import argparse
+import ctypes as C
+import os
+import shutil
+import subprocess
+import sys
+import tempfile
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+PHASES = ("tile setup", "camera + encodings", "tap table", "blend P0", "layers 0-2", "blend P3", "layer 3 + head", "colour head + stores")
+LAUNCHES = ("fg coarse", "bg coarse", "fg fine", "bg fine")      # order of the field launches of one frame (render.cu)
+MAX_LAUNCHES = 64
+
+
+def build_instrumented(out_dir):
+    from neo360_b200 import build as b
+    path = os.path.join(out_dir, "libneo360_b200_phases.so")
+    nvcc = shutil.which("nvcc") or "/usr/local/cuda/bin/nvcc"
+    cmd = [nvcc] + b.FLAGS + ["-DNEO_FIELD_PHASES", "-o", path] + [os.path.join(b.CSRC, s) for s in b.SOURCES]
+    res = subprocess.run(cmd, capture_output=True, text=True)
+    if res.returncode != 0:
+        raise RuntimeError("nvcc failed:\n" + res.stdout + res.stderr)
+    return path
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--lib", default=None, help="instrumented library to load instead of building one")
+    args = ap.parse_args()
+    tmp = tempfile.TemporaryDirectory(prefix="neo360_phases_")
+    os.environ["NEO360_B200_LIB"] = os.path.abspath(args.lib) if args.lib else build_instrumented(tmp.name)
+
+    import torch
+    import bench as Bm
+    from neo360_b200 import NeRF_TP, _lib
+    lib = _lib.load()
+    if not hasattr(lib, "neo_field_phases_read"):
+        raise RuntimeError(f"{os.environ['NEO360_B200_LIB']} was not built with -DNEO_FIELD_PHASES")
+    lib.neo_field_phases_reset.restype = C.c_int
+    lib.neo_field_phases_read.restype = C.c_int
+    lib.neo_field_phases_read.argtypes = [C.POINTER(C.c_ulonglong), C.c_int]
+
+    dev = torch.device("cuda:0")
+    sc, P = Bm.build_scene_cpu()
+    net = NeRF_TP(num_coarse_samples=Bm.N_COARSE, num_fine_samples=Bm.N_FINE, num_src_views=Bm.NV, precision="tc").eval()
+    net.load_state_dict(P)
+    net = net.to(dev)
+    net.set_scene(*[sc[k].to(dev) for k in ("planes_xz", "planes_xy", "planes_yz", "latent", "src_poses", "src_focal", "src_c")],
+                  sc["img_wh"])
+    o, d = Bm.frame_rays_cpu(0)
+    rays = {"rays_o": o.to(dev), "rays_d": d.to(dev), "viewdirs": d.to(dev)}
+    wh = (Bm.IMG_W, Bm.IMG_H)
+    with torch.no_grad():
+        net.render_rays_test(rays, chunk=Bm.CHUNK, img_wh=wh)            # warm-up: module load, first-launch set-up
+        torch.cuda.synchronize()
+        if lib.neo_field_phases_reset() != 0:
+            raise RuntimeError("neo_field_phases_reset failed")
+        net.render_rays_test(rays, chunk=Bm.CHUNK, img_wh=wh)
+        torch.cuda.synchronize()
+    net.check()
+    cols = len(PHASES) + 1
+    buf = (C.c_ulonglong * (MAX_LAUNCHES * cols))()
+    n = lib.neo_field_phases_read(buf, MAX_LAUNCHES)
+    if n < 0:
+        raise RuntimeError("neo_field_phases_read failed")
+    name = torch.cuda.get_device_name(0)
+    print(f"{name}; library {os.environ['NEO360_B200_LIB']}; {n} field launches; cycles per tile (64 points x {Bm.NV} views) per phase")
+    print(f"{'launch':<12}{'tiles':>9}" + "".join(f"{p:>22}" for p in PHASES) + f"{'total':>12}")
+    for li in range(n):
+        row = buf[li * cols:(li + 1) * cols]
+        tiles = max(row[-1], 1)
+        per = [c / tiles for c in row[:-1]]
+        print(f"{LAUNCHES[li % 4]:<12}{row[-1]:>9}" + "".join(f"{x:>14.0f} ({x / sum(per):4.0%})" for x in per) + f"{sum(per):>12.0f}")
+
+
+if __name__ == "__main__":
+    main()
