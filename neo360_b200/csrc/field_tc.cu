@@ -293,17 +293,59 @@ __device__ __noinline__ void load_timeout(int* trapinfo, uint32_t bar) {
 
 __device__ __forceinline__ float sel4(const float* x, int i) { return i == 0 ? x[0] : i == 1 ? x[1] : i == 2 ? x[2] : x[3]; }
 
-// encoding column `col` (enc_col<> order) of the point x (3 coordinates, + t for the background MLP)
-template <int ICH>
-__device__ __forceinline__ float enc_value(const float* x, int col) {
-    const EncCol e = enc_col<ICH>(col);
-    if (e.kind == 0) return 0.f;
-    if (e.kind == 1) return 1.f;
-    const float xc = sel4(x, e.cc);
-    if (e.kind == 2) return xc;
-    const float a = xc * (float)(1 << e.lvl);            // exact: power-of-two scaling
-    return e.kind == 3 ? sinf(a) : cosf(a);
+// Encoding staging: per (tile, view) a warpgroup computes its 64 points' encodings once, as a flat set of items, into one row of 64
+// fp16 per point (in the bytes of its tap table, before the table is built); then every thread loads its A-fragment columns from
+// the rows.  Row slot 21 j + k holds column k of staged coordinate j: k = 0 the coordinate, 1 + l sin(2^l x), 11 + l cos(2^l x), the
+// order of enc_col<3> (slot == column for the foreground).  The 32-bit words of a row are XOR-swizzled by the point (bits 2-4), so
+// that the 8 points x 4 words a warp loads per fragment register fall on 32 distinct banks.
+constexpr int kStageRow = 64;
+__device__ __forceinline__ int stage_slot(int n, int k) { return n * kStageRow + ((((k >> 1) ^ ((n & 7) << 2))) << 1 | (k & 1)); }
+
+// items first .. first + count - 1 of one point (item i: staged coordinate i / 10, level i % 10): sin and cos of 2^l x, rounded to
+// fp16 as pack_h2 does.  Rolled, so the kernel has one sincosf call site per use instead of one sinf / cosf per fragment column.
+__device__ __forceinline__ void stage_items(__half* stage, int n, const float (&x)[3], int first, int count) {
+#pragma unroll 1
+    for (int i = first; i < first + count; ++i) {
+        const int j = i / 10, l = i - 10 * j;
+        const float xc = j == 0 ? x[0] : j == 1 ? x[1] : x[2];
+        float s, c;
+        sincosf(xc * (float)(1 << l), &s, &c);           // exact: power-of-two scaling
+        stage[stage_slot(n, 21 * j + 1 + l)] = __float2half_rn(s);
+        stage[stage_slot(n, 21 * j + 11 + l)] = __float2half_rn(c);
+    }
 }
+
+// fp16 bits of encoding column c = c0 + u (enc_col<ICH> order; c0 a multiple of 8, u < 8) of point n, from rows that stage
+// coordinates j0, j0 + 1, ...  Beyond a coordinate's 21 columns: the constant one (column 21 of the background) or zero.
+template <int ICH>
+__device__ __forceinline__ uint32_t enc_staged(const __half* stage, int n, int c0, int u, int j0) {
+    if (ICH == 3) {                                      // stride 21: the slot is the column
+        const int c = c0 + u;
+        return c == 63 ? 0x3c00u : __half_as_ushort(stage[stage_slot(n, c)]);
+    }
+    const int j = c0 / 24, k = c0 % 24 + u;              // c0 % 24 <= 16: the 8 columns from c0 share one coordinate block
+    if (k >= 21) return (j == 0 && k == 21) ? 0x3c00u : 0u;
+    return __half_as_ushort(stage[stage_slot(n, 21 * (j - j0) + k)]);
+}
+// the slot arithmetic above, checked against enc_col<> for every column
+template <int ICH>
+constexpr bool stage_layout_ok() {
+    for (int c = 0; c < (ICH == 3 ? 64 : 96); ++c) {
+        const EncCol e = enc_col<ICH>(c);
+        const int k = e.kind == 2 ? 0 : e.kind == 3 ? 1 + e.lvl : 11 + e.lvl;
+        if (ICH == 3 && e.kind >= 2 && c != 21 * e.cc + k) return false;
+        if (ICH == 4) {
+            const int j = c / 24, kk = c % 24;
+            if (e.kind >= 2 && (kk >= 21 || j != e.cc || kk != k)) return false;
+            if (e.kind < 2 && kk < 21) return false;
+            if ((e.kind == 1) != (j == 0 && kk == 21)) return false;
+        }
+        if (ICH == 3 && (e.kind == 1) != (c == 63)) return false;
+        if (ICH == 3 && e.kind == 0) return false;
+    }
+    return true;
+}
+static_assert(stage_layout_ok<3>() && stage_layout_ok<4>(), "enc_staged does not match enc_col");
 
 // column e of the direction encoding of the conditioning ray in one source camera's frame (model.py:357-360): [d, sin(2^k d),
 // sin(2^k d + pi/2)], 27 columns, zero beyond
@@ -343,6 +385,7 @@ struct TapTable {
     int4 tex[4][kTilePts];
     float4 w[4][kTilePts];
 };
+static_assert(kTilePts * kStageRow * sizeof(__half) <= sizeof(TapTable), "the encoding staging rows live in the tap table's bytes");
 __device__ __forceinline__ int comp4(const int4& x, int k) { return k == 0 ? x.x : k == 1 ? x.y : k == 2 ? x.z : x.w; }
 __device__ __forceinline__ float comp4(const float4& x, int k) { return k == 0 ? x.x : k == 1 ? x.y : k == 2 ? x.z : x.w; }
 
@@ -487,37 +530,55 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
 #endif
         FIELD_PHASE(0);
 
+        // Encodings: thread wt stages point n = wt % 64, items 15 (wt / 64) .. + 14 of its 30 (3 coordinates x 10 levels) per view.
+        // A-fragment columns 16 ks + 8 h + 2 t + e of rows r0, r0 + 8, as enc_staged reads them (c0 = 16 ks + 8 h, u = 2 t + e).
+        __half* stage = reinterpret_cast<__half*>(tab);
+        const int sn = wt & (kTilePts - 1), shf = wt >> 6;
+        uint32_t enc[KS][4];
+        auto load_enc = [&](int ks, int h, int j0) {
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+                enc[ks][2 * h + i] = enc_staged<ICH>(stage, r0 + 8 * i, 16 * ks + 8 * h, 2 * t, j0) |
+                                     enc_staged<ICH>(stage, r0 + 8 * i, 16 * ks + 8 * h, 2 * t + 1, j0) << 16;
+        };
+        if constexpr (IS_BG) {
+            // the s columns 72-92 (enc[4][2..3], enc[5][*]) do not depend on the view: staged as coordinate 0 once per tile
+            const float sx[3] = {pts[sn].tv, 0.f, 0.f};
+            if (shf == 0) stage[stage_slot(sn, 0)] = __float2half_rn(sx[0]);
+            stage_items(stage, sn, sx, 5 * shf, 5);
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+            load_enc(KS - 2, 1, 3);
+            load_enc(KS - 1, 0, 3);
+            load_enc(KS - 1, 1, 3);
+        }
+
         float hacc[40];                                 // folded head: [q (64) | sigma | pad], summed over the views
 #pragma unroll
         for (int i = 0; i < 40; ++i) hacc[i] = 0.f;
 #pragma unroll 1
         for (int v = 0; v < nv; ++v) {
-            float ce[2][4];
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // the previous view's table (or the s columns) has been read
+            float ce[3];
+            to_camera(vxs[v], pts[sn].xe, ce);
+            if (shf == 0)
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                const PtsRow& pr = pts[r0 + 8 * i];
-                to_camera(vxs[v], pr.xe, ce[i]);
-                ce[i][3] = pr.tv;
-            }
-            uint32_t enc[KS][4];
+                for (int j = 0; j < 3; ++j) stage[stage_slot(sn, 21 * j)] = __float2half_rn(ce[j]);
+            stage_items(stage, sn, ce, 15 * shf, 15);
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
 #pragma unroll
-            for (int ks = 0; ks < KS; ++ks)
+            for (int ks = 0; ks < 4; ++ks)
 #pragma unroll
-                for (int h = 0; h < 2; ++h)
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        const int c = 16 * ks + 8 * h + 2 * t;
-                        enc[ks][2 * h + i] = pack_h2(enc_value<ICH>(ce[i], c), enc_value<ICH>(ce[i], c + 1));
-                    }
+                for (int h = 0; h < 2; ++h) load_enc(ks, h, 0);
+            if constexpr (IS_BG) load_enc(4, 0, 0);                                  // columns 64-71: the last levels of coordinate 2
             FIELD_PHASE(1);
             // tap table of this view, built once for both halves: thread wt does point wt % 64, maps 2 (wt / 64) and 2 (wt / 64) + 1
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // the previous view's table has been read
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // the staged encodings have been read
             {
-                const int n = wt & (kTilePts - 1), m0 = 2 * (wt >> 6);
-                float cl[3];
-                to_camera(vxs[v], pts[n].xl, cl);               // foreground: xl == xe, the lookup point IS the encoded point
-                tap_entry(*tab, P.sc, cl, v, n, m0);
-                tap_entry(*tab, P.sc, cl, v, n, m0 + 1);
+                const int m0 = 2 * shf;
+                float cl[3] = {ce[0], ce[1], ce[2]};            // foreground: xl == xe, the lookup point IS the encoded point
+                if constexpr (IS_BG) to_camera(vxs[v], pts[sn].xl, cl);
+                tap_entry(*tab, P.sc, cl, v, sn, m0);
+                tap_entry(*tab, P.sc, cl, v, sn, m0 + 1);
             }
             asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
             FIELD_PHASE(2);
