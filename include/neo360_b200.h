@@ -233,6 +233,25 @@ int neo_clipped_sq_err_masked(const float* pred, const float* gt, const uint8_t*
 size_t neo_ssim_workspace_bytes(int n, int H, int W);
 int neo_ssim(const float* pred, const float* gt, int n, int H, int W, double* ssim, float* ss_map, void* workspace, size_t workspace_bytes,
              void* stream);
+/* LPIPS (VGG) around a trunk the caller runs (definition in csrc/lpips.cu): LitModel.lpips_each with piqa's LPIPS (models/interface.py:
+ * 113-122) and the fine-tuning loss with lpips.LPIPS (models/neo360/model.py:1283-1309).  Asynchronous on `stream`, nothing allocated,
+ * NEO_ERR_INVALID before any launch on a NULL buffer or sizes out of range.
+ * neo_lpips_prepare: img (n, H, W, 3) fp32 channel-last, clipped to [0, 1] -> out (n, 3, H, W), scaled by form 0 (piqa: (x - mean) / std)
+ * or form 1 (lpips: ((2x - 1) - shift) / scale).  neo_lpips_prepare_bwd: g_out (n, 3, H, W) -> g_img (n, H, W, 3), zero where img is
+ * outside [0, 1] (inclusive bounds pass, as torch.clamp's backward). */
+int neo_lpips_prepare(const float* img, int n, int H, int W, int form, float* out, void* stream);
+int neo_lpips_prepare_bwd(const float* img, const float* g_out, int n, int H, int W, int form, float* g_img, void* stream);
+/* neo_lpips_head: fx, fy, w are host arrays of 5 device pointers: the features of relu1_2 .. relu5_3 of the frames (n, C_k, H >> k, W >> k)
+ * fp32 NCHW with C = 64, 128, 256, 512, 512, and the layers' 1x1 weights (C_k).  lpips (n) device doubles; per_layer (n, 5) device doubles
+ * or NULL.  Workspace: neo_lpips_workspace_bytes(n, H, W) bytes, 8-byte aligned, caller-owned (0 = invalid sizes: n >= 1, H, W >= 16).
+ * No floating-point atomics: two calls are bit-identical and a frame gives the same bits alone or in any batch.
+ * neo_lpips_head_bwd: g (n) fp32 device, the upstream gradient of each frame's value; writes every element of g_fx[k] (shaped as fx[k]) and,
+ * when g_fy is not NULL, of g_fy[k].  A pixel whose features are all zero gets a zero gradient. */
+size_t neo_lpips_workspace_bytes(int n, int H, int W);
+int neo_lpips_head(const float* const* fx, const float* const* fy, const float* const* w, int n, int H, int W, double* lpips, double* per_layer,
+                   void* workspace, size_t workspace_bytes, void* stream);
+int neo_lpips_head_bwd(const float* const* fx, const float* const* fy, const float* const* w, int n, int H, int W, const float* g,
+                       float* const* g_fx, float* const* g_fy, void* stream);
 
 /* ---- backward of the hand-written stages (training: models/neo360/model.py:697-820 differentiates through this path) ----
  * The field's backward is split: the lookups' scatter and the compositing backward are the entry points below; the dense layers of

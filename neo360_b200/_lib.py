@@ -111,6 +111,11 @@ SYMBOLS = {
     "neo_clipped_sq_err_masked": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_ssim_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "neo_ssim": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "neo_lpips_prepare": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "neo_lpips_prepare_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "neo_lpips_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "neo_lpips_head": (C.c_int, [C.POINTER(C.c_void_p)] * 3 + [C.c_int] * 3 + [C.c_void_p] * 3 + [C.c_size_t, C.c_void_p]),
+    "neo_lpips_head_bwd": (C.c_int, [C.POINTER(C.c_void_p)] * 3 + [C.c_int] * 3 + [C.c_void_p] + [C.POINTER(C.c_void_p)] * 2 + [C.c_void_p]),
     "neo_volumetric_rendering_bwd": (C.c_int, [C.c_void_p] * 5 + [C.c_int] * 4 + [C.c_void_p] * 8),
     "neo_index_grid_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_index_local_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),

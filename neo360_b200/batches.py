@@ -12,12 +12,14 @@ from __future__ import annotations
 
 from typing import Dict, Optional
 
+import numpy as np
 import torch
 
 from . import ops
 
 RAY_BATCH_SIZE = 500      # nerds360_ae.py:535-538
 NUM_TARGET_VIEWS = 20     # nerds360_ae.py dest views per item (SURVEY.md section 8 f3)
+PATCH = 30                # LPIPS fine-tuning patch side (nerds360_ae.py:638-664)
 
 
 class TargetViews:
@@ -61,3 +63,25 @@ def train_batch(views: TargetViews, src: Dict[str, torch.Tensor], pix_inds: Opti
     sample["multloss"] = torch.zeros(n, 1, device=dev)
     sample["normals"] = torch.zeros_like(o)
     return sample
+
+
+def patch_pix_inds(view: int, x: int, y: int, H: int, W: int) -> torch.Tensor:
+    """The flat indices into the (T,H,W) stack of the 30x30 patch at row x, column y of target view `view`, in the reference's order
+    (`view(H, W)[x:x+30, y:y+30].reshape(-1)`, nerds360_ae.py:638-664): row-major over the patch."""
+    if not (0 <= x <= H - PATCH and 0 <= y <= W - PATCH):
+        raise ValueError(f"patch at ({x}, {y}) does not fit a {H}x{W} view")
+    r = torch.arange(PATCH, dtype=torch.int64)
+    return (view * H * W + (x + r)[:, None] * W + (y + r)[None, :]).reshape(-1)
+
+
+def patch_batch(views: TargetViews, src: Dict[str, torch.Tensor], view: int, x: Optional[int] = None, y: Optional[int] = None) -> Dict[str, torch.Tensor]:
+    """The LPIPS fine-tuning sample (nerds360_ae.py:598-664): the 900 rays of one 30x30 patch of target view `view`, with the keys of
+    train_batch.  x (row) and y (column) not given are drawn as the reference draws them: np.random.randint(0, H - 30 + 1), then
+    np.random.randint(0, W - 30 + 1), from numpy's global generator."""
+    if not 0 <= view < views.T:
+        raise ValueError(f"view {view} of {views.T}")
+    if x is None:
+        x = np.random.randint(0, views.H - PATCH + 1)
+    if y is None:
+        y = np.random.randint(0, views.W - PATCH + 1)
+    return train_batch(views, src, pix_inds=patch_pix_inds(view, int(x), int(y), views.H, views.W))

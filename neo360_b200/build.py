@@ -7,7 +7,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libneo360_b200.so")
-SOURCES = ["scene.cu", "sampling.cu", "field_fp32.cu", "field_tc.cu", "render.cu", "vanilla.cu", "mip.cu", "gemm_tc.cu", "encoder.cu", "metrics.cu", "det.cu"]
+SOURCES = ["scene.cu", "sampling.cu", "field_fp32.cu", "field_tc.cu", "render.cu", "vanilla.cu", "mip.cu", "gemm_tc.cu", "encoder.cu", "metrics.cu", "det.cu", "lpips.cu"]
 FLAGS = ["-shared", "-Xcompiler", "-fPIC", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
          "-std=c++17", "--threads", "4"]
 

@@ -7,11 +7,16 @@
     LitModel.ssim_each         models/interface.py:101-111  ssim_each() / ssim(): piqa's SSIM() in CUDA (neo_ssim, csrc/metrics.cu)
     get_obj_rgbs_from_segmap + psnr_each  models/utils.py:102-109
                                                            psnr_obj_each(): the same reduction over the masked pixels (neo_clipped_sq_err_masked)
-    LitModel.psnr / .ssim      models/interface.py:124-155  stat(): the {"name", "mean", "test"} dicts write_stats takes
+    LitModel.lpips_each        models/interface.py:113-122  lpips_each() / lpips(): piqa's LPIPS(network="vgg") with the user's weight files
+                                                           (lpips.LPIPS.from_files): VGG-16 trunk as framework convolutions, scaling and
+                                                           the distance head in CUDA (neo_lpips_prepare, neo_lpips_head, csrc/lpips.cu)
+    LitModel.psnr / .ssim / .lpips  models/interface.py:124-172
+                                                           stat(): the {"name", "mean", "test"} dicts write_stats takes
     store_image / store_depth_img / store_depth_raw  models/utils.py:21-53
                                                            store_image() / store_depth_img() / store_depth_raw() (same file naming)
     write_stats                models/utils.py:62-73        write_stats(): results.json, byte for byte
-LPIPS is not provided: it needs pretrained VGG / AlexNet weights (DESIGN.md section 8), so results.json has no LPIPS entry.
+results.json has an LPIPS entry when the caller passes stat("LPIPS", lpips_each(...)) to write_stats; without an LPIPS model nothing
+changes.
 """
 from __future__ import annotations
 
@@ -120,6 +125,22 @@ def ssim_each(preds: Sequence[torch.Tensor], gts: Sequence[torch.Tensor]) -> tor
     for idx in groups.values():
         vals[idx] = ssim_batch(torch.stack([preds[i] for i in idx]), torch.stack([gts[i] for i in idx])).cpu()
     return vals.float()
+
+
+def lpips(pred: torch.Tensor, gt: torch.Tensor, model) -> float:
+    """LPIPS of one (h,w,3) frame with an `neo360_b200.lpips.LPIPS` model on the frame's device: inputs clipped to [0, 1] and scaled as
+    piqa scales them (csrc/lpips.cu)."""
+    with torch.no_grad():
+        return float(model(pred.unsqueeze(0), gt.unsqueeze(0))[0])
+
+
+def lpips_each(preds: Sequence[torch.Tensor], gts: Sequence[torch.Tensor], model) -> torch.Tensor:
+    """models/interface.py:113-122: one LPIPS per frame, one frame at a time as the reference runs them, a float32 tensor like
+    ssim_each's."""
+    preds, gts = list(preds), list(gts)
+    if len(preds) != len(gts):
+        raise ValueError(f"{len(preds)} preds and {len(gts)} gts")
+    return torch.tensor([lpips(p, g, model) for p, g in zip(preds, gts)], dtype=torch.float64).float()
 
 
 def stat(name: str, values: torch.Tensor) -> dict:

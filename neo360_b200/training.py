@@ -342,9 +342,39 @@ def distortion_loss(w: Tensor, m: Tensor, interval: Tensor) -> Tensor:
     return loss_uni + loss_bi
 
 
-def training_loss(ret, target: Tensor, dist_weight: float = 0.01) -> Tensor:
-    """MSE of both levels + distortion regulariser on the fine level (model.py:740-748, 1246-1260)."""
+LPIPS_LAMBDA = 0.3      # model.py:1308
+
+
+def lpips_loss(rgb: Tensor, target: Tensor, model) -> Tensor:
+    """NeRF_TP.lpips_loss (model.py:1283-1309): 0.3 LPIPS of the 30x30 patch whose (900, 3) colours are `rgb` (patch order of
+    batches.patch_batch) against `target`, with lpips' scaling (csrc/lpips.cu form 1) and an `neo360_b200.lpips.LPIPS` model.  The
+    gradient flows to `rgb`.  The 1x1 layers have no dropout: the term is the reference's in eval mode (DESIGN.md section 8)."""
+    from .lpips import FORM_LPIPS
+    from .batches import PATCH
+    d = model(rgb.reshape(1, PATCH, PATCH, 3), target.reshape(1, PATCH, PATCH, 3), FORM_LPIPS)
+    return d.float()[0] * LPIPS_LAMBDA
+
+
+def setup_finetune_lpips(net) -> List[torch.nn.Parameter]:
+    """What configure_optimizers does for --finetune_lpips (model.py:957-981): freeze the encoder's spatial_encoder and put it in eval
+    mode, put every BatchNorm2d of `net` in eval mode.  Returns the parameters that still train, for the optimiser and the gradient clip;
+    the LPIPS model is not part of `net`, so its parameters stay out of both.  Call it after `net.train()`, which would undo the eval
+    modes."""
+    if getattr(net, "encoder", None) is not None:
+        net.encoder.spatial_encoder.requires_grad_(False)
+        net.encoder.spatial_encoder.eval()
+    for m in net.modules():
+        if isinstance(m, torch.nn.BatchNorm2d):
+            m.eval()
+    return [p for p in net.parameters() if p.requires_grad]
+
+
+def training_loss(ret, target: Tensor, dist_weight: float = 0.01, lpips_model=None) -> Tensor:
+    """MSE of both levels + distortion regulariser on the fine level (model.py:740-748, 1246-1260).  With `lpips_model` (the
+    --finetune_lpips variant, model.py:750-755) the LPIPS loss of both levels' patch colours is added before the regulariser."""
     loss = ((ret[0][0] - target) ** 2).mean() + ((ret[1][0] - target) ** 2).mean()
+    if lpips_model is not None:
+        loss = loss + (lpips_loss(ret[0][0], target, lpips_model) + lpips_loss(ret[1][0], target, lpips_model))
     _, fg_w, bg_w, fg_m, bg_m, _ = ret[1]
     n = fg_w.shape[-1]
     loss = loss + dist_weight * (distortion_loss(fg_w, fg_m, torch.full_like(fg_w, 1.0 / n)) + distortion_loss(bg_w, bg_m, torch.full_like(bg_w, 1.0 / n)))
