@@ -16,7 +16,8 @@
 // m64nNk16 with the activations as REGISTER A fragments: the fp32 accumulator of one layer is rectified, packed to fp16 and fed to
 // the next layer without touching shared memory.  The projected-map blends are added straight into the accumulators of layers 0 and
 // 3: the projected maps are stored with their channels in the accumulator-fragment order (pmap_logical), so the 32 channels a thread
-// owns for a point are 64 contiguous bytes of each texel (four 16-byte loads per tap, a quad of lanes reads whole 256-byte rows).
+// owns for a point are four 16-byte chunks of each texel, one per 64-byte block (four 16-byte loads per tap; each load of a quad
+// of lanes is one contiguous 64-byte block, the four together a whole 256-byte half row).
 #include "common.cuh"
 #include "hopper.cuh"
 #include <cuda.h>
@@ -46,10 +47,13 @@ __host__ __device__ constexpr uint32_t trunk_off(int KE, int seg) { return seg =
 __host__ __device__ constexpr uint32_t trunk_bytes(int KE) { return trunk_off(KE, 4) + (uint32_t)enc_slabs(KE) * SLAB; }
 
 // channel order of the projected maps: physical channel p of a texel holds logical channel pmap_logical(p) of [P0 | P3], so that
-// thread t (lane % 4) of an accumulator fragment finds its channels 8 j + 2 t + e (j < 16, e < 2) at p = 32 t + 2 j + e
+// thread t (lane % 4) of an accumulator fragment finds its channels 8 j + 2 t + e (j < 16, e < 2) of a half at
+// p = 32 (j / 4) + 8 t + 2 (j % 4) + e: in 16-byte chunk u = j / 4 of a 64-byte block per t, the four lanes of a quad reading one
+// contiguous 64-byte block per load.  (With each thread's 64 bytes contiguous instead, one warp load of 8 points touches two
+// 128-byte lines per point rather than one, and the blends' L1 wavefronts double.)
 __host__ __device__ inline int pmap_logical(int p) {
-    const int q = p & 127, t = q >> 5, j = (q & 31) >> 1, e = q & 1;
-    return (p & 128) + 8 * j + 2 * t + e;
+    const int q = p & 127, u = q >> 5, t = (q >> 3) & 3, jj = (q >> 1) & 3, e = q & 1;
+    return (p & 128) + 8 * (4 * u + jj) + 2 * t + e;
 }
 
 struct PtsRow {        // 48 bytes: view-independent data of one point of a tile
@@ -95,11 +99,12 @@ struct Params {
 // exactly, the source order.  Without the macro the kernel has no marks at all.
 #ifdef NEO_FIELD_PHASES
 constexpr int kPhases = 8;          // tile setup | camera + encodings | tap table | blend P0 | layers 0-2 | blend P3 | layer 3 + head | colour head + stores
-constexpr uint32_t kPhaseBytes = kWarpgroups * (kPhases + 1) * 8;        // per-warpgroup sums in shared memory
+constexpr int kPhaseCols = kPhases + 2;                                  // the phases, then tiles, then taps of non-zero weight
+constexpr uint32_t kPhaseBytes = kWarpgroups * (kPhases + 1) * 8;        // per-warpgroup sums (phases, tiles) in shared memory
 constexpr int kPhaseSlots = 64;
-__device__ unsigned long long g_phase_cycles[kPhaseSlots][kPhases + 1];    // [launch][phase], column kPhases: tiles
+__device__ unsigned long long g_phase_cycles[kPhaseSlots][kPhaseCols];    // [launch][column]
 static int g_phase_launches = 0;
-#define FIELD_PHASE_INIT() long long ph_t = clock64()
+#define FIELD_PHASE_INIT() long long ph_t = clock64(); unsigned long long ph_taps = 0
 #define FIELD_PHASE(p)                                   \
     do {                                                 \
         const long long now_ = clock64();                \
@@ -426,14 +431,14 @@ __device__ __forceinline__ void blend_maps(float (&acc)[64], const Params& P, co
         for (int m = 0; m < 4; ++m) {
             const int4 tx = tab.tex[m][r0 + 8 * i];
             const float4 wv = tab.w[m][r0 + 8 * i];
-            const uint4* base = reinterpret_cast<const uint4*>(P.mlp.pmap[m] + HALF * 128 + t * 32);
+            const uint4* base = reinterpret_cast<const uint4*>(P.mlp.pmap[m] + HALF * 128 + t * 8);
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 const float w = comp4(wv, k);
                 if (w == 0.f) continue;                                // out-of-range tap (zeros padding): no contribution
                 uint4 q[4];
 #pragma unroll
-                for (int u = 0; u < 4; ++u) q[u] = __ldg(base + (size_t)comp4(tx, k) * 32 + u);   // 32 uint4 per texel
+                for (int u = 0; u < 4; ++u) q[u] = __ldg(base + (size_t)comp4(tx, k) * 32 + 4 * u);   // 32 uint4 per texel
 #pragma unroll
                 for (int u = 0; u < 4; ++u) {
                     const uint32_t wd[4] = {q[u].x, q[u].y, q[u].z, q[u].w};
@@ -579,6 +584,10 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
                 if constexpr (IS_BG) to_camera(vxs[v], pts[sn].xl, cl);
                 tap_entry(*tab, P.sc, cl, v, sn, m0);
                 tap_entry(*tab, P.sc, cl, v, sn, m0 + 1);
+#ifdef NEO_FIELD_PHASES
+                for (int m = m0; m < m0 + 2; ++m)
+                    for (int k = 0; k < 4; ++k) ph_taps += comp4(tab->w[m][sn], k) != 0.f;
+#endif
             }
             asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
             FIELD_PHASE(2);
@@ -720,6 +729,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
 #ifdef NEO_FIELD_PHASES
     if (wt == 0)
         for (int p = 0; p <= kPhases; ++p) atomicAdd(&g_phase_cycles[P.phase_slot][p], ph_acc[wg][p]);
+    atomicAdd(&g_phase_cycles[P.phase_slot][kPhases + 1], ph_taps);
 #endif
 }
 
@@ -895,7 +905,8 @@ extern "C" const char* neo_tc_trap_info(void) { return neo::tc_trap_info(); }
 
 #ifdef NEO_FIELD_PHASES
 // diagnostic build only (not part of include/neo360_b200.h): zero the phase clocks, and read them back after a synchronise as
-// [launch][kPhases + 1] (cycles per phase, then tiles), one row per field launch since the reset; returns the number of launches
+// [launch][kPhases + 2] (cycles per phase, then tiles, then taps of non-zero weight), one row per field launch since the reset;
+// returns the number of launches
 extern "C" int neo_field_phases_reset(void) {
     neo::tc::g_phase_launches = 0;
     void* p = nullptr;
@@ -906,7 +917,7 @@ extern "C" int neo_field_phases_read(unsigned long long* out, int max_launches) 
     using namespace neo::tc;
     if (g_phase_launches > kPhaseSlots) return -1;          // rows have wrapped
     const int n = g_phase_launches < max_launches ? g_phase_launches : max_launches;
-    if (n > 0 && cudaMemcpyFromSymbol(out, g_phase_cycles, sizeof(unsigned long long) * n * (kPhases + 1)) != cudaSuccess) return -1;
+    if (n > 0 && cudaMemcpyFromSymbol(out, g_phase_cycles, sizeof(unsigned long long) * n * kPhaseCols) != cudaSuccess) return -1;
     return n;
 }
 #endif

@@ -3,9 +3,12 @@
 Builds a copy of the library with -DNEO_FIELD_PHASES (clock64() marks in field_tc_kernel, see csrc/field_tc.cu) into a temporary
 directory, loads it through NEO360_B200_LIB, renders the headline frame of bench.py (same scene, rays, img_wh block order and chunk)
 once to warm up and once measured, and prints for each field launch the cycles per tile (64 points, all views) of every phase,
-summed over the warpgroups.  Usage on a GPU box:
+summed over the warpgroups, and the texel traffic the blends request: taps of non-zero weight per tile (each one 2 x 256 bytes,
+the P0 and P3 halves of a texel) over the cycles of the two blend phases.  Usage on a GPU box:
 
-  python tools/field_phases.py [--lib PATH]      (--lib: an instrumented library built beforehand, e.g. from another source tree)
+  python tools/field_phases.py [--lib PATH] [--clock-mhz F]
+      --lib: an instrumented library built beforehand, e.g. from another source tree
+      --clock-mhz: SM clock the request rate is converted at (read it with nvidia-smi in the same run)
 """
 import argparse
 import ctypes as C
@@ -37,6 +40,7 @@ def build_instrumented(out_dir):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--lib", default=None, help="instrumented library to load instead of building one")
+    ap.add_argument("--clock-mhz", type=float, default=1980.0, help="SM clock for the bytes/s figures")
     args = ap.parse_args()
     tmp = tempfile.TemporaryDirectory(prefix="neo360_phases_")
     os.environ["NEO360_B200_LIB"] = os.path.abspath(args.lib) if args.lib else build_instrumented(tmp.name)
@@ -69,19 +73,31 @@ def main():
         net.render_rays_test(rays, chunk=Bm.CHUNK, img_wh=wh)
         torch.cuda.synchronize()
     net.check()
-    cols = len(PHASES) + 1
+    cols = len(PHASES) + 2                                               # phases, tiles, non-zero-weight taps
     buf = (C.c_ulonglong * (MAX_LAUNCHES * cols))()
     n = lib.neo_field_phases_read(buf, MAX_LAUNCHES)
     if n < 0:
         raise RuntimeError("neo_field_phases_read failed")
     name = torch.cuda.get_device_name(0)
+    n_sm = torch.cuda.get_device_properties(0).multi_processor_count
     print(f"{name}; library {os.environ['NEO360_B200_LIB']}; {n} field launches; cycles per tile (64 points x {Bm.NV} views) per phase")
     print(f"{'launch':<12}{'tiles':>9}" + "".join(f"{p:>22}" for p in PHASES) + f"{'total':>12}")
+    rows = []
     for li in range(n):
         row = buf[li * cols:(li + 1) * cols]
-        tiles = max(row[-1], 1)
-        per = [c / tiles for c in row[:-1]]
-        print(f"{LAUNCHES[li % 4]:<12}{row[-1]:>9}" + "".join(f"{x:>14.0f} ({x / sum(per):4.0%})" for x in per) + f"{sum(per):>12.0f}")
+        tiles = max(row[-2], 1)
+        per = [c / tiles for c in row[:-2]]
+        rows.append((tiles, per, row[-1] / tiles))
+        print(f"{LAUNCHES[li % 4]:<12}{row[-2]:>9}" + "".join(f"{x:>14.0f} ({x / sum(per):4.0%})" for x in per) + f"{sum(per):>12.0f}")
+    # request rate of the blends: a warpgroup's texel bytes per tile over its blend cycles per tile; the GPU figure assumes both
+    # warpgroups of every SM blend at once (an upper bound), the launch figure spreads the bytes over the whole tile
+    print(f"texel requests ({n_sm} SMs, 2 warpgroups each, SM clock {args.clock_mhz:.0f} MHz):")
+    print(f"{'launch':<12}{'taps/tile':>10}{'KB/tile':>9}{'B/cycle in blends':>19}{'GPU TB/s in blends':>20}{'GPU TB/s over tile':>20}")
+    for li, (tiles, per, taps) in enumerate(rows):
+        by = taps * 512
+        blend = per[PHASES.index("blend P0")] + per[PHASES.index("blend P3")]
+        scale = 2 * n_sm * args.clock_mhz * 1e6 / 1e12
+        print(f"{LAUNCHES[li % 4]:<12}{taps:>10.0f}{by / 1024:>9.0f}{by / blend:>19.1f}{by / blend * scale:>20.2f}{by / sum(per) * scale:>20.2f}")
 
 
 if __name__ == "__main__":
