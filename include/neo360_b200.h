@@ -487,6 +487,23 @@ const char* neo_last_error(void);
 /* "neo360_b200 <version> sm_90a" */
 const char* neo_version(void);
 
+/* ---- NeO-360 training on the tensor cores (csrc/field_train.cu): layers 0-3 of one NeRFPPMLP in the projected formulation, bf16
+ * operands, fp32 accumulation.  cam (nv*M, in_ch) camera-frame encoding points (row v M + j: point j in source view v); local_p,
+ * world_p (nv*M, 256) looked-up projected rows [P0 | P3]; w0 (128, 21 in_ch) = pts_linears.0 encoding columns, w3 (128, 128 + 21 in_ch)
+ * = pts_linears.3 [h | encoding] columns, w1 / w2 (128,128), biases (128), all fp32 nn.Linear layout.  hbar (M, 128) = the view mean of
+ * h3.  Saved state: neo_field_train_workspace_bytes(..., 0) bytes written by the forward and read by the backward; the backward's
+ * scratch: (..., 1) bytes (0 = invalid sizes).  Backward: g_hbar (M,128) -> d_pm (nv*M, 256), the row gradient of both local_p and
+ * world_p, and every weight / bias gradient in the layout of the inputs (written, not accumulated).  NEO_ERR_INVALID before any launch
+ * on a NULL buffer, nv outside 1..8, in_ch not 3 or 4, M <= 0, or a buffer not 16-byte aligned; NEO_ERR_WORKSPACE on a short
+ * workspace.  No floating-point atomics: two calls are bit-identical. ---- */
+size_t neo_field_train_workspace_bytes(int nv, int M, int in_ch, int which);
+int neo_field_train_fwd(const float* cam, const float* local_p, const float* world_p, int nv, int M, int in_ch,
+                        const float* w0, const float* b0, const float* w1, const float* b1, const float* w2, const float* b2,
+                        const float* w3, const float* b3, float* hbar, void* saved, size_t saved_bytes, void* stream);
+int neo_field_train_bwd(const float* g_hbar, int nv, int M, int in_ch, const float* w1, const float* w2, const float* w3,
+                        const void* saved, size_t saved_bytes, float* d_pm, float* gw0, float* gb0, float* gw1, float* gb1,
+                        float* gw2, float* gb2, float* gw3, float* gb3, void* scratch, size_t scratch_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -96,12 +96,15 @@ class NeRF_TP(nn.Module):
     def __init__(self, num_levels: int = 2, min_deg_point: int = 0, max_deg_point: int = 10, deg_view: int = 4,
                  num_coarse_samples: int = 128, num_fine_samples: int = 256, use_viewdirs: bool = True,
                  num_src_views: int = 3, density_noise: float = 0.0, lindisp: bool = False, encoder: Optional[nn.Module] = None,
-                 precision: str = "tc", chunk: Optional[int] = None, **unused):
+                 precision: str = "tc", chunk: Optional[int] = None, train_precision: str = "fp32", **unused):
         super().__init__()
         if num_levels != 2 or lindisp or density_noise != 0.0 or not use_viewdirs:
             raise NotImplementedError("reference defaults only: 2 levels, lindisp=False, density_noise=0 (model.py:165-175)")
         self.num_coarse_samples, self.num_fine_samples, self.num_src_views = num_coarse_samples, num_fine_samples, num_src_views
         self.precision = precision
+        # arithmetic of the MLPs in a training step: "fp32" (framework layers under autograd) or "tc" (bf16 tensor-core trunk,
+        # projected formulation only; training._TrunkTC).  An attribute like train_projected.
+        self.train_precision = train_precision
         self.chunk = chunk
         self.encoder = encoder
         mk = lambda ch: NeRFPPMLP(min_deg_point, max_deg_point, deg_view, num_src_views=num_src_views, input_ch=ch)

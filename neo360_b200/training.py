@@ -15,6 +15,9 @@ What runs where
     layers shrink to K = 63|84 and the lookups fetch 2 x 256 projected channels (`neo_index_maps`, backward `neo_index_maps_bwd`).  Autograd
     differentiates through the projection, so the map-column weights and the encoder outputs get exactly the reference's gradients (to
     fp32 re-association).  `train_projected = False` keeps the reference formulation row by row.
+  * `net.train_precision = "tc"` (projected formulation only): layers 0-3 of the four MLPs and their view mean run forward and
+    backward on the tensor cores in bf16 with fp32 accumulation (`_TrunkTC`, csrc/field_train.cu); the head runs once per point on the
+    view mean (exact re-association).  The default "fp32" runs `_mlp_projected` under autograd.
   * NCCL: ONE all-reduce over the flat gradient slab of the four MLPs per step (`allreduce_flat`), as the reference's DDP does.
   * under torch.use_deterministic_algorithms(True) the lookups' backward is the order-fixed `neo_index_maps_bwd_det` (sort + segmented
     reduction, bit-reproducible) and the distortion loss comes from `neo_distortion_loss`; with the flag off the code above runs unchanged.
@@ -241,6 +244,70 @@ def _mlp_projected(mlp, enc: Tensor, dir_tile: Tensor, local_p: Tensor, world_p:
     return lin(mlp.rgb_layer, q), raw_sigma
 
 
+class _TrunkTC(torch.autograd.Function):
+    """Layers 0-3 of a NeRFPPMLP and the view mean, projected formulation, on the tensor cores (csrc/field_train.cu, bf16 operands, fp32
+    accumulation): cam (NV, M, in_ch) camera-frame encoding points, local_p / world_p (NV*M, 256) looked-up [P0 | P3], the encoding and
+    h columns of layers 0 / 3 -> hbar (M, 128) = mean over the views of h3.  The backward returns one row gradient for local_p and
+    world_p (their sum enters the layers) and every weight / bias gradient; no floating-point atomics."""
+
+    @staticmethod
+    def forward(ctx, cam, local_p, world_p, w0e, b0, w1, b1, w2, b2, w3e, b3):
+        lib = L.load()
+        nv, M, ich = cam.shape
+        f = lambda t: t.detach().contiguous().float()
+        cam_c, lp, wp = f(cam), f(local_p), f(world_p)
+        ws = [f(t) for t in (w0e, b0, w1, b1, w2, b2, w3e, b3)]
+        need = lib.neo_field_train_workspace_bytes(nv, M, ich, 0)
+        if need == 0:
+            L.check(-1)
+        saved = torch.empty(need, dtype=torch.uint8, device=cam.device)
+        hbar = torch.empty(M, 128, device=cam.device)
+        with torch.cuda.device(cam.device):
+            L.check(lib.neo_field_train_fwd(L.ptr(cam_c), L.ptr(lp), L.ptr(wp), nv, M, ich, *[L.ptr(t) for t in ws], L.ptr(hbar),
+                                            L.ptr(saved), need, _stream()))
+        ctx.save_for_backward(saved, ws[2], ws[4], ws[6])
+        ctx.dims = (nv, M, ich)
+        return hbar
+
+    @staticmethod
+    def backward(ctx, g_hbar):
+        lib = L.load()
+        saved, w1, w2, w3e = ctx.saved_tensors
+        nv, M, ich = ctx.dims
+        E, dev = 21 * ich, saved.device
+        need = lib.neo_field_train_workspace_bytes(nv, M, ich, 1)
+        if need == 0:
+            L.check(-1)
+        scratch = torch.empty(need, dtype=torch.uint8, device=dev)
+        d_pm = torch.empty(nv * M, 256, device=dev)
+        g = [torch.empty(128, E, device=dev), torch.empty(128, device=dev), torch.empty(128, 128, device=dev), torch.empty(128, device=dev),
+             torch.empty(128, 128, device=dev), torch.empty(128, device=dev), torch.empty(128, 128 + E, device=dev), torch.empty(128, device=dev)]
+        with torch.cuda.device(dev):
+            L.check(lib.neo_field_train_bwd(L.ptr(g_hbar.contiguous().float()), nv, M, ich, L.ptr(w1), L.ptr(w2), L.ptr(w3e), L.ptr(saved),
+                                            saved.numel(), L.ptr(d_pm), *[L.ptr(t) for t in g], L.ptr(scratch), need, _stream()))
+        return (None, d_pm, d_pm, *g)
+
+
+def _mlp_projected_tc(mlp, cam: Tensor, dir_tile: Tensor, local_p: Tensor, world_p: Tensor, nv: int):
+    """`_mlp_projected` with the trunk (layers 0-3 and the view mean) on the tensor cores (`_TrunkTC`).  The head is re-associated
+    exactly: bottleneck -> views_linear.0 is linear and so is the view mean, so it runs once per point on hbar and the view mean of the
+    direction encodings, in fp32."""
+    E = 21 * cam.shape[-1]
+    lin = lambda m, x: F.linear(x, m.weight, m.bias)
+    p = mlp.pts_linears
+    hbar = _TrunkTC.apply(cam, local_p, world_p, p[0].weight[:, :E], p[0].bias, p[1].weight, p[1].bias, p[2].weight, p[2].bias,
+                          p[3].weight[:, :128 + E], p[3].bias)
+    M = hbar.shape[0]
+    raw_sigma = lin(mlp.density_layer, hbar)
+    dbar = dir_tile.reshape(nv, M, -1).mean(0)
+    q = lin(mlp.views_linear[0], torch.cat([lin(mlp.bottleneck_layer, hbar), dbar], -1))
+    q = torch.relu(lin(mlp.views_linear[1], torch.relu(q)))
+    return lin(mlp.rgb_layer, q), raw_sigma
+
+
+TRAIN_PRECISIONS = ("fp32", "tc")
+
+
 def render_train(net, rays: Dict[str, Tensor], planes: List[Tensor], latent: Tensor, randomized: bool, white_bkgd: bool,
                  out_depth: bool = False, uniforms: Optional[List[Tensor]] = None):
     """NeRF_TP.forward (model.py:266-581, encoder hoisted) with autograd through the MLP parameters, `planes` (xz, xy, yz) and `latent`.
@@ -258,6 +325,12 @@ def render_train(net, rays: Dict[str, Tensor], planes: List[Tensor], latent: Ten
     u = uniforms if uniforms is not None else [None] * 4
     mlps = net._mlps()                                                           # fg_coarse, bg_coarse, fg_fine, bg_fine
     projected = getattr(net, "train_projected", True)
+    tc = getattr(net, "train_precision", "fp32")
+    if tc not in TRAIN_PRECISIONS:
+        raise ValueError(f"train_precision must be one of {TRAIN_PRECISIONS}, got {tc!r}")
+    tc = tc == "tc"
+    if tc and not projected:
+        raise ValueError("train_precision='tc' runs the projected formulation only: set train_projected=True")
     if projected:
         latent_cl = latent.permute(0, 2, 3, 1)                                   # channel-last views: the projection contracts the last axis
         planes_cl = [pl.permute(0, 2, 3, 1) for pl in planes]
@@ -281,7 +354,10 @@ def render_train(net, rays: Dict[str, Tensor], planes: List[Tensor], latent: Ten
             if projected:
                 pl_cl, pp_cl = _project_maps(mlp, 63 if b == 0 else 84, latent_cl, planes_cl)
                 local_p, world_p = _LookupMaps.apply(look_pts.reshape(-1, 3), pl_cl, pp_cl[0], pp_cl[1], pp_cl[2], net)
-                raw_rgb, raw_sigma = _mlp_projected(mlp, _pos_enc(cam, 0, 10), dir_tile, local_p, world_p, nv)
+                if tc:
+                    raw_rgb, raw_sigma = _mlp_projected_tc(mlp, cam, dir_tile, local_p, world_p, nv)
+                else:
+                    raw_rgb, raw_sigma = _mlp_projected(mlp, _pos_enc(cam, 0, 10), dir_tile, local_p, world_p, nv)
             else:
                 world, local = _Lookup.apply(look_pts.reshape(-1, 3), planes[0], planes[1], planes[2], latent, net)
                 raw_rgb, raw_sigma = _mlp(mlp, _pos_enc(cam, 0, 10), dir_tile, world, local, nv)
