@@ -504,6 +504,34 @@ int neo_field_train_bwd(const float* g_hbar, int nv, int M, int in_ch, const flo
                         const void* saved, size_t saved_bytes, float* d_pm, float* gw0, float* gb0, float* gw1, float* gb1,
                         float* gw2, float* gb2, float* gw3, float* gb3, void* scratch, size_t scratch_bytes, void* stream);
 
+/* ---- Vanilla NeRF and Mip-NeRF 360 training on the tensor cores (csrc/dense_train.cu, csrc/gemm_tc.cu): the products of their dense
+ * layers, bf16 operands (row-major, row strides in elements), fp32 accumulation, asynchronous on `stream`, no floating-point atomics.
+ * Each returns NEO_ERR_INVALID before any launch on a NULL buffer it needs, a shape or stride outside its contract, or a misaligned
+ * operand, with neo_last_error naming the entry point.
+ * neo_tc_gemm_bf16: C (M,N; ldc) = A (M,K; lda) . W (N,K; ldw)^T + bias (N, fp32 or NULL), then epilogue 0 = ReLU -> bf16, 1 -> bf16,
+ *   2 = no bias -> fp32.  Shape rules of neo_tc_gemm_f16 (K % 64, N % 64, strides % 8, 16-byte aligned); writes columns [0, N) of C only.
+ * neo_tc_dgrad_bf16: dX (M,N; lddx) bf16 = (dY (M,K; ldy) . Wt (N,K; ldwt)^T + g_sig w_sig^T) [X > 0]: Wt = W^T of the layer's weight,
+ *   X (M,N; ldx) its saved bf16 input (NULL: no mask), g_sig (M) and w_sig (N) fp32 or both NULL.  Shape rules of neo_tc_gemm_bf16.
+ * neo_tc_wgrad_bf16: dW (N, k_valid) fp32 = dY (M,N; ldy)^T X (M,K; ldx), columns k >= k_valid dropped; db (N) = column sums of dY, or
+ *   NULL.  N % 64, K % 64, N*K*4 <= 32 MB, strides % 8, 16-byte aligned dY, X and workspace; the workspace is
+ *   neo_tc_wgrad_bf16_workspace_bytes(M, N, K) bytes (0 = invalid shape), NEO_ERR_WORKSPACE if short.  Written, not accumulated.
+ * neo_tc_pack_bf16: bf16 copy of an fp32 (rows, cols_in; ld_in) matrix: transpose 0 -> out (rows, cols_out; ld_out), zero columns past
+ *   cols_in; transpose 1 -> out (cols_out, rows; ld_out) = the first cols_out columns transposed.
+ * neo_tc_relu_rank1_bf16: out (M,N; ldo) bf16 = (g (M) w (N)^T) [X (M,N; ldx) > 0], fp32 product rounded once.
+ * neo_tc_rowdot_bf16: neo_tc_rowdot_f16 with a bf16 H (the density head over the last trunk activation). ---- */
+int neo_tc_gemm_bf16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M,
+                     int N, int K, int epilogue, void* stream);
+int neo_tc_dgrad_bf16(const void* dY, long long ldy, const void* Wt, long long ldwt, const void* X, long long ldx, const float* g_sig,
+                      const float* w_sig, void* dX, long long lddx, long long M, int N, int K, void* stream);
+size_t neo_tc_wgrad_bf16_workspace_bytes(long long M, int N, int K);
+int neo_tc_wgrad_bf16(const void* dY, long long ldy, const void* X, long long ldx, long long M, int N, int K, float* dW, int k_valid,
+                      float* db, void* workspace, size_t workspace_bytes, void* stream);
+int neo_tc_pack_bf16(const float* in, long long rows, int cols_in, long long ld_in, void* out, int cols_out, long long ld_out, int transpose,
+                     void* stream);
+int neo_tc_relu_rank1_bf16(const float* g, const float* w, const void* X, long long ldx, long long M, int N, void* out, long long ldo,
+                           void* stream);
+int neo_tc_rowdot_bf16(const void* H, long long ld, int K, const float* W, const float* b, int N, long long M, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -161,6 +161,17 @@ SYMBOLS = {
     "neo_tc_gemm_f16": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong, C.c_longlong,
                                   C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "neo_tc_rowdot_f16": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]),
+    "neo_tc_gemm_bf16": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong, C.c_longlong,
+                                   C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "neo_tc_dgrad_bf16": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_longlong, C.c_longlong, C.c_int, C.c_int, C.c_void_p]),
+    "neo_tc_wgrad_bf16_workspace_bytes": (C.c_size_t, [C.c_longlong, C.c_int, C.c_int]),
+    "neo_tc_wgrad_bf16": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_longlong, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                    C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "neo_tc_pack_bf16": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_longlong, C.c_void_p, C.c_int, C.c_longlong, C.c_int, C.c_void_p]),
+    "neo_tc_relu_rank1_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.c_longlong, C.c_int, C.c_void_p, C.c_longlong,
+                                         C.c_void_p]),
+    "neo_tc_rowdot_bf16": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]),
     "neo_tc_enc_column": (C.c_int, [C.c_int, C.c_int]),
     "neo_tc_trap_info": (C.c_char_p, []),
     "neo_last_error": (C.c_char_p, []),

@@ -336,6 +336,15 @@ int launch_field_tc(const NeoScene* sc, const NeoRays* rays, const float* far, c
 // gemm_tc.cu: the tensor-core dense layer, fp16 operand packing and the tiny-N head (contracts at their definitions)
 int gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M, int N, int K,
              int relu, cudaStream_t s);
-int f32_to_f16_pad(const float* in, long long rows, int cols_in, long long ld_in, void* out, int cols_out, long long ld_out, cudaStream_t s);
-int launch_rowdot_f16(const void* H, long long ld, int K, const float* W, const float* b, int N, long long M, float* out, cudaStream_t s);
+int f32_to_f16_pad(const float* in, long long rows, int cols_in, long long ld_in, void* out, int cols_out, long long ld_out, cudaStream_t s,
+                   int bf16 = 0);
+int launch_rowdot_f16(const void* H, long long ld, int K, const float* W, const float* b, int N, long long M, float* out, cudaStream_t s,
+                      int bf16 = 0);
+// gemm_tc.cu: the bf16 training forms of the same dense layer (csrc/dense_train.cu)
+int gemm_bf16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M, int N, int K,
+              int epi, cudaStream_t s);
+int dgrad_bf16(const void* dY, long long ldy, const void* Wt, long long ldwt, const void* X, long long ldx, const float* g_sig,
+               const float* w_sig, void* dX, long long lddx, long long M, int N, int K, cudaStream_t s);
+int wgrad_bf16_partials(const void* dY, long long ldy, const void* X, long long ldx, long long M, int N, int K, int splits, float* part,
+                        cudaStream_t s);
 }  // namespace neo

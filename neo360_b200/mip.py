@@ -10,7 +10,8 @@ Training: with autograd on, the module in train mode and parameters that require
 `(renderings, ray_history)` differentiable w.r.t. every MLP parameter (LitMipNeRF360.training_step, model.py:427-456): `density`, `rgb`
 and `weights` of every level and each level's rendered `rgb` carry gradients, `sdist` is detached (model.py:309-310) and the proposal
 levels' `rgb` are zeros.  Resampling, IPE features, direction encoding and compositing forward and backward are hand-written CUDA; the
-dense layers are framework fp32 GEMMs under autograd.  `precision` applies to inference only: training runs fp32 whatever it is set to.
+dense layers are framework fp32 GEMMs under autograd, or with `train_precision="tc"` bf16 tensor-core GEMMs forward and backward
+(training._MLPTrainTC, csrc/dense_train.cu).  `precision` applies to inference only.
 `training_loss` is the reference's training loss on those outputs."""
 from __future__ import annotations
 
@@ -23,7 +24,7 @@ import torch.nn.functional as F
 
 from . import _lib as L
 from .mip_basis import POS_BASIS_T
-from .training import distortion_loss
+from .training import check_train_precision, distortion_loss, mlp_train_tc
 
 
 class MipNeRF360MLP(nn.Module):
@@ -73,8 +74,9 @@ class PropMLP(MipNeRF360MLP):
 
 class MipNeRF360(nn.Module):
     def __init__(self, num_prop_samples: int = 64, num_nerf_samples: int = 32, num_levels: int = 3, precision: str = "fp32",
-                 **reference_defaults):
+                 train_precision: str = "fp32", **reference_defaults):
         super().__init__()
+        self.train_precision = check_train_precision(train_precision)   # "fp32": framework GEMMs; "tc": bf16 tensor cores (training only)
         self.precision = precision          # "fp32": CUDA-core SGEMM chain (tight parity); "tc": every dense layer on the tensor cores (fp16 operands)
         if num_levels != 3 or reference_defaults:
             raise NotImplementedError("reference defaults only (models/mipnerf360/model.py:199-223)")
@@ -127,7 +129,7 @@ class MipNeRF360(nn.Module):
     def _forward_train(self, batch: Dict[str, torch.Tensor], train_frac: float, randomized: bool, near, far) -> Tuple[List[dict], List[dict]]:
         """MipNeRF360.forward under autograd (what LitMipNeRF360.training_step calls, model.py:427-456).  Per level: `neo_mip_resample` on the
         detached previous weights, `neo_mip_encode`, the MLP as `F.linear` on the modules' own parameters (fp32 whatever `self.precision`
-        is), then `_MipComposite` (the eval path's compositing kernel forward, `neo_mip_composite_bwd` backward)."""
+        is; bf16 tensor-core GEMMs, `training.mlp_train_tc`, with `self.train_precision == "tc"`), then `_MipComposite` (the eval path's compositing kernel forward, `neo_mip_composite_bwd` backward)."""
         o = batch["rays_o"].contiguous().float()
         if not o.is_cuda:
             raise RuntimeError("neo360_b200 needs CUDA tensors (no CPU fallback)")
@@ -141,6 +143,7 @@ class MipNeRF360(nn.Module):
             jit = [j.reshape(-1).contiguous().float() for j in jit]
         stream = torch.cuda.current_stream(dev).cuda_stream
         ns = (self.num_prop_samples, self.num_prop_samples, self.num_nerf_samples)
+        tc = check_train_precision(self.train_precision) == "tc"
         ren, hist = [], []
         sdist = w = None
         for lvl, mlp in enumerate(self.mlps):
@@ -155,7 +158,11 @@ class MipNeRF360(nn.Module):
                 basis = mlp.pos_basis_t.to(dev).contiguous().float()
                 L.check(lib.neo_mip_encode(L.ptr(o), L.ptr(d), L.ptr(vd), L.ptr(radii), L.ptr(t1), L.ptr(basis), n, N, L.ptr(feats), L.ptr(denc),
                                            stream))
-            raw_density, raw_rgb = _mlp_train(mlp, feats, denc, n, N)
+            if tc:
+                raw_density, raw_rgb = mlp_train_tc(mlp, feats, denc, n, N)
+                raw_density = raw_density.reshape(n, N)
+            else:
+                raw_density, raw_rgb = _mlp_train(mlp, feats, denc, n, N)
             rgb, w, density, rgb_s = _MipComposite.apply(raw_density, raw_rgb, t1, d)
             ren.append({"rgb": rgb})
             hist.append({"density": density, "rgb": rgb_s, "sdist": sdist, "weights": w})

@@ -308,6 +308,153 @@ def _mlp_projected_tc(mlp, cam: Tensor, dir_tile: Tensor, local_p: Tensor, world
 TRAIN_PRECISIONS = ("fp32", "tc")
 
 
+def check_train_precision(p: str) -> str:
+    if p not in TRAIN_PRECISIONS:
+        raise ValueError(f"train_precision must be one of {TRAIN_PRECISIONS}, got {p!r}")
+    return p
+
+
+def _bf16(*shape, dev):
+    return torch.empty(*shape, dtype=torch.bfloat16, device=dev)
+
+
+def _ceil64(x: int) -> int:
+    return (x + 63) // 64 * 64
+
+
+class _MLPTrainTC(torch.autograd.Function):
+    """The dense layers of vanilla NeRF's NeRFMLP and Mip-NeRF 360's PropMLP / NeRFMLP on the tensor cores (csrc/dense_train.cu and
+    gemm_tc.cu: bf16 operands, fp32 accumulation, no floating-point atomics).  `depth` ReLU layers of width W on feats (M, F), the
+    features concatenated after layer 4 when depth > 5, then the density head (bf16 rowdot) and, when the bottleneck parameters are
+    given, the bottleneck and the beta columns of views_linear.0 (no bias).  params = w_i, b_i for every layer, density w, b, then
+    optionally bottleneck w, b and views_linear.0.weight[:, :256] -> raw sigma (M, 1) fp32 and, with the bottleneck, y_beta (M, 128) fp32.
+    Activations live in bf16: feats sit beside h4 in one [h4 | feats] buffer, so the skip layer reads one operand and the concatenation
+    is never copied.  The backward runs dgrad (ReLU mask of the saved layer input in its epilogue, the density head's rank-1 gradient
+    added to the last activation's) and wgrad per layer."""
+
+    @staticmethod
+    def forward(ctx, depth, feats, *params):
+        lib = L.load()
+        dev, s = feats.device, _stream()
+        M, F = feats.shape
+        f = lambda t: t.detach().contiguous().float()
+        P = [f(t) for t in params]
+        ws = [(P[2 * i], P[2 * i + 1]) for i in range(depth)]
+        wsig, bsig = P[2 * depth], P[2 * depth + 1]
+        rgb = len(P) > 2 * depth + 2
+        W, Kf = ws[0][0].shape[0], _ceil64(F)
+        skip = depth > 5
+        fo = W if skip else 0
+        XS = _bf16(M, fo + Kf, dev=dev)                                          # [h4 | feats] (feats alone without a skip)
+        e = XS.data_ptr() + 2 * fo
+        fc = f(feats)
+        with torch.cuda.device(dev):
+            L.check(lib.neo_tc_pack_bf16(L.ptr(fc), M, F, F, e, Kf, fo + Kf, 0, s))
+            H, Wp, WT, X = [], [], [], []
+            for i, (w, b) in enumerate(ws):
+                kin = Kf if i == 0 else (W + Kf if skip and i == 5 else W)
+                wp = _bf16(W, kin, dev=dev)
+                L.check(lib.neo_tc_pack_bf16(L.ptr(w), W, w.shape[1], w.shape[1], wp.data_ptr(), kin, kin, 0, s))
+                Wp.append(wp)
+                if i > 0:
+                    wt = _bf16(W, W, dev=dev)
+                    L.check(lib.neo_tc_pack_bf16(L.ptr(w), W, w.shape[1], w.shape[1], wt.data_ptr(), W, W, 1, s))
+                    WT.append(wt)
+                x = (e, fo + Kf) if i == 0 else ((XS.data_ptr(), W + Kf) if skip and i == 5 else (H[-1].data_ptr(), W))
+                X.append(x + (kin,))
+                h = XS if skip and i == 4 else _bf16(M, W, dev=dev)
+                L.check(lib.neo_tc_gemm_bf16(x[0], x[1], wp.data_ptr(), kin, L.ptr(b), h.data_ptr(), W + Kf if h is XS else W, M, W, kin, 0, s))
+                H.append(h)
+            hl = H[-1]
+            sig = torch.empty(M, 1, device=dev)
+            L.check(lib.neo_tc_rowdot_bf16(hl.data_ptr(), W, W, L.ptr(wsig), L.ptr(bsig), 1, M, L.ptr(sig), s))
+            out, saved = (sig,), []
+            if rgb:
+                wb, bb, wv = P[2 * depth + 2], P[2 * depth + 3], P[2 * depth + 4]
+                nb, nv = wb.shape[0], wv.shape[0]
+                wbp, wvp, wbt, wvt = _bf16(nb, W, dev=dev), _bf16(nv, nb, dev=dev), _bf16(W, nb, dev=dev), _bf16(nb, nv, dev=dev)
+                L.check(lib.neo_tc_pack_bf16(L.ptr(wb), nb, W, W, wbp.data_ptr(), W, W, 0, s))
+                L.check(lib.neo_tc_pack_bf16(L.ptr(wv), nv, nb, nb, wvp.data_ptr(), nb, nb, 0, s))
+                L.check(lib.neo_tc_pack_bf16(L.ptr(wb), nb, W, W, wbt.data_ptr(), W, nb, 1, s))
+                L.check(lib.neo_tc_pack_bf16(L.ptr(wv), nv, nb, nb, wvt.data_ptr(), nb, nv, 1, s))
+                beta = _bf16(M, nb, dev=dev)
+                yb = torch.empty(M, nv, device=dev)
+                L.check(lib.neo_tc_gemm_bf16(hl.data_ptr(), W, wbp.data_ptr(), W, L.ptr(bb), beta.data_ptr(), nb, M, nb, W, 1, s))
+                L.check(lib.neo_tc_gemm_bf16(beta.data_ptr(), nb, wvp.data_ptr(), nb, None, yb.data_ptr(), nv, M, nv, nb, 2, s))
+                out, saved = (sig, yb), [beta, wbt, wvt]
+        ctx.save_for_backward(XS, *H, *WT, wsig, *saved)
+        ctx.meta = (depth, M, F, W, Kf, fo, X, [w.shape[1] for w, _ in ws], rgb)
+        return out if rgb else sig
+
+    @staticmethod
+    def backward(ctx, g_sig, g_yb=None):
+        lib = L.load()
+        depth, M, F, W, Kf, fo, X, kvalid, rgb = ctx.meta
+        T = ctx.saved_tensors
+        XS, H, WT, wsig = T[0], T[1:1 + depth], T[1 + depth:2 * depth], T[2 * depth]
+        hl = H[-1]
+        dev, s = XS.device, _stream()
+        g_sig = torch.zeros(M, 1, device=dev) if g_sig is None else g_sig.contiguous().float()
+        calls = [(M, 64, W)] + [(M, W, x[2]) for x in X]
+        if rgb:
+            beta, wbt, wvt = T[2 * depth + 1:]
+            nb, nv = beta.shape[1], wvt.shape[1]
+            calls += [(M, nv, nb), (M, nb, W)]
+        need = max(lib.neo_tc_wgrad_bf16_workspace_bytes(*c) for c in calls)
+        if need == 0:
+            L.check(-1)
+        ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        wg = lambda dy, ldy, x, ldx, N, K, dw, kv, db: L.check(lib.neo_tc_wgrad_bf16(dy, ldy, x, ldx, M, N, K, L.ptr(dw), kv, L.ptr(db),
+                                                                                     L.ptr(ws), need, s))
+        G = [_bf16(M, W, dev=dev), _bf16(M, W, dev=dev)]
+        grads = [None] * (2 * depth + 2)
+        extra = []
+        with torch.cuda.device(dev):
+            if rgb:
+                g_yb = torch.zeros(M, nv, device=dev) if g_yb is None else g_yb.contiguous().float()
+                dyb, dbeta = _bf16(M, nv, dev=dev), _bf16(M, nb, dev=dev)
+                gwv, gwb, gbb = torch.empty(nv, nb, device=dev), torch.empty(nb, W, device=dev), torch.empty(nb, device=dev)
+                L.check(lib.neo_tc_pack_bf16(L.ptr(g_yb), M, nv, nv, dyb.data_ptr(), nv, nv, 0, s))
+                wg(dyb.data_ptr(), nv, beta.data_ptr(), nb, nv, nb, gwv, nb, None)
+                L.check(lib.neo_tc_dgrad_bf16(dyb.data_ptr(), nv, wvt.data_ptr(), nv, None, 0, None, None, dbeta.data_ptr(), nb, M, nb, nv, s))
+                wg(dbeta.data_ptr(), nb, hl.data_ptr(), W, nb, W, gwb, W, gbb)
+                L.check(lib.neo_tc_dgrad_bf16(dbeta.data_ptr(), nb, wbt.data_ptr(), nb, hl.data_ptr(), W, L.ptr(g_sig), L.ptr(wsig),
+                                              G[0].data_ptr(), W, M, W, nb, s))
+                extra = [gwb, gbb, gwv]
+            else:
+                L.check(lib.neo_tc_relu_rank1_bf16(L.ptr(g_sig), L.ptr(wsig), hl.data_ptr(), W, M, W, G[0].data_ptr(), W, s))
+            gs = _bf16(M, 64, dev=dev)
+            gwsig = torch.empty(64, W, device=dev)
+            L.check(lib.neo_tc_pack_bf16(L.ptr(g_sig), M, 1, 1, gs.data_ptr(), 64, 64, 0, s))
+            wg(gs.data_ptr(), 64, hl.data_ptr(), W, 64, W, gwsig, W, None)
+            grads[2 * depth], grads[2 * depth + 1] = gwsig[:1].clone(), g_sig.sum(0)
+            for i in range(depth - 1, -1, -1):
+                xp, ldx, kin = X[i]
+                gw, gb = torch.empty(W, kvalid[i], device=dev), torch.empty(W, device=dev)
+                wg(G[0].data_ptr(), W, xp, ldx, W, kin, gw, kvalid[i], gb)
+                grads[2 * i], grads[2 * i + 1] = gw, gb
+                if i > 0:
+                    L.check(lib.neo_tc_dgrad_bf16(G[0].data_ptr(), W, WT[i - 1].data_ptr(), W, xp, ldx, None, None, G[1].data_ptr(), W, M, W, W, s))
+                    G.reverse()
+        return (None, None, *grads, *extra)
+
+
+def mlp_train_tc(m, feats: Tensor, denc: Tensor, n: int, N: int):
+    """`_mlp_train` of vanilla.NeRFMLP, mip.PropMLP or mip.NeRFMLP with the dense layers on the tensor cores (`_MLPTrainTC`): feats
+    (n*N, F), denc (n, 27) -> raw sigma (n*N, 1), raw rgb (n, N, 3) or None.  The direction columns of views_linear.0 with its bias and
+    ReLU, and rgb_layer, stay fp32 framework ops, the direction columns applied once per ray."""
+    layers = m.pts_linears if hasattr(m, "pts_linears") else m.pts_linear
+    params = [t for lin in layers for t in (lin.weight, lin.bias)] + [m.density_layer.weight, m.density_layer.bias]
+    rgb = hasattr(m, "rgb_layer")
+    if not rgb:
+        return _MLPTrainTC.apply(len(layers), feats, *params), None
+    v, kb = m.views_linear[0], m.bottleneck_layer.out_features
+    params += [m.bottleneck_layer.weight, m.bottleneck_layer.bias, v.weight[:, :kb]]
+    sig, yb = _MLPTrainTC.apply(len(layers), feats, *params)
+    y = yb.reshape(n, N, -1) + F.linear(denc, v.weight[:, kb:], v.bias)[:, None, :]
+    return sig, F.linear(torch.relu(y), m.rgb_layer.weight, m.rgb_layer.bias)
+
+
 def render_train(net, rays: Dict[str, Tensor], planes: List[Tensor], latent: Tensor, randomized: bool, white_bkgd: bool,
                  out_depth: bool = False, uniforms: Optional[List[Tensor]] = None):
     """NeRF_TP.forward (model.py:266-581, encoder hoisted) with autograd through the MLP parameters, `planes` (xz, xy, yz) and `latent`.

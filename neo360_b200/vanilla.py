@@ -7,8 +7,8 @@ formulation; `"tc"` runs them as fp16 wgmma GEMMs with fp32 accumulation (csrc/g
 
 Training: with autograd on, the module in train mode and parameters that require grad, `NeRF.forward` returns the same tuples
 differentiable w.r.t. every MLP parameter (LitNeRF.training_step, model.py:273-299).  Sampling, encodings and compositing forward and
-backward are hand-written CUDA; the dense layers are framework fp32 GEMMs under autograd.  `precision` applies to inference only: training
-runs fp32 whatever it is set to.  After an optimiser step the next inference call re-packs the weights (`_ensure` keys on each
+backward are hand-written CUDA; the dense layers are framework fp32 GEMMs under autograd, or with `train_precision="tc"` bf16 tensor-core
+GEMMs forward and backward (training._MLPTrainTC, csrc/dense_train.cu).  `precision` applies to inference only.  After an optimiser step the next inference call re-packs the weights (`_ensure` keys on each
 parameter's storage and version)."""
 from __future__ import annotations
 
@@ -20,7 +20,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib as L
-from .training import _Composite
+from .training import _Composite, check_train_precision, mlp_train_tc
 
 
 class NeRFMLP(nn.Module):
@@ -81,8 +81,10 @@ def _mlp_train(m: NeRFMLP, enc: torch.Tensor, denc: torch.Tensor, n: int, N: int
 
 class NeRF(nn.Module):
     def __init__(self, num_levels: int = 2, min_deg_point: int = 0, max_deg_point: int = 10, deg_view: int = 4, num_coarse_samples: int = 64,
-                 num_fine_samples: int = 128, use_viewdirs: bool = True, noise_std: float = 0.0, lindisp: bool = False):
+                 num_fine_samples: int = 128, use_viewdirs: bool = True, noise_std: float = 0.0, lindisp: bool = False,
+                 train_precision: str = "fp32"):
         super().__init__()
+        self.train_precision = check_train_precision(train_precision)   # "fp32": framework GEMMs; "tc": bf16 tensor cores (training only)
         if num_levels != 2 or lindisp or noise_std != 0.0 or not use_viewdirs:
             raise NotImplementedError("reference defaults only (models/vanilla_nerf/model.py:129-139)")
         self.num_coarse_samples, self.num_fine_samples = num_coarse_samples, num_fine_samples
@@ -167,7 +169,7 @@ class NeRF(nn.Module):
         """NeRF.forward under autograd (what LitNeRF.training_step calls, models/vanilla_nerf/model.py:273-299): the same tuples,
         differentiable w.r.t. every parameter of coarse_mlp and fine_mlp.  Sampling, encodings and compositing (forward and backward) are
         the library's stages; the NeRFMLP layers are framework GEMMs (`F.linear`) on the modules' own parameters, in fp32 whatever
-        `self.precision` is.  `debug=True` keeps each level's sample positions and (detached) weights in `self.last_debug`."""
+        `self.precision` is, or with `self.train_precision == "tc"` bf16 tensor-core GEMMs (`training.mlp_train_tc`).  `debug=True` keeps each level's sample positions and (detached) weights in `self.last_debug`."""
         o = rays["rays_o"].contiguous().float()
         d = rays["rays_d"].contiguous().float()
         vd = rays["viewdirs"].contiguous().float()
@@ -181,6 +183,7 @@ class NeRF(nn.Module):
             u = rays.get("_uniforms") or [torch.rand((n, nc + 1), device=dev), torch.rand((n, nf), device=dev)]   # helper.py:438, 587
             u = [x.contiguous().float() for x in u]
         stream = torch.cuda.current_stream(dev).cuda_stream
+        tc = check_train_precision(self.train_precision) == "tc"
         ret, t, w = [], None, None
         dbg = {"t": [], "weights": []}
         for lvl, mlp in enumerate((self.coarse_mlp, self.fine_mlp)):
@@ -196,7 +199,11 @@ class NeRF(nn.Module):
                 N = t.shape[1]
                 enc, denc = torch.empty(n * N, 63, device=dev), torch.empty(n, 27, device=dev)
                 L.check(lib.neo_vanilla_encode(L.ptr(o), L.ptr(vd), L.ptr(t), n, N, L.ptr(enc), L.ptr(denc), stream))
-            raw_rgb, raw_sigma = _mlp_train(mlp, enc, denc, n, N)
+            if tc:
+                raw_sigma, raw_rgb = mlp_train_tc(mlp, enc, denc, n, N)
+                raw_sigma = raw_sigma.reshape(n, N, 1)
+            else:
+                raw_rgb, raw_sigma = _mlp_train(mlp, enc, denc, n, N)
             rgb = torch.sigmoid(raw_rgb) * (1 + 2 * 0.001) - 0.001              # model.py:197-205
             sigma = F.softplus(raw_sigma - 1.0)
             comp, acc, w, _, depth = _Composite.apply(rgb, sigma, t, d, None, white_bkgd, 2)
