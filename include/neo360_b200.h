@@ -480,6 +480,13 @@ int neo_tc_rowdot_f16(const void* H, long long ld, int K, const float* W, const 
  * -1 for the constant-one (bias) column, -2 for a zero padding column, -3 for invalid arguments.  Pure host code (no GPU). */
 int neo_tc_enc_column(int in_ch, int col);
 
+/* NEO_PREC_TC: the direction fragments of `rays` (exposed for tests; neo_render_fwd and neo_field_eval compute them before their field
+ * launches).  For every ray r, the mean over the scene's source views of the direction encoding of viewdirs[r] in the view's camera
+ * frame (model.py:357-360: [d, sin(2^k d), sin(2^k d + pi/2)], k < 4, 27 columns, then 5 zero columns), fp16, as the field kernel's
+ * A fragments: out + 64 r + 16 t (t < 4) holds the fp16 pairs of columns {16 ks + 8 h + 2 t, + 1} in the order (ks, h) = (0,0),
+ * (0,1), (1,0), (1,1).  out: n_rays * 64 bytes, 16-byte aligned. */
+int neo_tc_dir_fragments(const NeoScene* scene, const NeoRays* rays, void* out, void* stream);
+
 /* "" or a description of the mbarrier wait that timed out inside the NEO_PREC_TC field kernel (the kernel bounds its wait for the
  * weight copies and traps instead of hanging; the waiter's identity is recorded in host-mapped memory, which survives the failed context). */
 const char* neo_tc_trap_info(void);

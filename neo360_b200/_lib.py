@@ -173,6 +173,7 @@ SYMBOLS = {
                                          C.c_void_p]),
     "neo_tc_rowdot_bf16": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]),
     "neo_tc_enc_column": (C.c_int, [C.c_int, C.c_int]),
+    "neo_tc_dir_fragments": (C.c_int, [C.c_void_p, C.POINTER(NeoRays), C.c_void_p, C.c_void_p]),
     "neo_tc_trap_info": (C.c_char_p, []),
     "neo_last_error": (C.c_char_p, []),
     "neo_version": (C.c_char_p, []),

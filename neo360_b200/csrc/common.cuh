@@ -331,7 +331,10 @@ void index_det_sizes(const NeoScene* sc, int M, bool local, bool world, long lon
 // field_tc.cu
 int tc_scene_create(NeoScene* sc, const NeoMLPParams mlps[4], cudaStream_t s);
 void tc_scene_free(NeoScene* sc);
-int launch_field_tc(const NeoScene* sc, const NeoRays* rays, const float* far, const float* t, int N, int mlp_index,
+// direction fragments of every ray for the field launches of one call: kDirFragBytes per ray, 16-byte aligned
+constexpr size_t kDirFragBytes = 64;
+int launch_dir_frags(const NeoScene* sc, const NeoRays* rays, void* dir, cudaStream_t s);
+int launch_field_tc(const NeoScene* sc, const NeoRays* rays, const float* far, const float* t, int N, int mlp_index, const void* dir,
                     float* rgb, float* sigma, cudaStream_t s);
 // gemm_tc.cu: the tensor-core dense layer, fp16 operand packing and the tiny-N head (contracts at their definitions)
 int gemm_f16(const void* A, long long lda, const void* W, long long ldw, const float* bias, void* C, long long ldc, long long M, int N, int K,

@@ -79,7 +79,8 @@ struct State {
 };
 
 struct Params {
-    const float *rays_o, *rays_d, *viewdirs, *far, *tvals;
+    const float *rays_o, *rays_d, *far, *tvals;
+    const uint4* dir;   // direction fragments of every ray (dir_frag_kernel), 4 per ray
     const int* ray_order;
     int n_rays, N, chunk, nv, n_tiles, sg;
     float far_unc;
@@ -98,7 +99,8 @@ struct Params {
 // into the launch's row of g_phase_cycles.  The marks bound the phases as the compiler scheduled them, which is close to, but not
 // exactly, the source order.  Without the macro the kernel has no marks at all.
 #ifdef NEO_FIELD_PHASES
-constexpr int kPhases = 8;          // tile setup | camera + encodings | tap table | blend P0 | layers 0-2 | blend P3 | layer 3 + head | colour head + stores
+constexpr int kPhases = 9;          // tile setup | camera + encodings | tap table | blend P0 | layers 0-2 | blend P3 | layer 3 + head |
+                                    // direction term | colour head + stores
 constexpr int kPhaseCols = kPhases + 2;                                  // the phases, then tiles, then taps of non-zero weight
 constexpr uint32_t kPhaseBytes = kWarpgroups * (kPhases + 1) * 8;        // per-warpgroup sums (phases, tiles) in shared memory
 constexpr int kPhaseSlots = 64;
@@ -362,6 +364,34 @@ __device__ __forceinline__ float dir_value(const float* dc, int e) {
     const int qq = shifted ? q0 - 12 : q0;
     const float xb = sel4(dc, qq % 3) * (float)(1 << (qq / 3));
     return sinf(shifted ? xb + 1.57079637f : xb);
+}
+
+// Direction fragments.  The direction term of the head, hacc += mean_v(dir_enc_v) . Whead_dir^T (K = 32: 27 columns + zero padding),
+// has an A operand that depends only on the conditioning ray of the point (quirk Q1) and the source cameras, so it is computed once
+// per ray and call (dir_frag_kernel) and every field launch of the call loads it.  Record of a ray: 64 bytes, 16 per thread t (lane
+// % 4) of an accumulator quad: word 2 ks + h packs columns 16 ks + 8 h + 2 t + {0, 1}, i.e. the thread's A-fragment words (k-step ks,
+// half h) of one row.  The view sum runs over the views in order, then is scaled by 1 / nv and rounded to fp16.
+__device__ __forceinline__ uint4 dir_words(const ViewXform* vxs, int nv, const float (&wd)[3], int t) {
+    float dsum[8];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) dsum[c] = 0.f;
+    for (int vv = 0; vv < nv; ++vv) {
+        float dc[3];
+        rotate_to_camera(vxs[vv], wd, dc);
+#pragma unroll
+        for (int c = 0; c < 8; ++c) dsum[c] += dir_value(dc, 16 * (c >> 2) + 8 * ((c >> 1) & 1) + 2 * t + (c & 1));
+    }
+    const float inv = 1.0f / (float)nv;
+    return make_uint4(pack_h2(dsum[0] * inv, dsum[1] * inv), pack_h2(dsum[2] * inv, dsum[3] * inv), pack_h2(dsum[4] * inv, dsum[5] * inv),
+                      pack_h2(dsum[6] * inv, dsum[7] * inv));
+}
+// thread 4 r + t writes the 16 bytes of thread t of ray r's record
+__global__ void dir_frag_kernel(const float* __restrict__ viewdirs, int n_rays, const ViewXform* __restrict__ views, int nv, uint4* __restrict__ out) {
+    const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= 4LL * n_rays) return;
+    const long long r = idx >> 2;
+    const float wd[3] = {viewdirs[3 * r], viewdirs[3 * r + 1], viewdirs[3 * r + 2]};
+    out[idx] = dir_words(views, nv, wd, (int)(idx & 3));
 }
 
 // rectified accumulator (NC columns) -> fp16 A fragments of the next layer (K = NC, NC / 16 k-steps)
@@ -637,39 +667,17 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
             wgmma_wait<0>();
             FIELD_PHASE(6);
         }
-        // direction term: hacc += mean_v(dir_enc_v) . Whead_dir^T   (K = 32: 27 columns + zero padding)
+        // direction term: hacc += mean_v(dir_enc_v) . Whead_dir^T, A = the direction fragments of the points' conditioning rays
         {
-            uint32_t dfr[2][4];
-            float dsum[2][8];
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                const int src = pts[r0 + 8 * i].src;
-                const float wd[3] = {P.viewdirs[3 * src], P.viewdirs[3 * src + 1], P.viewdirs[3 * src + 2]};
-#pragma unroll
-                for (int c = 0; c < 8; ++c) dsum[i][c] = 0.f;
-                for (int vv = 0; vv < nv; ++vv) {
-                    float dc[3];
-                    rotate_to_camera(vxs[vv], wd, dc);
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) dsum[i][c] += dir_value(dc, 16 * (c >> 2) + 8 * ((c >> 1) & 1) + 2 * t + (c & 1));
-                }
-            }
-            const float inv = 1.0f / (float)nv;
-#pragma unroll
-            for (int ks = 0; ks < 2; ++ks)
-#pragma unroll
-                for (int h = 0; h < 2; ++h)
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-                        const int c = 4 * ks + 2 * h;
-                        dfr[ks][2 * h + i] = pack_h2(dsum[i][c] * inv, dsum[i][c + 1] * inv);
-                    }
+            const uint4 d0 = __ldg(P.dir + 4LL * pts[r0].src + t), d1 = __ldg(P.dir + 4LL * pts[r0 + 8].src + t);
+            const uint32_t dfr[2][4] = {{d0.x, d1.x, d0.y, d1.y}, {d0.z, d1.z, d0.w, d1.w}};
             wgmma_fence();
 #pragma unroll
             for (int ks = 0; ks < 2; ++ks) wgmma_rs_n80(hacc, dfr[ks], wdesc(sH + WH_DIR, ks, 80 * 128));
             wgmma_commit();
             wgmma_wait<0>();
         }
+        FIELD_PHASE(7);
         // sigma (column 64: thread t = 0 of each quad), q = relu(hacc + bq) -> colour head 64 x 64 -> relu -> 64 x 3 -> sigmoid
         const PtsRow pr0 = pts[r0], pr1 = pts[r0 + 8];
         if (t == 0) {
@@ -724,7 +732,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
                 }
             }
         }
-        FIELD_PHASE(7);
+        FIELD_PHASE(8);
     }
 #ifdef NEO_FIELD_PHASES
     if (wt == 0)
@@ -847,10 +855,21 @@ void tc_scene_free(NeoScene* sc) {
     if (sc && sc->tc_state) { delete reinterpret_cast<tc::State*>(sc->tc_state); sc->tc_state = nullptr; }
 }
 
-int launch_field_tc(const NeoScene* sc, const NeoRays* rays, const float* far, const float* t, int N, int mlp_index,
+int launch_dir_frags(const NeoScene* sc, const NeoRays* rays, void* dir, cudaStream_t s) {
+    if (!rays->viewdirs || !dir || (uintptr_t)dir % 16) { set_error("direction fragments: need viewdirs and a 16-byte aligned output"); return NEO_ERR_INVALID; }
+    const long long threads = 4LL * rays->n_rays;
+    if (threads <= 0) return NEO_OK;
+    tc::dir_frag_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, s>>>(rays->viewdirs, rays->n_rays, sc->dev.views, sc->dev.nv,
+                                                                         static_cast<uint4*>(dir));
+    NEO_LAUNCH_CHECK("dir_frag_kernel");
+    return NEO_OK;
+}
+
+int launch_field_tc(const NeoScene* sc, const NeoRays* rays, const float* far, const float* t, int N, int mlp_index, const void* dir,
                     float* rgb, float* sigma, cudaStream_t s) {
     using namespace tc;
     if (!(sc->precision_mask & (1 << NEO_PREC_TC)) || !sc->tc_state) { set_error("scene was not prepared for NEO_PREC_TC"); return NEO_ERR_INVALID; }
+    if (!dir) { set_error("NEO_PREC_TC field launch without direction fragments"); return NEO_ERR_INVALID; }
     const State* st = reinterpret_cast<const State*>(sc->tc_state);
     static int n_sm_of[64] = {0};          // per device: a process may drive several GPUs
     int dev = 0;
@@ -859,7 +878,8 @@ int launch_field_tc(const NeoScene* sc, const NeoRays* rays, const float* far, c
     if (!n_sm_of[dev]) NEO_CUDA(cudaDeviceGetAttribute(&n_sm_of[dev], cudaDevAttrMultiProcessorCount, dev));
     const int n_sm = n_sm_of[dev];
     Params P;
-    P.rays_o = rays->rays_o; P.rays_d = rays->rays_d; P.viewdirs = rays->viewdirs; P.far = far; P.tvals = t;
+    P.rays_o = rays->rays_o; P.rays_d = rays->rays_d; P.far = far; P.tvals = t;
+    P.dir = static_cast<const uint4*>(dir);
     P.ray_order = rays->ray_order;
     P.n_rays = rays->n_rays; P.N = N; P.chunk = rays->chunk; P.nv = sc->dev.nv;
     P.sg = (N + kTileSamples - 1) / kTileSamples;

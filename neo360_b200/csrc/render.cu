@@ -10,6 +10,7 @@ namespace {
 struct WS {
     float *far, *t0[2], *w0[2], *t1[2], *w1[2], *sig[2], *rgb[2];
     float *c[2], *acc[2], *lam, *dep[2];
+    unsigned char* dir;      // NEO_PREC_TC: direction fragments of every ray (launch_dir_frags), shared by the four field launches
 };
 
 size_t carve(Carve& cv, int n, int N0, int N1, WS& w) {
@@ -26,6 +27,7 @@ size_t carve(Carve& cv, int n, int N0, int N1, WS& w) {
         w.dep[b] = cv.take<float>(n);
     }
     w.lam = cv.take<float>(n);
+    w.dir = cv.take<unsigned char>((size_t)n * kDirFragBytes);
     return cv.used;
 }
 
@@ -48,8 +50,8 @@ struct Prof {
     double field_points = 0;             // (ray, sample) points pushed through field kernels
 } g_prof;
 
-int field(const NeoScene* sc, const NeoRays* rays, const float* far, const float* t, int N, int mi, int prec, float* rgb,
-          float* sigma, cudaStream_t s) {
+int field(const NeoScene* sc, const NeoRays* rays, const float* far, const float* t, int N, int mi, int prec, const void* dir,
+          float* rgb, float* sigma, cudaStream_t s) {
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (g_prof.on) {
         if (g_prof.used == g_prof.pool.size()) {
@@ -64,7 +66,7 @@ int field(const NeoScene* sc, const NeoRays* rays, const float* far, const float
         NEO_CUDA(cudaEventRecord(e0, s));
     }
     int rc = (prec == NEO_PREC_FP32) ? launch_field_fp32(sc, rays, far, t, N, mi, rgb, sigma, s)
-                                     : launch_field_tc(sc, rays, far, t, N, mi, rgb, sigma, s);
+                                     : launch_field_tc(sc, rays, far, t, N, mi, dir, rgb, sigma, s);
     if (g_prof.on && e1) NEO_CUDA(cudaEventRecord(e1, s));
     g_prof.launches += 1;
     g_prof.field_points += (double)rays->n_rays * N;
@@ -96,6 +98,10 @@ extern "C" int neo_render_fwd(const NeoScene* sc, const NeoRays* rays, const Neo
 
     if ((rc = launch_far(rays->rays_o, rays->rays_d, n, w.far, sc->err_flag, s))) return rc;
     g_prof.launches += 1 + 2 * (2 + 2 + 1);      // far + per level: 2 sampling, 2 composite, 1 combine (field counted in field())
+    if (cfg->precision == NEO_PREC_TC) {
+        if ((rc = launch_dir_frags(sc, rays, w.dir, s))) return rc;
+        g_prof.launches += 1;
+    }
     const int white = cfg->out_depth ? 0 : cfg->white_bkgd;       // model.py:501,519 vs 551,560
     for (int lvl = 0; lvl < 2; ++lvl) {
         const int N = lvl ? N1 : N0;
@@ -109,7 +115,7 @@ extern "C" int neo_render_fwd(const NeoScene* sc, const NeoRays* rays, const Neo
             if ((rc = launch_resample(rays->rays_o, rays->rays_d, w.far, w.t0[1], w.w0[1], n, N0, cfg->n_fine, 0, 3.0f, cfg->u_bg1, t[1], nullptr, nullptr, s))) return rc;
         }
         for (int b = 0; b < 2; ++b)
-            if ((rc = field(sc, rays, w.far, t[b], N, 2 * lvl + b, cfg->precision, w.rgb[b], w.sig[b], s))) return rc;
+            if ((rc = field(sc, rays, w.far, t[b], N, 2 * lvl + b, cfg->precision, w.dir, w.rgb[b], w.sig[b], s))) return rc;
         if ((rc = launch_composite(w.rgb[0], w.sig[0], t[0], rays->rays_d, w.far, n, N, white, 1, w.c[0], w.acc[0], wt[0], w.lam, w.dep[0], s))) return rc;
         if ((rc = launch_composite(w.rgb[1], w.sig[1], t[1], rays->rays_d, w.far, n, N, white, 0, w.c[1], w.acc[1], wt[1], nullptr, w.dep[1], s))) return rc;
         if ((rc = launch_combine(n, N, w.c[0], w.c[1], w.lam, w.dep[0], w.dep[1], t[0], t[1], out->comp_rgb[lvl],
@@ -309,7 +315,27 @@ extern "C" int neo_index_local(const NeoScene* sc, const float* pts, int M, floa
 extern "C" int neo_field_eval(const NeoScene* sc, const NeoRays* rays, const float* far, const float* t, int N, int mlp_index,
                               int precision, float* rgb, float* sigma, void* stream) {
     if (!sc || !rays || mlp_index < 0 || mlp_index > 3 || N < 1) { set_error("neo_field_eval: bad arguments"); return NEO_ERR_INVALID; }
-    return field(sc, rays, far, t, N, mlp_index, precision, rgb, sigma, (cudaStream_t)stream);
+    cudaStream_t s = (cudaStream_t)stream;
+    if (precision == NEO_PREC_FP32) return field(sc, rays, far, t, N, mlp_index, precision, nullptr, rgb, sigma, s);
+    // no caller workspace here: the direction fragments go to a pool block, handed back once the stream has drained
+    if (rays->n_rays <= 0) { set_error("neo_field_eval: empty rays"); return NEO_ERR_INVALID; }
+    const size_t bytes = (size_t)rays->n_rays * kDirFragBytes;
+    void* dir = nullptr;
+    int rc = pool_alloc(&dir, bytes);
+    if (rc) return rc;
+    if (!(rc = launch_dir_frags(sc, rays, dir, s))) {
+        g_prof.launches += 1;
+        rc = field(sc, rays, far, t, N, mlp_index, precision, dir, rgb, sigma, s);
+    }
+    const cudaError_t e = cudaStreamSynchronize(s);
+    pool_release(dir, bytes);
+    if (rc) return rc;
+    NEO_CUDA(e);
+    return NEO_OK;
+}
+extern "C" int neo_tc_dir_fragments(const NeoScene* sc, const NeoRays* rays, void* out, void* stream) {
+    if (!sc || !rays || rays->n_rays <= 0) { set_error("neo_tc_dir_fragments: bad arguments"); return NEO_ERR_INVALID; }
+    return launch_dir_frags(sc, rays, out, (cudaStream_t)stream);
 }
 
 // ---- profiling / accounting (bench.py) ----

@@ -21,7 +21,8 @@ import tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-PHASES = ("tile setup", "camera + encodings", "tap table", "blend P0", "layers 0-2", "blend P3", "layer 3 + head", "colour head + stores")
+PHASES = ("tile setup", "camera + encodings", "tap table", "blend P0", "layers 0-2", "blend P3", "layer 3 + head", "direction term",
+          "colour head + stores")
 LAUNCHES = ("fg coarse", "bg coarse", "fg fine", "bg fine")      # order of the field launches of one frame (render.cu)
 MAX_LAUNCHES = 64
 
