@@ -10,7 +10,11 @@
 //     i.e. the cross-view means become one register accumulator summed over the views.
 //   * b0 and b3 ride on a constant-one column of the positional encoding; b1, b2 and the head biases seed the accumulators.
 //
-// Layout: one persistent CTA per SM, two warpgroups, each working on its own tiles of 64 points (16 rays x 4 consecutive samples).
+// Layout: one persistent CTA per SM, two warpgroups, each working on its own tiles of 64 points (32 rays x 2 consecutive samples).
+// The rays of a tile are 32 consecutive slots of the ray order (one 8x4 pixel block of a frame, renderer._blocked_order): rays that
+// close together read the same texels at a sample, while consecutive samples move on to the next texel, so a tile that spans more
+// rays and fewer samples reads fewer distinct texels per point (on H100 the field launches are 1.11x faster than with 16 rays x 4
+// samples, DESIGN.md §5).
 // Every weight matrix of the branch's MLP (trunk, folded head, colour head: up to 200 KB fp16, 128-byte-swizzled K-major tiles) is
 // copied into shared memory once per CTA by TMA bulk copies.  Per (tile, view) a warpgroup runs the whole MLP as wgmma.mma_async
 // m64nNk16 with the activations as REGISTER A fragments: the fp32 accumulator of one layer is rectified, packed to fp16 and fed to
@@ -29,8 +33,8 @@ namespace neo {
 namespace tc {
 using namespace hopper;
 
-constexpr int kTileRays = 16;
-constexpr int kTileSamples = 4;
+constexpr int kTileRays = 32;
+constexpr int kTileSamples = 2;
 constexpr int kTilePts = kTileRays * kTileSamples;  // = the M of one wgmma
 constexpr int kWarpgroups = 2;
 constexpr int kThreads = 128 * kWarpgroups;
