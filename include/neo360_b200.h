@@ -433,6 +433,25 @@ int neo_grid_encoder_pool(const float* lat, const float* logits, int nv, float* 
  * floating-point atomics (two calls give bit-identical results). */
 int neo_grid_encoder_pool_bwd(const float* lat, const float* logits, int nv, const float* g_xz, const float* g_xy, const float* g_yz,
                               float* d_lat, float* d_logits, void* stream);
+/* Tensor-core training form (GridEncoder.dense_train_tc): bf16 rows around the neo_tc_*_bf16 products.  Each returns NEO_ERR_INVALID
+ * before any launch on a NULL buffer, nv < 1, or a stride / alignment its kernel cannot address; the geometry rules are those above.
+ * neo_grid_encoder_features_bf16: the rows of neo_grid_encoder_features as bf16, each element the fp32 entry's value rounded once;
+ *   518 <= ldx <= 640, ldx % 8 == 0, X 16-byte aligned.
+ * neo_grid_encoder_coords_bf16: columns 512, 513, 514 of every row of L (nv*64^3, ld) = the cell's world x, y, z in bf16, columns
+ *   515..ld-1 = 0 (L = [lat | x y z | 0], the input of the aggregators' stacked first layer); 520 <= ld <= 640, ld % 8 == 0, 16-byte aligned.
+ * neo_grid_encoder_pool_bf16 / _pool_bwd_bf16: neo_grid_encoder_pool / _pool_bwd with lat the first 512 bf16 columns of rows of stride
+ *   ld >= 512 (pool: ld % 8 == 0 and lat 16-byte aligned); logits, the floor plans, d_lat (nv*64^3, 512) and d_logits stay fp32, with the
+ *   same fixed orders (two calls are bit-identical).
+ * neo_grid_encoder_lat_grad_bf16: d_lat (nv*64^3, 512) bf16 = bf16(d_pool + d_agg), both fp32 (nv*64^3, 512), inputs 16-byte and the
+ *   output 8-byte aligned. */
+int neo_grid_encoder_features_bf16(const float* latent_cl, int nv, int lat_h, int lat_w, int img_w, int img_h, const float* src_poses,
+                                   float focal, float cx, float cy, void* X, int ldx, void* stream);
+int neo_grid_encoder_coords_bf16(void* L, int nv, int ld, void* stream);
+int neo_grid_encoder_pool_bf16(const void* lat, long long ld, const float* logits, int nv, float* floor_xz, float* floor_xy, float* floor_yz,
+                               void* stream);
+int neo_grid_encoder_pool_bwd_bf16(const void* lat, long long ld, const float* logits, int nv, const float* g_xz, const float* g_xy,
+                                   const float* g_yz, float* d_lat, float* d_logits, void* stream);
+int neo_grid_encoder_lat_grad_bf16(const float* d_pool, const float* d_agg, int nv, void* d_lat, void* stream);
 
 /* ---- per-ray training losses and the encoder's upsampling adjoint, for training under torch.use_deterministic_algorithms (csrc/det.cu):
  * one warp per ray with fixed-order sums, every output written once, no floating-point atomics; two calls are bit-identical.  All return

@@ -152,6 +152,12 @@ SYMBOLS = {
     "neo_upsample_bilinear_bwd": (C.c_int, [C.c_void_p, C.c_longlong, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "neo_grid_encoder_pool": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 4),
     "neo_grid_encoder_pool_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int] + [C.c_void_p] * 6),
+    "neo_grid_encoder_features_bf16": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_float, C.c_float,
+                                                 C.c_float, C.c_void_p, C.c_int, C.c_void_p]),
+    "neo_grid_encoder_coords_bf16": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "neo_grid_encoder_pool_bf16": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_int] + [C.c_void_p] * 4),
+    "neo_grid_encoder_pool_bwd_bf16": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_int] + [C.c_void_p] * 6),
+    "neo_grid_encoder_lat_grad_bf16": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "neo_field_train_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
     "neo_field_train_fwd": (C.c_int, [C.c_void_p] * 3 + [C.c_int] * 3 + [C.c_void_p] * 10 + [C.c_size_t, C.c_void_p]),
     "neo_field_train_bwd": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 4 + [C.c_size_t] + [C.c_void_p] * 10 +

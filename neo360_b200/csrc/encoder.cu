@@ -6,11 +6,16 @@
 // 786 432 rows per scene at NV = 3: every dense layer runs on the tensor cores through gemm_f16 (csrc/gemm_tc.cu); the gather, the logit
 // reduction and the softmax-weighted pillar sum are the kernels below.  fp16 weights / activations, fp32 accumulation and softmax.
 // Training (GridEncoder.dense_train) uses the same gather and pillar-sum kernels in fp32, their backward kernels below, and the host
-// framework's GEMMs for the dense layers.
+// framework's GEMMs for the dense layers.  Its tensor-core form (GridEncoder.dense_train_tc) uses their bf16 instances around gemm_tc.cu's
+// bf16 products: lookup rows and the latent buffer L = [lat | x y z | 0] (coords_kernel) in bf16, the pillar sums and their backward
+// reading lat from L, and lat_grad_kernel joining the pool's and the aggregators' latent gradients.
 #include "common.cuh"
 #include <cuda_fp16.h>
+#include <cuda_bf16.h>
 
 namespace neo {
+template <> __device__ __forceinline__ __nv_bfloat16 from_f32<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+
 namespace enc {
 
 constexpr int kG = 64, kNC = kG * kG * kG, kLat = 512, kIn = 518, kLd = 576;      // 518 -> 576 (multiple of 64) zero padded
@@ -61,15 +66,30 @@ __device__ __forceinline__ void store4(__half* p, float4 a) {
     pk.x = *reinterpret_cast<uint32_t*>(&lo); pk.y = *reinterpret_cast<uint32_t*>(&hi);
     *reinterpret_cast<uint2*>(p) = pk;
 }
+__device__ __forceinline__ void store4(__nv_bfloat16* p, float4 a) {
+    __nv_bfloat162 lo = __floats2bfloat162_rn(a.x, a.y), hi = __floats2bfloat162_rn(a.z, a.w);
+    uint2 pk;
+    pk.x = *reinterpret_cast<uint32_t*>(&lo); pk.y = *reinterpret_cast<uint32_t*>(&hi);
+    *reinterpret_cast<uint2*>(p) = pk;
+}
 __device__ __forceinline__ float4 load4(const float* p) { return *reinterpret_cast<const float4*>(p); }
 __device__ __forceinline__ float4 load4(const __half* p) {
     const uint2 pk = *reinterpret_cast<const uint2*>(p);
     const float2 f0 = __half22float2(*reinterpret_cast<const __half2*>(&pk.x)), f1 = __half22float2(*reinterpret_cast<const __half2*>(&pk.y));
     return make_float4(f0.x, f0.y, f1.x, f1.y);
 }
+__device__ __forceinline__ float4 load4(const __nv_bfloat16* p) {
+    const uint2 pk = *reinterpret_cast<const uint2*>(p);
+    const float2 f0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&pk.x));
+    const float2 f1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&pk.y));
+    return make_float4(f0.x, f0.y, f1.x, f1.y);
+}
+__device__ __forceinline__ float to_f32(float v) { return v; }
+__device__ __forceinline__ float to_f32(__nv_bfloat16 v) { return __bfloat162float(v); }
 
 // one block (128 threads = 512 channels / 4) per (view, grid cell): row (stride ld, 518 <= ld <= 640) =
-// [latent lookup (512) | cam xyz (3) | direction (3) | 0 ...].  T = __half: the tensor-core eval path; T = float: the training path.
+// [latent lookup (512) | cam xyz (3) | direction (3) | 0 ...].  T = __half: the tensor-core eval path; T = float: the training path;
+// T = __nv_bfloat16: its tensor-core form (every element the fp32 instance's value rounded once).
 template <class T>
 __global__ void __launch_bounds__(128) grid_gather_kernel(const float* __restrict__ lat_cl, int lh, int lw, const float* __restrict__ poses,
                                                           float focal, float cx, float cy, float sx, float sy, T* __restrict__ X, int ld) {
@@ -147,6 +167,30 @@ __global__ void coord_col_kernel(__half* __restrict__ L, long long rows, int axi
     L[row * kLd + kLat + c] = __float2half_rn(val);
 }
 
+// columns 512, 513, 514 of every row (stride ld) = the world x, y, z of its cell in bf16, columns 515..ld-1 = 0: the coordinate inputs of
+// the three aggregators' stacked first layer (aggregator a reads column 512 + a)
+__global__ void coords_kernel(__nv_bfloat16* __restrict__ L, long long rows, int ld) {
+    const int w = ld - kLat;
+    const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (gid >= rows * w) return;
+    const long long row = gid / w;
+    const int c = (int)(gid % w);
+    float x[3];
+    cell_xyz((int)(row % kNC), x);
+    L[row * ld + kLat + c] = __float2bfloat16_rn(c == 0 ? x[0] : c == 1 ? x[1] : c == 2 ? x[2] : 0.f);
+}
+
+// d_lat (rows, 512) bf16 = bf16(d_pool + d_agg), both fp32 (rows, 512): the latent gradient of the tensor-core training form, rounded once
+__global__ void lat_grad_kernel(const float4* __restrict__ a, const float4* __restrict__ b, long long n4, uint2* __restrict__ out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n4) return;
+    const float4 x = a[i], y = b[i];
+    __nv_bfloat162 lo = __floats2bfloat162_rn(x.x + y.x, x.y + y.y), hi = __floats2bfloat162_rn(x.z + y.z, x.w + y.w);
+    uint2 pk;
+    pk.x = *reinterpret_cast<uint32_t*>(&lo); pk.y = *reinterpret_cast<uint32_t*>(&hi);
+    out[i] = pk;
+}
+
 // The 64 cells of pillar (p, q) along `axis` (plane dims = the two remaining grid axes in (x, y, z) order): cell i = base + i * stride.
 __device__ __forceinline__ void pillar_cells(int axis, int p, int q, int& base, int& stride) {
     stride = axis == 0 ? kG * kG : (axis == 1 ? kG : 1);
@@ -161,7 +205,8 @@ __device__ __forceinline__ void pillar_softmax(const float* wsm, float& mx, floa
 }
 
 // softmax of the 64 logits of a pillar along `axis` and the weighted sum of its latent rows (row stride ld): out (nv, 512, 64, 64) NCHW.
-// One block (128 threads x 4 channels) per pillar.  T = __half: the eval path's L; T = float: the training path's depth_fc output.
+// One block (128 threads x 4 channels) per pillar.  T = __half: the eval path's L; T = float: the training path's depth_fc output;
+// T = __nv_bfloat16: the latent columns of its tensor-core form's L.
 template <class T>
 __global__ void __launch_bounds__(128) pillar_sum_kernel(const T* __restrict__ L, int ld, const float* __restrict__ logits, int axis, float* __restrict__ out) {
     const int pillar = blockIdx.x % (kG * kG), v = blockIdx.x / (kG * kG);
@@ -212,7 +257,9 @@ __global__ void __launch_bounds__(64) pillar_softmax_bwd_kernel(const float* __r
 }
 
 // launch (2): 256 threads per xy pillar (v, ix, iy); channels in chunks of 32, lane = channel, warp w = rows iz = w, w + 8, ...
-__global__ void __launch_bounds__(256) pool_bwd_rows_kernel(const float* __restrict__ lat, const float* __restrict__ logits, const float* __restrict__ g_yz,
+// lat rows have stride ld (T = float: the fp32 training path, ld 512; T = __nv_bfloat16: its tensor-core form's L); d_lat has stride 512.
+template <class T>
+__global__ void __launch_bounds__(256) pool_bwd_rows_kernel(const T* __restrict__ lat, long long ld, const float* __restrict__ logits, const float* __restrict__ g_yz,
                                                             const float* __restrict__ g_xz, const float* __restrict__ g_xy, float* __restrict__ d_lat,
                                                             float* __restrict__ dl, long long R) {
     constexpr int kCh = 32, kRows = kG / 8;
@@ -254,7 +301,7 @@ __global__ void __launch_bounds__(256) pool_bwd_rows_kernel(const float* __restr
         for (int k = 0; k < kRows; ++k) {
             const int iz = warp + 8 * k;
             const size_t e = (r0 + iz) * kLat + c0 + lane;
-            const float x = lat[e], a0 = g0[lane][iz], a1 = g1[lane][iz], a2 = g2[lane];
+            const float x = to_f32(lat[(r0 + iz) * ld + c0 + lane]), a0 = g0[lane][iz], a1 = g1[lane][iz], a2 = g2[lane];
             d_lat[e] = (s[0][iz] * a0 + s[1][iz] * a1) + s[2][iz] * a2;
             acc[0][k] += a0 * x; acc[1][k] += a1 * x; acc[2][k] += a2 * x;
         }
@@ -477,9 +524,90 @@ extern "C" int neo_grid_encoder_pool_bwd(const float* lat, const float* logits, 
     const long long R = (long long)nv * kNC;
     pillar_softmax_bwd_kernel<<<dim3((unsigned)(nv * kG * kG), 2), kG, 0, s>>>(logits, d_logits, R, 0);
     NEO_LAUNCH_CHECK("pillar_softmax_bwd_kernel");
-    pool_bwd_rows_kernel<<<(unsigned)(nv * kG * kG), 256, 0, s>>>(lat, logits, g_yz, g_xz, g_xy, d_lat, d_logits, R);
+    pool_bwd_rows_kernel<float><<<(unsigned)(nv * kG * kG), 256, 0, s>>>(lat, kLat, logits, g_yz, g_xz, g_xy, d_lat, d_logits, R);
     NEO_LAUNCH_CHECK("pool_bwd_rows_kernel");
     pillar_softmax_bwd_kernel<<<dim3((unsigned)(nv * kG * kG), 2), kG, 0, s>>>(logits, d_logits, R, 1);
     NEO_LAUNCH_CHECK("pillar_softmax_bwd_kernel");
+    return NEO_OK;
+}
+
+// ---- tensor-core training form (bf16 rows; GridEncoder.dense_train_tc): same contracts as the fp32 entries above ----
+
+extern "C" int neo_grid_encoder_features_bf16(const float* latent_cl, int nv, int lat_h, int lat_w, int img_w, int img_h, const float* src_poses,
+                                              float focal, float cx, float cy, void* X, int ldx, void* stream) {
+    using namespace enc;
+    if (!enc_geometry_ok("neo_grid_encoder_features_bf16", nv, lat_h, lat_w, img_w, img_h, src_poses)) return NEO_ERR_INVALID;
+    if (!latent_cl || !X || ldx < kIn || ldx > kLat + 128 || ldx % 8 || !aligned(latent_cl, 16) || !aligned(X, 16)) {
+        set_error("neo_grid_encoder_features_bf16: NULL or unaligned buffer, or row stride %d outside [518, 640] or not a multiple of 8", ldx);
+        return NEO_ERR_INVALID;
+    }
+    float sx, sy;
+    lat_scale(lat_h, lat_w, img_w, img_h, sx, sy);
+    grid_gather_kernel<__nv_bfloat16><<<(unsigned)((long long)nv * kNC), 128, 0, (cudaStream_t)stream>>>(latent_cl, lat_h, lat_w, src_poses, focal,
+                                                                                                        cx, cy, sx, sy, (__nv_bfloat16*)X, ldx);
+    NEO_LAUNCH_CHECK("grid_gather_kernel<bf16>");
+    return NEO_OK;
+}
+
+extern "C" int neo_grid_encoder_coords_bf16(void* L, int nv, int ld, void* stream) {
+    using namespace enc;
+    if (!L || nv < 1 || ld < kLat + 3 || ld > kLat + 128 || ld % 8 || !aligned(L, 16)) {
+        set_error("neo_grid_encoder_coords_bf16: NULL or unaligned buffer, nv %d < 1, or row stride %d outside [520, 640] or not a multiple of 8",
+                  nv, ld);
+        return NEO_ERR_INVALID;
+    }
+    const long long rows = (long long)nv * kNC, n = rows * (ld - kLat);
+    coords_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>((__nv_bfloat16*)L, rows, ld);
+    NEO_LAUNCH_CHECK("coords_kernel");
+    return NEO_OK;
+}
+
+extern "C" int neo_grid_encoder_pool_bf16(const void* lat, long long ld, const float* logits, int nv, float* floor_xz, float* floor_xy,
+                                          float* floor_yz, void* stream) {
+    using namespace enc;
+    if (!lat || !logits || !floor_xz || !floor_xy || !floor_yz || nv < 1 || ld < kLat || ld % 8 || !aligned(lat, 16)) {
+        set_error("neo_grid_encoder_pool_bf16: bad arguments (NULL buffer, nv %d < 1, row stride %lld < 512 or not a multiple of 8, or lat not "
+                  "16-byte aligned)", nv, ld);
+        return NEO_ERR_INVALID;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    const long long R = (long long)nv * kNC;
+    float* outs[3] = {floor_yz, floor_xz, floor_xy};
+    for (int axis = 0; axis < 3; ++axis) {
+        pillar_sum_kernel<__nv_bfloat16><<<(unsigned)(nv * kG * kG), 128, 0, s>>>((const __nv_bfloat16*)lat, (int)ld, logits + axis * R, axis,
+                                                                                 outs[axis]);
+        NEO_LAUNCH_CHECK("pillar_sum_kernel<bf16>");
+    }
+    return NEO_OK;
+}
+
+extern "C" int neo_grid_encoder_pool_bwd_bf16(const void* lat, long long ld, const float* logits, int nv, const float* g_xz, const float* g_xy,
+                                              const float* g_yz, float* d_lat, float* d_logits, void* stream) {
+    using namespace enc;
+    if (!lat || !logits || !d_lat || !d_logits || nv < 1 || ld < kLat) {
+        set_error("neo_grid_encoder_pool_bwd_bf16: bad arguments (NULL buffer, nv %d < 1 or row stride %lld < 512)", nv, ld);
+        return NEO_ERR_INVALID;
+    }
+    cudaStream_t s = (cudaStream_t)stream;
+    const long long R = (long long)nv * kNC;
+    pillar_softmax_bwd_kernel<<<dim3((unsigned)(nv * kG * kG), 2), kG, 0, s>>>(logits, d_logits, R, 0);
+    NEO_LAUNCH_CHECK("pillar_softmax_bwd_kernel");
+    pool_bwd_rows_kernel<__nv_bfloat16><<<(unsigned)(nv * kG * kG), 256, 0, s>>>((const __nv_bfloat16*)lat, ld, logits, g_yz, g_xz, g_xy, d_lat,
+                                                                                d_logits, R);
+    NEO_LAUNCH_CHECK("pool_bwd_rows_kernel<bf16>");
+    pillar_softmax_bwd_kernel<<<dim3((unsigned)(nv * kG * kG), 2), kG, 0, s>>>(logits, d_logits, R, 1);
+    NEO_LAUNCH_CHECK("pillar_softmax_bwd_kernel");
+    return NEO_OK;
+}
+
+extern "C" int neo_grid_encoder_lat_grad_bf16(const float* d_pool, const float* d_agg, int nv, void* d_lat, void* stream) {
+    using namespace enc;
+    if (!d_pool || !d_agg || !d_lat || nv < 1 || !aligned(d_pool, 16) || !aligned(d_agg, 16) || !aligned(d_lat, 8)) {
+        set_error("neo_grid_encoder_lat_grad_bf16: bad arguments (NULL buffer, nv %d < 1, or inputs not 16-byte / output not 8-byte aligned)", nv);
+        return NEO_ERR_INVALID;
+    }
+    const long long n4 = (long long)nv * kNC * kLat / 4;
+    lat_grad_kernel<<<(unsigned)((n4 + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const float4*)d_pool, (const float4*)d_agg, n4, (uint2*)d_lat);
+    NEO_LAUNCH_CHECK("lat_grad_kernel");
     return NEO_OK;
 }

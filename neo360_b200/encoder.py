@@ -15,8 +15,10 @@
                                                                    grid lookup and the softmax pillar sums run forward and backward in
                                                                    hand-written fp32 CUDA (`neo_grid_encoder_features(_bwd)`,
                                                                    `neo_grid_encoder_pool(_bwd)`) and the dense layers as framework fp32
-                                                                   GEMMs; under autograd on the CPU the same algebra runs as framework ops
-                                                                   (`dense_torch`).
+                                                                   GEMMs; with `train_precision="tc"` the whole dense part trains on the
+                                                                   tensor cores instead (`dense_train_tc`: bf16 operands, fp32
+                                                                   accumulation, `_DenseTC`); under autograd on the CPU the same algebra
+                                                                   runs as framework ops (`dense_torch`).
 """
 from __future__ import annotations
 
@@ -29,6 +31,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib as L
+from .training import check_train_precision
 
 
 def _init_linear_kaiming(m):
@@ -170,22 +173,8 @@ class _Features(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, g_X):
-        lib = L.load()
         (pose_c,) = ctx.saved_tensors
-        nv, lh, lw, _, _ = ctx.geo
-        g = g_X.contiguous().float()
-        g_lat = torch.zeros(nv, lh, lw, 512, device=g.device)
-        with torch.cuda.device(g.device):
-            if ctx.det:                 # order-fixed scatter: bit-reproducible
-                need = lib.neo_grid_encoder_features_bwd_det_workspace_bytes(nv, lh, lw)
-                if need == 0:
-                    L.check(-1)
-                ws = torch.empty(need, dtype=torch.uint8, device=g.device)
-                L.check(lib.neo_grid_encoder_features_bwd_det(*ctx.geo, L.ptr(pose_c), *ctx.cam, L.ptr(g), g.stride(0), L.ptr(g_lat), L.ptr(ws),
-                                                              need, _stream()))
-            else:
-                L.check(lib.neo_grid_encoder_features_bwd(*ctx.geo, L.ptr(pose_c), *ctx.cam, L.ptr(g), g.stride(0), L.ptr(g_lat), _stream()))
-        return g_lat, None, None, None, None, None, None
+        return _lookup_bwd(L.load(), ctx, pose_c, g_X.contiguous().float()), None, None, None, None, None, None
 
 
 class _Pool(torch.autograd.Function):
@@ -215,11 +204,143 @@ class _Pool(torch.autograd.Function):
         return d_lat, d_logits
 
 
+class _DenseTC(torch.autograd.Function):
+    """The dense part of `GridEncoder.dense_train` on the tensor cores (csrc/encoder.cu, gemm_tc.cu, dense_train.cu: bf16 operands, fp32
+    accumulation, no floating-point atomics); oracle/encoder_train_tc_model.py states the formulation and its rounding points.
+    latent_cl (NV,Hl,Wl,512) channel-last, params = depth_fc's three (w, b), then per aggregator in axis order (yz, xz, xy) its
+    Linear(513, 512) w, b and Linear(512, 1) w, b -> floor plans xz, xy, yz (NV,512,G,G) fp32.  Activations live in bf16: the lookup rows
+    X (R, 576), h0, h1 (R, 512), L = [lat | x y z | 0] (R, 576) and the three aggregators' hidden layers side by side in A (R, 1536), the
+    output of one GEMM over L with their first layers stacked (row block a = aggregator a's 512 latent columns, its coordinate column at
+    column 512 + a, zeros elsewhere)."""
+
+    @staticmethod
+    def forward(ctx, latent_cl, poses, focal, cx, cy, W, H, *params):
+        lib = L.load()
+        lat = latent_cl.detach().contiguous().float()
+        nv, lh, lw, _ = lat.shape
+        dev, s = lat.device, _stream()
+        pose_c = poses.detach().contiguous().float()
+        R = nv * GridEncoder.GRID ** 3
+        P = [t.detach().contiguous().float() for t in params]
+        w, b = P[0:6:2], P[1:6:2]
+        u, c, q, e = P[6::4], P[7::4], P[8::4], P[9::4]
+        bf = lambda *shape: torch.empty(*shape, dtype=torch.bfloat16, device=dev)
+        U = torch.zeros(1536, 576, device=dev)                  # the stacked first layers (fp32 master values)
+        for a in range(3):
+            U[512 * a:512 * (a + 1), :512] = u[a][:, :512]
+            U[512 * a:512 * (a + 1), 512 + a] = u[a][:, 512]
+        cs = torch.cat(c)
+        X, H0, H1, Lb, A = bf(R, 576), bf(R, 512), bf(R, 512), bf(R, 576), bf(R, 1536)
+        Wp = [bf(512, 576), bf(512, 512), bf(512, 512)]
+        Up = bf(1536, 576)
+        WT = [bf(512, 512) for _ in range(3)]                   # W_i^T (W_0: its 512 lookup columns), the data gradients' operands
+        UT = bf(512, 1536)                                      # U[:, :512]^T
+        logits = torch.empty(3, R, device=dev)
+        out = [torch.empty(nv, 512, GridEncoder.GRID, GridEncoder.GRID, device=dev) for _ in range(3)]
+        geo, cam = (nv, lh, lw, int(W), int(H)), (focal, cx, cy)
+        gemm = lambda a_, lda, w_, ldw, bias, c_, ldc, N, K, epi: L.check(lib.neo_tc_gemm_bf16(a_, lda, w_, ldw, L.ptr(bias), c_, ldc, R, N, K,
+                                                                                               epi, s))
+        with torch.cuda.device(dev):
+            for i, wi in enumerate(w):
+                L.check(lib.neo_tc_pack_bf16(L.ptr(wi), 512, wi.shape[1], wi.shape[1], Wp[i].data_ptr(), Wp[i].shape[1], Wp[i].shape[1], 0, s))
+                L.check(lib.neo_tc_pack_bf16(L.ptr(wi), 512, wi.shape[1], wi.shape[1], WT[i].data_ptr(), 512, 512, 1, s))
+            L.check(lib.neo_tc_pack_bf16(L.ptr(U), 1536, 576, 576, Up.data_ptr(), 576, 576, 0, s))
+            L.check(lib.neo_tc_pack_bf16(L.ptr(U), 1536, 576, 576, UT.data_ptr(), 512, 1536, 1, s))
+            L.check(lib.neo_grid_encoder_features_bf16(L.ptr(lat), *geo, L.ptr(pose_c), *cam, X.data_ptr(), 576, s))
+            gemm(X.data_ptr(), 576, Wp[0].data_ptr(), 576, b[0], H0.data_ptr(), 512, 512, 576, 0)
+            gemm(H0.data_ptr(), 512, Wp[1].data_ptr(), 512, b[1], H1.data_ptr(), 512, 512, 512, 0)
+            gemm(H1.data_ptr(), 512, Wp[2].data_ptr(), 512, b[2], Lb.data_ptr(), 576, 512, 512, 1)
+            L.check(lib.neo_grid_encoder_coords_bf16(Lb.data_ptr(), nv, 576, s))
+            gemm(Lb.data_ptr(), 576, Up.data_ptr(), 576, cs, A.data_ptr(), 1536, 1536, 576, 0)
+            for a in range(3):
+                L.check(lib.neo_tc_rowdot_bf16(A.data_ptr() + 1024 * a, 1536, 512, L.ptr(q[a]), L.ptr(e[a]), 1, R, logits[a].data_ptr(), s))
+            L.check(lib.neo_grid_encoder_pool_bf16(Lb.data_ptr(), 576, L.ptr(logits), nv, *[t.data_ptr() for t in out], s))
+        ctx.save_for_backward(X, H0, H1, Lb, A, logits, *WT, UT, pose_c, *q)
+        ctx.geo, ctx.cam = geo, cam
+        ctx.det = torch.are_deterministic_algorithms_enabled()
+        return tuple(out)
+
+    @staticmethod
+    def backward(ctx, g_xz, g_xy, g_yz):
+        lib = L.load()
+        X, H0, H1, Lb, A, logits, *rest = ctx.saved_tensors
+        WT, UT, pose_c, q = rest[0:3], rest[3], rest[4], rest[5:8]
+        nv, lh, lw, _, _ = ctx.geo
+        R, dev, s = X.shape[0], X.device, _stream()
+        bf = lambda *shape: torch.empty(*shape, dtype=torch.bfloat16, device=dev)
+        gs = [None if g is None else g.contiguous().float() for g in (g_xz, g_xy, g_yz)]
+        need = max(lib.neo_tc_wgrad_bf16_workspace_bytes(*c) for c in ((R, 64, 512), (R, 1536, 576), (R, 512, 512), (R, 512, 576)))
+        if need == 0:
+            L.check(-1)
+        ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        wg = lambda dy, ldy, x, ldx, N, K, dw, kv, db: L.check(lib.neo_tc_wgrad_bf16(dy, ldy, x, ldx, R, N, K, L.ptr(dw), kv, L.ptr(db),
+                                                                                     ws.data_ptr(), need, s))
+        d_pool, d_lg = torch.empty(R, 512, device=dev), torch.empty(3, R, device=dev)
+        dA, g1 = bf(R, 1536), bf(R, 64)
+        agg = []
+        with torch.cuda.device(dev):
+            L.check(lib.neo_grid_encoder_pool_bwd_bf16(Lb.data_ptr(), 576, L.ptr(logits), nv, *[L.ptr(g) for g in gs], L.ptr(d_pool),
+                                                       L.ptr(d_lg), s))
+            for a in range(3):
+                L.check(lib.neo_tc_relu_rank1_bf16(L.ptr(d_lg[a]), L.ptr(q[a]), A.data_ptr() + 1024 * a, 1536, R, 512, dA.data_ptr() + 1024 * a,
+                                                   1536, s))
+                L.check(lib.neo_tc_pack_bf16(L.ptr(d_lg[a]), R, 1, 1, g1.data_ptr(), 64, 64, 0, s))
+                gq = torch.empty(64, 512, device=dev)
+                wg(g1.data_ptr(), 64, A.data_ptr() + 1024 * a, 1536, 64, 512, gq, 512, None)
+                agg.append((gq[:1].clone(), d_lg[a].sum().reshape(1)))
+            gU, gc = torch.empty(1536, 515, device=dev), torch.empty(1536, device=dev)
+            wg(dA.data_ptr(), 1536, Lb.data_ptr(), 576, 1536, 576, gU, 515, gc)
+            d_agg = torch.empty(R, 512, device=dev)
+            L.check(lib.neo_tc_gemm_bf16(dA.data_ptr(), 1536, UT.data_ptr(), 1536, None, d_agg.data_ptr(), 512, R, 512, 1536, 2, s))
+            del dA
+            G = [bf(R, 512), bf(R, 512)]
+            L.check(lib.neo_grid_encoder_lat_grad_bf16(L.ptr(d_pool), L.ptr(d_agg), nv, G[0].data_ptr(), s))
+            del d_pool, d_agg
+            grads = [None] * 6
+            for i, x, ldx in ((2, H1, 512), (1, H0, 512), (0, X, 576)):
+                gw, gb = torch.empty(512, 518 if i == 0 else 512, device=dev), torch.empty(512, device=dev)
+                wg(G[0].data_ptr(), 512, x.data_ptr(), ldx, 512, ldx, gw, gw.shape[1], gb)
+                grads[2 * i], grads[2 * i + 1] = gw, gb
+                if i > 0:
+                    L.check(lib.neo_tc_dgrad_bf16(G[0].data_ptr(), 512, WT[i].data_ptr(), 512, x.data_ptr(), 512, None, None, G[1].data_ptr(), 512,
+                                                  R, 512, 512, s))
+                    G.reverse()
+            g_lat = None
+            if ctx.needs_input_grad[0]:
+                g_X = torch.empty(R, 512, device=dev)
+                L.check(lib.neo_tc_gemm_bf16(G[0].data_ptr(), 512, WT[0].data_ptr(), 512, None, g_X.data_ptr(), 512, R, 512, 512, 2, s))
+                g_lat = _lookup_bwd(lib, ctx, pose_c, g_X)
+        for a in range(3):
+            rows = slice(512 * a, 512 * (a + 1))
+            grads += [torch.cat([gU[rows, :512], gU[rows, 512 + a:513 + a]], 1), gc[rows].clone(), *agg[a]]
+        return (g_lat, None, None, None, None, None, None, *grads)
+
+
+def _lookup_bwd(lib, ctx, pose_c, g):
+    """Latent gradient (NV,Hl,Wl,512) of the lookup rows' 512 lookup columns g (R, ld) fp32: the order-fixed scatter under
+    torch.use_deterministic_algorithms (ctx.det, recorded in the forward), the atomic one otherwise."""
+    nv, lh, lw, _, _ = ctx.geo
+    g_lat = torch.zeros(nv, lh, lw, 512, device=g.device)
+    with torch.cuda.device(g.device):
+        if ctx.det:                 # order-fixed scatter: bit-reproducible
+            need = lib.neo_grid_encoder_features_bwd_det_workspace_bytes(nv, lh, lw)
+            if need == 0:
+                L.check(-1)
+            ws = torch.empty(need, dtype=torch.uint8, device=g.device)
+            L.check(lib.neo_grid_encoder_features_bwd_det(*ctx.geo, L.ptr(pose_c), *ctx.cam, L.ptr(g), g.stride(0), L.ptr(g_lat), L.ptr(ws),
+                                                          need, _stream()))
+        else:
+            L.check(lib.neo_grid_encoder_features_bwd(*ctx.geo, L.ptr(pose_c), *ctx.cam, L.ptr(g), g.stride(0), L.ptr(g_lat), _stream()))
+    return g_lat
+
+
 class GridEncoder(nn.Module):
     GRID = 64
 
-    def __init__(self, encoder_type="resnet", **unused):
+    def __init__(self, encoder_type="resnet", train_precision="fp32", **unused):
         super().__init__()
+        # "fp32": the dense part trains through framework fp32 GEMMs (dense_train); "tc": on the tensor cores (dense_train_tc)
+        self.train_precision = train_precision
         if encoder_type != "resnet":
             raise NotImplementedError("reference default only (encoder_type='resnet')")
         self.grid_size = [self.GRID] * 3
@@ -233,6 +354,14 @@ class GridEncoder(nn.Module):
                   self.pillar_aggregator_xz, self.pillar_aggregator_yz, self.pillar_aggregator_xy):
             m.apply(_init_linear_kaiming)
         self._ws = None
+
+    @property
+    def train_precision(self) -> str:
+        return self._train_precision
+
+    @train_precision.setter
+    def train_precision(self, p: str):
+        self._train_precision = check_train_precision(p)
 
     # ---- the dense part, framework ops (autograd; also the fp32 reference of the CUDA path in the tests) ----
     def dense_torch(self, latent, poses, focal, c, W, H):
@@ -287,6 +416,19 @@ class GridEncoder(nn.Module):
             logits.append(lin(agg[2], torch.relu_(a)).reshape(-1))
         return _Pool.apply(lat, torch.stack(logits))
 
+    # ---- the dense part for training on the tensor cores: bf16 products, hand-written lookup and pillar sums (forward and backward) ----
+    def dense_train_tc(self, latent, poses, focal, c, W, H):
+        """`dense_train` with every dense layer on the tensor cores (`_DenseTC`), differentiable with respect to `latent` and every
+        parameter of depth_fc and the three aggregators."""
+        if not latent.is_cuda:
+            raise RuntimeError("neo360_b200 needs CUDA tensors (no CPU fallback)")
+        fc = self.depth_fc
+        params = [t for m in (fc.common_branch[0], fc.common_branch[2], fc.depth_encoder) for t in (m.weight, m.bias)]
+        for name in ("yz", "xz", "xy"):
+            agg = getattr(self, f"pillar_aggregator_{name}")
+            params += [agg[0].weight, agg[0].bias, agg[2].weight, agg[2].bias]
+        return _DenseTC.apply(latent.permute(0, 2, 3, 1), poses, float(focal[0]), float(c[0, 0]), float(c[0, 1]), int(W), int(H), *params)
+
     # ---- the dense part, hand-written CUDA (wgmma) ----
     def dense_cuda(self, latent, poses, focal, c, W, H):
         if not latent.is_cuda:
@@ -323,7 +465,10 @@ class GridEncoder(nn.Module):
         trained = [self.depth_fc, self.pillar_aggregator_xz, self.pillar_aggregator_yz, self.pillar_aggregator_xy]
         needs_grad = torch.is_grad_enabled() and (latent.requires_grad or any(q.requires_grad for m in trained for q in m.parameters()))
         if needs_grad:
-            dense = self.dense_train if latent.is_cuda else self.dense_torch
+            if not latent.is_cuda:
+                dense = self.dense_torch
+            else:
+                dense = self.dense_train_tc if self.train_precision == "tc" else self.dense_train
             fxz, fxy, fyz = dense(latent, poses.float(), focal.float(), c.float(), W, H)
         else:
             fxz, fxy, fyz = self.dense_cuda(latent, poses, focal, c, W, H)

@@ -1,6 +1,9 @@
 """GridEncoder training throughput on one GPU at the NeO-360 training shape: NV = 3 source views of 640 x 480 (latent 240 x 320),
-the 64^3 grid, a fixed random loss on the three output planes.  The CUDA form (`dense_train`: hand-written lookup and softmax pillar sums
-forward and backward, framework GEMMs) and the framework form (`dense_torch`) alternate in the same run, in fp32 and with TF32 GEMMs.
+the 64^3 grid, a fixed random loss on the three output planes.  Variants, alternated in the same run:
+  * cuda_fp32 / cuda_tf32 / cuda_autocast: the CUDA form (`dense_train`: hand-written lookup and softmax pillar sums forward and backward,
+    framework GEMMs) with fp32 GEMMs, TF32 GEMMs, and under torch.autocast(bfloat16);
+  * tc: the tensor-core form (`dense_train_tc`, `GridEncoder(train_precision="tc")`: every dense layer a bf16 product of csrc/gemm_tc.cu);
+  * torch_fp32 / torch_tf32: the framework form (`dense_torch`).
 
 Per form and precision it reports, from CUDA events after warm-up:
   * the dense part's forward + backward (latent -> three floor plans; the ResNet and the conv stacks excluded) and the whole
@@ -63,42 +66,49 @@ def main():
     w_out = [torch.randn(NV, 128, 120, 160, generator=gen).to(dev) for _ in range(3)]
     with torch.no_grad():
         latent0 = enc.spatial_encoder(imgs).detach()
-    forms = {"cuda": enc.dense_train, "torch": enc.dense_torch}
+    # variant -> (dense-part method, TF32 GEMMs, autocast)
+    variants = {"cuda_fp32": (enc.dense_train, False, False), "cuda_tf32": (enc.dense_train, True, False),
+                "cuda_autocast": (enc.dense_train, False, True), "tc": (enc.dense_train_tc, False, False),
+                "torch_fp32": (enc.dense_torch, False, False), "torch_tf32": (enc.dense_torch, True, False)}
 
-    def dense_step(form):
+    def dense_step(v):
+        form, _, ac = variants[v]
         lat = latent0.clone().requires_grad_(True)
-        planes = forms[form](lat, poses, focal, c, W, H)
-        sum((p * w).sum() for p, w in zip(planes, w_dense)).backward()
+        with torch.autocast("cuda", dtype=torch.bfloat16, enabled=ac):
+            planes = form(lat, poses, focal, c, W, H)
+        sum((p.float() * w).sum() for p, w in zip(planes, w_dense)).backward()
 
-    def encoder_step(form):
-        enc.dense_train = forms[form]
+    def encoder_step(v):
+        form, _, ac = variants[v]
+        enc.dense_train = form                              # forward() routes the dense part through this instance attribute
         enc.zero_grad(set_to_none=True)
-        out = enc(imgs, poses, focal, c)
-        sum((o * w).sum() for o, w in zip(out, w_out)).backward()
+        with torch.autocast("cuda", dtype=torch.bfloat16, enabled=ac):
+            out = enc(imgs, poses, focal, c)
+        sum((o.float() * w).sum() for o, w in zip(out, w_out)).backward()
         del enc.dense_train
 
     res = {}
+    r = {v: {"dense_ms": [], "encoder_ms": [], "peak_gb": 0.0} for v in variants}
+    for _ in range(2):                                      # alternate the variants twice, keep the better time of each
+        for v in variants:
+            torch.backends.cuda.matmul.allow_tf32 = torch.backends.cudnn.allow_tf32 = variants[v][1]
+            r[v]["dense_ms"].append(events(lambda: dense_step(v), args.steps, args.warmup))
+            enc.zero_grad(set_to_none=True)
+            torch.cuda.empty_cache()
+            torch.cuda.reset_peak_memory_stats(dev)
+            r[v]["encoder_ms"].append(events(lambda: encoder_step(v), args.steps, args.warmup))
+            r[v]["peak_gb"] = max(r[v]["peak_gb"], torch.cuda.max_memory_allocated(dev) / 1e9)
+            enc.zero_grad(set_to_none=True)
+            torch.cuda.empty_cache()
+    for v in variants:
+        d, e = min(r[v]["dense_ms"]), min(r[v]["encoder_ms"])
+        res[v] = {"dense_fwd_bwd_ms": round(d, 2), "encoder_fwd_bwd_ms": round(e, 2), "peak_mem_gb": round(r[v]["peak_gb"], 2),
+                  "dense_whole_step_tflops": round(STEP_FLOP / (d * 1e-3) / 1e12, 1),
+                  "dense_ms_runs": [round(x, 2) for x in r[v]["dense_ms"]], "encoder_ms_runs": [round(x, 2) for x in r[v]["encoder_ms"]]}
+    for base in ("cuda_fp32", "cuda_tf32", "cuda_autocast"):
+        res[f"tc_speedup_dense_vs_{base}"] = round(min(r[base]["dense_ms"]) / min(r["tc"]["dense_ms"]), 2)
     for prec in ("fp32", "tf32"):
-        torch.backends.cuda.matmul.allow_tf32 = prec == "tf32"
-        torch.backends.cudnn.allow_tf32 = prec == "tf32"
-        r = {f: {"dense_ms": [], "encoder_ms": [], "peak_gb": 0.0} for f in forms}
-        for _ in range(2):                                  # alternate the two forms twice, keep the better time of each
-            for f in forms:
-                r[f]["dense_ms"].append(events(lambda: dense_step(f), args.steps, args.warmup))
-                enc.zero_grad(set_to_none=True)
-                torch.cuda.empty_cache()
-                torch.cuda.reset_peak_memory_stats(dev)
-                r[f]["encoder_ms"].append(events(lambda: encoder_step(f), args.steps, args.warmup))
-                r[f]["peak_gb"] = max(r[f]["peak_gb"], torch.cuda.max_memory_allocated(dev) / 1e9)
-                enc.zero_grad(set_to_none=True)
-                torch.cuda.empty_cache()
-        for f in forms:
-            d, e = min(r[f]["dense_ms"]), min(r[f]["encoder_ms"])
-            res[f"{prec}_{f}"] = {"dense_fwd_bwd_ms": round(d, 2), "encoder_fwd_bwd_ms": round(e, 2), "peak_mem_gb": round(r[f]["peak_gb"], 2),
-                                  "dense_whole_step_tflops": round(STEP_FLOP / (d * 1e-3) / 1e12, 1),
-                                  "dense_ms_runs": [round(x, 2) for x in r[f]["dense_ms"]], "encoder_ms_runs": [round(x, 2) for x in r[f]["encoder_ms"]]}
-        res[f"{prec}_speedup_dense"] = round(min(r["torch"]["dense_ms"]) / min(r["cuda"]["dense_ms"]), 2)
-        res[f"{prec}_speedup_encoder"] = round(min(r["torch"]["encoder_ms"]) / min(r["cuda"]["encoder_ms"]), 2)
+        res[f"{prec}_speedup_dense"] = round(min(r[f"torch_{prec}"]["dense_ms"]) / min(r[f"cuda_{prec}"]["dense_ms"]), 2)
     print(json.dumps({"metric": "GridEncoder forward + backward, NV = 3, 640x480, 64^3 grid", "card": name, "power_limit_w": power,
                       "dense_step_flop": STEP_FLOP, "steps": args.steps, "warmup": args.warmup, **res}))
 

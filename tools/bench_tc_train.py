@@ -1,7 +1,8 @@
 """NeO-360 training step (BASELINE configs[3]: 4096 rays, 128 + 64 samples, 3 source views) with the MLPs in four arithmetics, alternated
 in one process: "fp32" (framework GEMMs, fp32), "tf32" (the same with TF32 GEMMs), "autocast" (the framework MLP under
 torch.autocast(bfloat16)) and "tc" (train_precision="tc": csrc/field_train.cu).  The encoder is frozen (its outputs are leaf tensors) or,
-with --encoder, runs inside the step.  Reports ms per step (CUDA events around whole steps, after a device synchronise), the share of it
+with --encoder, runs inside the step; there a fifth variant, "tc_enc", trains both the MLPs and the encoder's dense part on the tensor
+cores (`GridEncoder(train_precision="tc")`, csrc/encoder.cu around the bf16 products of csrc/gemm_tc.cu).  Reports ms per step (CUDA events around whole steps, after a device synchronise), the share of it
 spent in the MLP forward (CUDA events around the MLP calls of the forward pass), peak device memory, and the GPU it ran on.
 Writes one JSON line to stdout and, with --out, to that file."""
 import argparse
@@ -22,7 +23,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--rays", type=int, default=4096)
     ap.add_argument("--encoder", action="store_true")
-    ap.add_argument("--variants", default="fp32,tf32,autocast,tc")
+    ap.add_argument("--variants", default=None, help="default: fp32,tf32,autocast,tc, and tc_enc with --encoder")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     from neo360_b200 import NeRF_TP, batches, synth, training
@@ -51,9 +52,9 @@ def main():
 
     def make(variant):
         torch.manual_seed(0)
-        enc = GridEncoder() if a.encoder else None
+        enc = GridEncoder(train_precision="tc" if variant == "tc_enc" else "fp32") if a.encoder else None
         net = NeRF_TP(num_coarse_samples=128, num_fine_samples=64, num_src_views=3, precision="fp32", encoder=enc,
-                      train_precision="tc" if variant == "tc" else "fp32")
+                      train_precision="tc" if variant in ("tc", "tc_enc") else "fp32")
         sd = net.state_dict()
         sd.update(synth.make_mlp_params(0))
         net.load_state_dict(sd)
@@ -80,7 +81,7 @@ def main():
         opt.step()
         return loss
 
-    variants = a.variants.split(",")
+    variants = (a.variants or "fp32,tf32,autocast,tc" + (",tc_enc" if a.encoder else "")).split(",")
     res = {v: {"ms": [], "mlp_fwd_ms": [], "peak_gb": 0.0, "loss": None} for v in variants}
     for rnd in range(a.rounds):
         for v in variants:
