@@ -327,6 +327,58 @@ int neo_vanilla_composite_bwd(const float* rgb, const float* sigma, const float*
                               const float* g_comp_rgb, const float* g_acc, const float* g_weights, const float* g_depth, float* d_rgb,
                               float* d_sigma, void* stream);
 
+/* ---- PixelNeRF (SURVEY.md section 2 row 11): models/vanilla_nerf/model_pixel.py:35-258, csrc/pixelnerf.cu ----
+ * Sampling, lookup backward and compositing are the stages above: neo_vanilla_sample_along_rays and neo_sample_pdf (t only, so rays_d
+ * may be passed as the direction), neo_index_maps / neo_index_maps_bwd(_det) on the caller's channel-last latent, and
+ * neo_volumetric_rendering mode 2 / neo_vanilla_composite_bwd on the activated rgb and sigma.
+ * `scene` below is a cameras-only NeoScene (precision_mask 0) built from the source poses with column 1 of each rotation negated
+ * (camera y flipped) and the image size of src_imgs: with it the shared projection gives PixelNeRF's pixel coordinates exactly, for
+ * these entry points and for neo_index_maps*.  One NeRFMLP: nn.Linear layers with the weights TRANSPOSED to (in, out), row-major,
+ * 16-byte aligned. */
+typedef struct {
+    const float* wt[4];         /* pts_linears.{0..3}.weight^T: (575,128) (128,128)x3 */
+    const float* b[4];
+    const float *wbt, *bb;      /* bottleneck_layer^T (128,128) */
+    const float *wsig, *bsig;   /* density_layer (1,128), not transposed */
+    const float *wv0t, *bv0;    /* views_linear.0^T (155,128) */
+    const float *wv1t, *bv1;    /* views_linear.1^T (128,128) */
+    const float *wrgb, *brgb;   /* rgb_layer (3,128), not transposed */
+} NeoPixelMLPParams;
+/* The field of one level, fp32 CUDA cores in the reference formulation: for t_vals (n_rays, N) the points o + t rays_d, per source view
+ * the camera transform, the view-0 projection, the bilinear lookup of latent_cl (nv, lat_h, lat_w, 512; zeros padding), the encodings
+ * of the camera-frame point (63) and of the camera-frame view direction (27; row b*N+s of a chunk of rays->chunk rays, <= 0 = all, is
+ * conditioned on ray ((b*N+s) mod B) of its chunk, quirk Q1), the 4x128 trunk, the per-view bottleneck, the view means, and
+ * rgb = sigmoid, sigma = relu -> rgb (n_rays, N, 3), sigma (n_rays, N).  1..8 views. */
+int neo_pixelnerf_field(const NeoScene* scene, const float* latent_cl, const NeoPixelMLPParams* mlp, const NeoRays* rays,
+                        const float* t_vals, int N, float* rgb, float* sigma, void* stream);
+/* The training path's inputs of one level, the field kernel's arithmetic: enc (nv*M, 63), dir_tile (nv*M, 27) with rows ordered
+ * (view, point), M = n_rays*N, and pts (M,3) = o + t rays_d (or NULL), the world points neo_index_maps looks up. */
+int neo_pixelnerf_encode(const NeoScene* scene, const NeoRays* rays, const float* t_vals, int N, float* enc, float* dir_tile,
+                         float* pts, void* stream);
+
+/* NEO_PREC_TC form of neo_pixelnerf_field: the same layers in the reference formulation on the tensor-core dense layer (gemm_f16: fp16
+ * operands, fp32 accumulation).  Per pass of up to 65536 points: fp16 rows [enc 63 | latent 512 | 0] (nv*M, 576); the trunk, fp16 after
+ * each bias + ReLU; the bottleneck (fp16, no ReLU) beside the fp16 direction encoding in rows [bottleneck | dir 27 | 0] (192); the view
+ * mean of h3 (fp32 sum, fp16) times density_layer (fp32, rowdot); views_linear.0 (fp16), its view mean + ReLU (fp16); views_linear.1
+ * (fp16 after ReLU); rgb_layer (fp32, rowdot); sigma = relu, rgb = sigmoid.  Weights fp16 nn.Linear layout (out, in) with the input
+ * width zero-padded: pts_linears.0 (128, 576), views_linear.0 (128, 192), the rest (128, 128); 16-byte aligned.  Workspace:
+ * neo_pixelnerf_tc_workspace_bytes(nv, n_rays*N) bytes, 256-byte aligned (0 = invalid sizes). */
+typedef struct {
+    const void* w16[4];         /* pts_linears.{0..3}.weight fp16 */
+    const float* b[4];
+    const void* wb16;           /* bottleneck_layer fp16 (128,128) */
+    const float* bb;
+    const float *wsig, *bsig;   /* density_layer fp32 (1,128) */
+    const void* wv016;          /* views_linear.0 fp16 (128,192) */
+    const float* bv0;
+    const void* wv116;          /* views_linear.1 fp16 (128,128) */
+    const float* bv1;
+    const float *wrgb, *brgb;   /* rgb_layer fp32 (3,128) */
+} NeoPixelTCParams;
+size_t neo_pixelnerf_tc_workspace_bytes(int nv, long long M);
+int neo_pixelnerf_field_tc(const NeoScene* scene, const float* latent_cl, const NeoPixelTCParams* mlp, const NeoRays* rays,
+                           const float* t_vals, int N, float* rgb, float* sigma, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- Mip-NeRF 360 (SURVEY.md section 8(a) row a18): models/mipnerf360/model.py:30-365 ---- */
 typedef struct {
     int depth, width;          /* PropMLP: 4 x 256 (density only), NeRFMLP: 8 x 1024 (model.py:176-195) */

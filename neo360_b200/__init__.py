@@ -2,7 +2,7 @@
 `model(rays, randomized, white_bkgd, near, far, out_depth)` call surface.  See DESIGN.md / INTEGRATION.md."""
 from . import synth  # noqa: F401
 
-__all__ = ["NeRF_TP", "NeRFPPMLP", "ops", "synth", "release_cached"]
+__all__ = ["NeRF_TP", "NeRFPPMLP", "PixelNeRF", "ops", "synth", "release_cached"]
 
 
 def release_cached() -> None:
@@ -15,6 +15,9 @@ def __getattr__(name):
     if name in ("NeRF_TP", "NeRFPPMLP"):
         from . import renderer
         return getattr(renderer, name)
+    if name == "PixelNeRF":
+        from . import pixelnerf
+        return pixelnerf.PixelNeRF
     if name == "ops":
         import importlib
         return importlib.import_module(".ops", __name__)

@@ -50,6 +50,16 @@ class NeoVanillaMLPParams(C.Structure):
     _fields_ = [("w", C.c_void_p * 8), ("b", C.c_void_p * 8)] + [(n, C.c_void_p) for n in ("wb", "bb", "wsig", "bsig", "wv0", "bv0", "wrgb", "brgb")]
 
 
+class NeoPixelMLPParams(C.Structure):
+    _fields_ = [("wt", C.c_void_p * 4), ("b", C.c_void_p * 4)] + [(n, C.c_void_p) for n in ("wbt", "bb", "wsig", "bsig", "wv0t", "bv0", "wv1t",
+                                                                                            "bv1", "wrgb", "brgb")]
+
+
+class NeoPixelTCParams(C.Structure):
+    _fields_ = [("w16", C.c_void_p * 4), ("b", C.c_void_p * 4)] + [(n, C.c_void_p) for n in ("wb16", "bb", "wsig", "bsig", "wv016", "bv0",
+                                                                                              "wv116", "bv1", "wrgb", "brgb")]
+
+
 class NeoVanillaCfg(C.Structure):
     _fields_ = [("n_coarse", C.c_int), ("n_fine", C.c_int), ("white_bkgd", C.c_int), ("near_plane", C.c_float), ("far_plane", C.c_float),
                 ("u0", C.c_void_p), ("u1", C.c_void_p), ("precision", C.c_int)]
@@ -126,6 +136,12 @@ SYMBOLS = {
     "neo_vanilla_render_fwd": (C.c_int, [C.c_void_p, C.POINTER(NeoRays), C.POINTER(NeoVanillaCfg), C.POINTER(NeoVanillaOut), C.c_void_p, C.c_size_t, C.c_void_p]),
     "neo_vanilla_sample_along_rays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_vanilla_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "neo_pixelnerf_field": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(NeoPixelMLPParams), C.POINTER(NeoRays), C.c_void_p, C.c_int, C.c_void_p,
+                                      C.c_void_p, C.c_void_p]),
+    "neo_pixelnerf_tc_workspace_bytes": (C.c_size_t, [C.c_int, C.c_longlong]),
+    "neo_pixelnerf_field_tc": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(NeoPixelTCParams), C.POINTER(NeoRays), C.c_void_p, C.c_int,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "neo_pixelnerf_encode": (C.c_int, [C.c_void_p, C.POINTER(NeoRays), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_vanilla_composite_bwd": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 3 + [C.c_void_p] * 7),
     "neo_mip_workspace_bytes": (C.c_size_t, [C.c_int, C.POINTER(NeoMipCfg), C.c_int]),
     "neo_mip_render_fwd": (C.c_int, [C.POINTER(NeoMipMLPParams), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(NeoMipCfg),

@@ -131,6 +131,25 @@ def make_vanilla_params(seed: int = 0, density_bias_shift: float = 1.0) -> Dict[
     return P
 
 
+def make_pixelnerf_params(seed: int = 0, density_bias_shift: float = 1.0) -> Dict[str, Tensor]:
+    """Two PixelNeRF NeRFMLP parameter sets with the reference's shapes (models/vanilla_nerf/model_pixel.py:35-93): pts_linears.0
+    (128,575), .1-.3 (128,128), views_linear.0 (128,155), .1 (128,128), bottleneck (128,128), density (1,128), rgb (3,128)."""
+    g = torch.Generator().manual_seed(3000 + seed)
+    P: Dict[str, Tensor] = {}
+    for pre in VANILLA_PREFIXES:
+        shapes = {f"pts_linears.{i}": (128, 63 + LOCAL_CH if i == 0 else 128) for i in range(4)}
+        shapes.update({"views_linear.0": (128, 155), "views_linear.1": (128, 128), "bottleneck_layer": (128, 128),
+                       "density_layer": (1, 128), "rgb_layer": (3, 128)})
+        for name, (o, i) in shapes.items():
+            w, b = _linear(o, i, g, xavier=(name != "views_linear.0"))
+            w = w * {"density_layer": 3.0, "rgb_layer": 4.0, "views_linear.0": 2.0}.get(name, 1.5)
+            if name == "density_layer":
+                b = b + density_bias_shift
+            P[pre + name + ".weight"] = w
+            P[pre + name + ".bias"] = b
+    return P
+
+
 def make_mip_params(seed: int = 0, width: int = 1024) -> Dict[str, Tensor]:
     """MipNeRF360 parameter set (models/mipnerf360/model.py:176-234): two PropMLPs (4x256, density only) and one NeRFMLP
     (8 x `width`, default 1024) under the reference's state-dict names, plus the `pos_basis_t` buffers."""
