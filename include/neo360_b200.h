@@ -582,6 +582,24 @@ int neo_field_train_bwd(const float* g_hbar, int nv, int M, int in_ch, const flo
                         const void* saved, size_t saved_bytes, float* d_pm, float* gw0, float* gb0, float* gw1, float* gb1,
                         float* gw2, float* gb2, float* gw3, float* gb3, void* scratch, size_t scratch_bytes, void* stream);
 
+/* ---- PixelNeRF training on the tensor cores (csrc/field_train.cu, the PixelNeRF form of the kernels above): layers 0-3 of one
+ * pixelnerf.NeRFMLP trunk in the projected formulation, bf16 operands, fp32 accumulation.  cam (nv*M, 3) camera-frame points (row v M + j:
+ * point j in source view v, the frame of neo_pixelnerf_encode's first three enc columns); p0 (nv*M, 128) looked-up rows of
+ * latent . W0[:, 63:575]^T, added to layer 0's pre-activation unrounded; w0 (128, 63) = pts_linears.0 encoding columns, w1 / w2 / w3
+ * (128,128), biases (128), all fp32 nn.Linear layout.  Layer 3 has no skip: h3 = relu(w3 h2 + b3).  hbar (M, 128) = the view mean of
+ * h3.  Saved state: neo_pixelnerf_train_workspace_bytes(nv, M, 0) bytes written by the forward and read by the backward; the backward's
+ * scratch: (nv, M, 1) bytes (0 = invalid sizes).  Backward: g_hbar (M,128) -> d_p0 (nv*M, 128) and every weight / bias gradient in the
+ * layout of the inputs (written, not accumulated).  NEO_ERR_INVALID before any launch on a NULL buffer, nv outside 1..8, M <= 0, more
+ * than 2^25 rows (nv*M), or a p0 / hbar / g_hbar / d_p0 / workspace buffer not 16-byte aligned; NEO_ERR_WORKSPACE on a short workspace.
+ * No floating-point atomics: two calls are bit-identical. ---- */
+size_t neo_pixelnerf_train_workspace_bytes(int nv, int M, int which);
+int neo_pixelnerf_train_fwd(const float* cam, const float* p0, int nv, int M, const float* w0, const float* b0, const float* w1,
+                            const float* b1, const float* w2, const float* b2, const float* w3, const float* b3, float* hbar,
+                            void* saved, size_t saved_bytes, void* stream);
+int neo_pixelnerf_train_bwd(const float* g_hbar, int nv, int M, const float* w1, const float* w2, const float* w3, const void* saved,
+                            size_t saved_bytes, float* d_p0, float* gw0, float* gb0, float* gw1, float* gb1, float* gw2, float* gb2,
+                            float* gw3, float* gb3, void* scratch, size_t scratch_bytes, void* stream);
+
 /* ---- Vanilla NeRF and Mip-NeRF 360 training on the tensor cores (csrc/dense_train.cu, csrc/gemm_tc.cu): the products of their dense
  * layers, bf16 operands (row-major, row strides in elements), fp32 accumulation, asynchronous on `stream`, no floating-point atomics.
  * Each returns NEO_ERR_INVALID before any launch on a NULL buffer it needs, a shape or stride outside its contract, or a misaligned

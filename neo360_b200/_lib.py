@@ -178,6 +178,10 @@ SYMBOLS = {
     "neo_field_train_fwd": (C.c_int, [C.c_void_p] * 3 + [C.c_int] * 3 + [C.c_void_p] * 10 + [C.c_size_t, C.c_void_p]),
     "neo_field_train_bwd": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int] + [C.c_void_p] * 4 + [C.c_size_t] + [C.c_void_p] * 10 +
                             [C.c_size_t, C.c_void_p]),
+    "neo_pixelnerf_train_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "neo_pixelnerf_train_fwd": (C.c_int, [C.c_void_p] * 2 + [C.c_int] * 2 + [C.c_void_p] * 10 + [C.c_size_t, C.c_void_p]),
+    "neo_pixelnerf_train_bwd": (C.c_int, [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 4 + [C.c_size_t] + [C.c_void_p] * 10 +
+                                [C.c_size_t, C.c_void_p]),
     "neo_profile": (C.c_int, [C.c_int]),
     "neo_profile_read": (C.c_int, [C.POINTER(C.c_float), C.POINTER(C.c_int), C.POINTER(C.c_ulonglong), C.POINTER(C.c_double)]),
     "neo_tc_gemm_f16": (C.c_int, [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_longlong, C.c_longlong,

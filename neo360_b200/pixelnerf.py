@@ -12,8 +12,12 @@ on the tensor cores through gemm_tc.cu, fp16 operands and fp32 accumulation; vie
 
 Training (autograd on, module in train mode, parameters that require grad): the encoder runs under autograd on every call so its
 convolutions train; sampling, encodings, the latent lookup and its backward (neo_index_maps / neo_index_maps_bwd, or the order-fixed
-_det form under torch.use_deterministic_algorithms) and compositing forward and backward are the library's; the dense layers are framework
-fp32 / TF32 GEMMs on the modules' parameters, as in vanilla NeRF's default training."""
+_det form under torch.use_deterministic_algorithms) and compositing forward and backward are the library's.  `train_precision` selects the
+MLP's arithmetic: "fp32" (default) runs the dense layers as framework fp32 / TF32 GEMMs on the modules' parameters in the reference
+formulation, as in vanilla NeRF's default training; "tc" applies the latent columns of pts_linears.0 to the latent map once per step
+(P0 = latent . W0[:, 63:575]^T under autograd, exact re-association: the lookup is linear), looks up 128 projected channels instead of 512,
+runs layers 0-3 and the view mean forward and backward on the tensor cores (training._PixelTrunkTC: bf16 operands, fp32 accumulation) and
+the head once per point on the view mean (training.view_mean_head, fp32)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -26,7 +30,7 @@ import torch.nn.functional as F
 from . import _lib as L
 from .encoder import SpatialEncoder
 from .renderer import Scene
-from .training import _Composite, _index_maps_bwd_det
+from .training import _Composite, _PixelTrunkTC, _index_maps_bwd_det, check_train_precision, view_mean_head
 
 
 def _stream():
@@ -106,6 +110,15 @@ def _mlp_train(m: NeRFMLP, enc: torch.Tensor, dir_tile: torch.Tensor, local: tor
     return lin(m.rgb_layer, torch.relu(lin(m.views_linear[1], q))), raw_sigma
 
 
+def _mlp_train_tc(m: NeRFMLP, cam: torch.Tensor, dir_tile: torch.Tensor, p0: torch.Tensor, nv: int):
+    """`_mlp_train` with the latent columns of layer 0 already applied (p0 (nv*M, 128) = looked-up rows of latent . W0[:, 63:]^T): the
+    trunk on the tensor cores from the camera-frame points cam (nv, M, 3), the head once per point -> raw rgb (M,3), raw sigma (M,1)."""
+    p = m.pts_linears
+    hbar = _PixelTrunkTC.apply(cam, p0, p[0].weight[:, :63], p[0].bias, p[1].weight, p[1].bias, p[2].weight, p[2].bias, p[3].weight,
+                               p[3].bias)
+    return view_mean_head(m, hbar, dir_tile, nv)
+
+
 class _LatentLookup(torch.autograd.Function):
     """SpatialEncoder.index rows of world points pts (M,3): latent_cl (nv,Hl,Wl,512) -> (nv*M,512); the backward scatters into the
     channel-last latent gradient (neo_index_maps_bwd, or neo_index_maps_bwd_det under deterministic algorithms)."""
@@ -138,13 +151,15 @@ class _LatentLookup(torch.autograd.Function):
 
 class PixelNeRF(nn.Module):
     def __init__(self, num_levels: int = 2, min_deg_point: int = 0, max_deg_point: int = 10, deg_view: int = 4, num_coarse_samples: int = 64,
-                 num_fine_samples: int = 64, use_viewdirs: bool = True, noise_std: float = 0.0, lindisp: bool = False, num_src_views: int = 3):
+                 num_fine_samples: int = 64, use_viewdirs: bool = True, noise_std: float = 0.0, lindisp: bool = False, num_src_views: int = 3,
+                 train_precision: str = "fp32"):
         super().__init__()
         if num_levels != 2 or lindisp or noise_std != 0.0 or not use_viewdirs:
             raise NotImplementedError("reference defaults only (models/vanilla_nerf/model_pixel.py:134-147)")
         self.num_levels, self.num_src_views = num_levels, num_src_views
         self.num_coarse_samples, self.num_fine_samples = num_coarse_samples, num_fine_samples
         self.precision = "fp32"
+        self.train_precision = check_train_precision(train_precision)   # "fp32": framework GEMMs; "tc": bf16 tensor cores (training only)
         self.encoder = SpatialEncoder()
         self.coarse_mlp = NeRFMLP(min_deg_point, max_deg_point, deg_view)
         self.fine_mlp = NeRFMLP(min_deg_point, max_deg_point, deg_view)
@@ -284,12 +299,15 @@ class PixelNeRF(nn.Module):
         """PixelNeRF.forward under autograd (LitPixelNeRF.training_step, model_pixel.py:322-347): differentiable w.r.t. every MLP and
         encoder parameter."""
         lib = L.load()
+        tc = check_train_precision(self.train_precision) == "tc"
         r, (o, d, vd) = self._rays(rays, chunk)
         n, dev = o.shape[0], o.device
         nv = self.num_src_views
         with torch.cuda.device(dev):
             latent = self.encoder(rays["src_imgs"])
-            lat_cl = latent.permute(0, 2, 3, 1).contiguous()
+            lat_cl = latent.permute(0, 2, 3, 1)                         # channel-last: the lookup's layout, the projection contracts it
+            if not tc:
+                lat_cl = lat_cl.contiguous()
             sc = self._ensure_scene(rays, lat_cl.shape[1:3])
             u = self._uniforms(rays, randomized, n, dev)
             ret, t, w = [], None, None
@@ -299,8 +317,12 @@ class PixelNeRF(nn.Module):
                 M = n * N
                 enc, dtile, pts = torch.empty(nv * M, 63, device=dev), torch.empty(nv * M, 27, device=dev), torch.empty(M, 3, device=dev)
                 L.check(lib.neo_pixelnerf_encode(sc.handle, C.byref(r), L.ptr(t), N, L.ptr(enc), L.ptr(dtile), L.ptr(pts), _stream()))
-                local = _LatentLookup.apply(pts, lat_cl, sc)
-                raw_rgb, raw_sigma = _mlp_train(mlp, enc, dtile, local, nv)
+                if tc:
+                    p0 = _LatentLookup.apply(pts, lat_cl @ mlp.pts_linears[0].weight[:, 63:].t(), sc)
+                    raw_rgb, raw_sigma = _mlp_train_tc(mlp, enc[:, :3].reshape(nv, M, 3), dtile, p0, nv)
+                else:
+                    local = _LatentLookup.apply(pts, lat_cl, sc)
+                    raw_rgb, raw_sigma = _mlp_train(mlp, enc, dtile, local, nv)
                 rgb = torch.sigmoid(raw_rgb).reshape(n, N, 3)               # model_pixel.py:245-246
                 sigma = torch.relu(raw_sigma).reshape(n, N, 1)
                 comp, acc, w, _, depth = _Composite.apply(rgb, sigma, t, d, None, white_bkgd, 2)

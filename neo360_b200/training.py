@@ -244,6 +244,19 @@ def _mlp_projected(mlp, enc: Tensor, dir_tile: Tensor, local_p: Tensor, world_p:
     return lin(mlp.rgb_layer, q), raw_sigma
 
 
+def _trunk_workspace(need: int, dev) -> Tensor:
+    """A byte buffer of the size a `*_train_workspace_bytes` query returned (0: the query refused the sizes)."""
+    if need == 0:
+        L.check(-1)
+    return torch.empty(need, dtype=torch.uint8, device=dev)
+
+
+def _trunk_grads(E: int, k3: int, dev) -> List[Tensor]:
+    """Outputs of a trunk backward: gw0 (128, E), gb0, gw1 (128, 128), gb1, gw2 (128, 128), gb2, gw3 (128, k3), gb3."""
+    return [torch.empty(128, E, device=dev), torch.empty(128, device=dev), torch.empty(128, 128, device=dev), torch.empty(128, device=dev),
+            torch.empty(128, 128, device=dev), torch.empty(128, device=dev), torch.empty(128, k3, device=dev), torch.empty(128, device=dev)]
+
+
 class _TrunkTC(torch.autograd.Function):
     """Layers 0-3 of a NeRFPPMLP and the view mean, projected formulation, on the tensor cores (csrc/field_train.cu, bf16 operands, fp32
     accumulation): cam (NV, M, in_ch) camera-frame encoding points, local_p / world_p (NV*M, 256) looked-up [P0 | P3], the encoding and
@@ -258,9 +271,7 @@ class _TrunkTC(torch.autograd.Function):
         cam_c, lp, wp = f(cam), f(local_p), f(world_p)
         ws = [f(t) for t in (w0e, b0, w1, b1, w2, b2, w3e, b3)]
         need = lib.neo_field_train_workspace_bytes(nv, M, ich, 0)
-        if need == 0:
-            L.check(-1)
-        saved = torch.empty(need, dtype=torch.uint8, device=cam.device)
+        saved = _trunk_workspace(need, cam.device)
         hbar = torch.empty(M, 128, device=cam.device)
         with torch.cuda.device(cam.device):
             L.check(lib.neo_field_train_fwd(L.ptr(cam_c), L.ptr(lp), L.ptr(wp), nv, M, ich, *[L.ptr(t) for t in ws], L.ptr(hbar),
@@ -276,33 +287,74 @@ class _TrunkTC(torch.autograd.Function):
         nv, M, ich = ctx.dims
         E, dev = 21 * ich, saved.device
         need = lib.neo_field_train_workspace_bytes(nv, M, ich, 1)
-        if need == 0:
-            L.check(-1)
-        scratch = torch.empty(need, dtype=torch.uint8, device=dev)
+        scratch = _trunk_workspace(need, dev)
         d_pm = torch.empty(nv * M, 256, device=dev)
-        g = [torch.empty(128, E, device=dev), torch.empty(128, device=dev), torch.empty(128, 128, device=dev), torch.empty(128, device=dev),
-             torch.empty(128, 128, device=dev), torch.empty(128, device=dev), torch.empty(128, 128 + E, device=dev), torch.empty(128, device=dev)]
+        g = _trunk_grads(E, 128 + E, dev)
         with torch.cuda.device(dev):
             L.check(lib.neo_field_train_bwd(L.ptr(g_hbar.contiguous().float()), nv, M, ich, L.ptr(w1), L.ptr(w2), L.ptr(w3e), L.ptr(saved),
                                             saved.numel(), L.ptr(d_pm), *[L.ptr(t) for t in g], L.ptr(scratch), need, _stream()))
         return (None, d_pm, d_pm, *g)
 
 
-def _mlp_projected_tc(mlp, cam: Tensor, dir_tile: Tensor, local_p: Tensor, world_p: Tensor, nv: int):
-    """`_mlp_projected` with the trunk (layers 0-3 and the view mean) on the tensor cores (`_TrunkTC`).  The head is re-associated
-    exactly: bottleneck -> views_linear.0 is linear and so is the view mean, so it runs once per point on hbar and the view mean of the
-    direction encodings, in fp32."""
-    E = 21 * cam.shape[-1]
+class _PixelTrunkTC(torch.autograd.Function):
+    """Layers 0-3 of PixelNeRF's NeRFMLP trunk and the view mean, projected formulation, on the tensor cores (the PixelNeRF form of
+    csrc/field_train.cu): cam (NV, M, 3) camera-frame points, p0 (NV*M, 128) looked-up rows of latent . W0[:, 63:575]^T, the encoding
+    columns of layer 0, layers 1-3 (no skip at layer 3) -> hbar (M, 128) = mean over the views of h3.  The backward returns the row
+    gradient of p0 and every weight / bias gradient; no floating-point atomics."""
+
+    @staticmethod
+    def forward(ctx, cam, p0, w0e, b0, w1, b1, w2, b2, w3, b3):
+        lib = L.load()
+        nv, M, _ = cam.shape
+        f = lambda t: t.detach().contiguous().float()
+        cam_c, p0c = f(cam), f(p0)
+        ws = [f(t) for t in (w0e, b0, w1, b1, w2, b2, w3, b3)]
+        saved = _trunk_workspace(lib.neo_pixelnerf_train_workspace_bytes(nv, M, 0), cam.device)
+        hbar = torch.empty(M, 128, device=cam.device)
+        with torch.cuda.device(cam.device):
+            L.check(lib.neo_pixelnerf_train_fwd(L.ptr(cam_c), L.ptr(p0c), nv, M, *[L.ptr(t) for t in ws], L.ptr(hbar), L.ptr(saved),
+                                                saved.numel(), _stream()))
+        ctx.save_for_backward(saved, ws[2], ws[4], ws[6])
+        ctx.dims = (nv, M)
+        return hbar
+
+    @staticmethod
+    def backward(ctx, g_hbar):
+        lib = L.load()
+        saved, w1, w2, w3 = ctx.saved_tensors
+        nv, M = ctx.dims
+        dev = saved.device
+        need = lib.neo_pixelnerf_train_workspace_bytes(nv, M, 1)
+        scratch = _trunk_workspace(need, dev)
+        d_p0 = torch.empty(nv * M, 128, device=dev)
+        g = _trunk_grads(63, 128, dev)
+        with torch.cuda.device(dev):
+            L.check(lib.neo_pixelnerf_train_bwd(L.ptr(g_hbar.contiguous().float()), nv, M, L.ptr(w1), L.ptr(w2), L.ptr(w3), L.ptr(saved),
+                                                saved.numel(), L.ptr(d_p0), *[L.ptr(t) for t in g], L.ptr(scratch), need, _stream()))
+        return (None, d_p0, *g)
+
+
+def view_mean_head(mlp, hbar: Tensor, dir_tile: Tensor, nv: int):
+    """The head after a view-averaged trunk, once per point: raw rgb and raw sigma from hbar (M, 128) and dir_tile (NV*M, 27).  Exact
+    re-association of the per-view head: bottleneck -> views_linear.0 is linear and so is the view mean, so it runs on hbar and the view
+    mean of the direction encodings, in fp32.  NeRFPPMLP and PixelNeRF's NeRFMLP share this head."""
     lin = lambda m, x: F.linear(x, m.weight, m.bias)
-    p = mlp.pts_linears
-    hbar = _TrunkTC.apply(cam, local_p, world_p, p[0].weight[:, :E], p[0].bias, p[1].weight, p[1].bias, p[2].weight, p[2].bias,
-                          p[3].weight[:, :128 + E], p[3].bias)
     M = hbar.shape[0]
     raw_sigma = lin(mlp.density_layer, hbar)
     dbar = dir_tile.reshape(nv, M, -1).mean(0)
     q = lin(mlp.views_linear[0], torch.cat([lin(mlp.bottleneck_layer, hbar), dbar], -1))
     q = torch.relu(lin(mlp.views_linear[1], torch.relu(q)))
     return lin(mlp.rgb_layer, q), raw_sigma
+
+
+def _mlp_projected_tc(mlp, cam: Tensor, dir_tile: Tensor, local_p: Tensor, world_p: Tensor, nv: int):
+    """`_mlp_projected` with the trunk (layers 0-3 and the view mean) on the tensor cores (`_TrunkTC`) and the head once per point
+    (`view_mean_head`)."""
+    E = 21 * cam.shape[-1]
+    p = mlp.pts_linears
+    hbar = _TrunkTC.apply(cam, local_p, world_p, p[0].weight[:, :E], p[0].bias, p[1].weight, p[1].bias, p[2].weight, p[2].bias,
+                          p[3].weight[:, :128 + E], p[3].bias)
+    return view_mean_head(mlp, hbar, dir_tile, nv)
 
 
 TRAIN_PRECISIONS = ("fp32", "tc")

@@ -1,6 +1,9 @@
 """PixelNeRF throughput on one GPU: 640x480 frame rays/s of fp32 and tensor-core inference, and the step time of a 1024-ray training step (forward +
-backward of both levels, encoder inside) with fp32 and with TF32 framework GEMMs, against the oracle's eager path on the same GPU.
-Variants alternate in one process.  Prints one JSON line.
+backward of both levels, encoder inside) with fp32 and with TF32 framework GEMMs, with the framework MLP under torch.autocast(bfloat16)
+(TF32 allowed elsewhere), and with train_precision="tc" (trunk on the tensor cores in bf16; encoder, projection and head framework ops with
+TF32 allowed), against the oracle's eager path on the same GPU.  Variants alternate in one process.  For each CUDA training variant it also
+prints the step's split by CUDA events (encoder forward + backward against the rest), its peak memory, and the projection GEMM of the "tc"
+path (P0 = latent . W0[:, 63:575]^T, forward + backward, one level) timed alone.  Prints one JSON line.
 
     python tools/bench_pixelnerf.py [--iters 5]"""
 import argparse
@@ -12,7 +15,7 @@ import time
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from neo360_b200 import PixelNeRF, synth  # noqa: E402
+from neo360_b200 import PixelNeRF, pixelnerf, synth  # noqa: E402
 from oracle import neo360_oracle as orc, pixelnerf_oracle as por  # noqa: E402
 
 NEAR, FAR = 0.02, 3.0
@@ -54,8 +57,9 @@ def main():
             for i in range(0, H * W, 4096):          # the reference's chunked render loop; the encoder runs once (hoisted)
                 net({**src, **{k: v[i:i + 4096] for k, v in frame.items() if k.startswith(("rays", "view"))}}, False, False, NEAR, FAR)
 
-    def step_cuda():
+    def step_cuda(tprec="fp32"):
         net.train()
+        net.train_precision = tprec
         net.zero_grad(set_to_none=True)
         ret = net({**rays, **src}, True, False, NEAR, FAR)
         (((ret[0][0] - target) ** 2).mean() + ((ret[1][0] - target) ** 2).mean()).backward()
@@ -70,6 +74,54 @@ def main():
         ret = por.render(rays, osc, P, 64, 64, NEAR, FAR, False, rand=u)
         (((ret[0][0] - target) ** 2).mean() + ((ret[1][0] - target) ** 2).mean()).backward()
 
+    mlp_train = pixelnerf._mlp_train
+
+    def step_autocast():
+        def mlp_autocast(*a):
+            with torch.autocast("cuda", dtype=torch.bfloat16):
+                return tuple(t.float() for t in mlp_train(*a))
+        pixelnerf._mlp_train = mlp_autocast
+        try:
+            step_cuda()
+        finally:
+            pixelnerf._mlp_train = mlp_train
+
+    lat_shape = net.encoder(imgs).shape
+    lat_p = torch.randn(lat_shape[0], lat_shape[2], lat_shape[3], lat_shape[1], device=dev, requires_grad=True)
+    w0 = net.coarse_mlp.pts_linears[0].weight
+
+    def projection():
+        lat_p.grad = None
+        w0.grad = None
+        p0 = lat_p @ w0[:, 63:].t()
+        p0.backward(torch.ones_like(p0))
+
+    def split(fn):
+        """(encoder forward + backward ms, rest ms) of one step by CUDA events: the encoder's backward runs from the moment the latent's
+        gradient is complete to the end of the step (its inputs are leaves)."""
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
+        enc_forward = net.encoder.forward
+
+        def forward(x):
+            ev[1].record()
+            lat = enc_forward(x)
+            ev[2].record()
+            lat.register_hook(lambda g: ev[3].record())
+            return lat
+
+        net.encoder.forward = forward
+        try:
+            torch.cuda.synchronize()
+            ev[0].record()
+            fn()
+            ev[4].record()
+        finally:
+            del net.encoder.forward
+        torch.cuda.synchronize()
+        total = ev[0].elapsed_time(ev[4])
+        enc = ev[1].elapsed_time(ev[2]) + ev[3].elapsed_time(ev[4])
+        return round(enc, 2), round(total - enc, 2)
+
     def with_tf32(flag, fn):
         def run():
             torch.backends.cuda.matmul.allow_tf32 = flag
@@ -78,14 +130,21 @@ def main():
         return run
 
     variants = {"render_fp32": lambda: render("fp32"), "render_tc": lambda: render("tc"), "train_fp32": with_tf32(False, step_cuda), "train_tf32": with_tf32(True, step_cuda),
+                "train_autocast": with_tf32(True, step_autocast), "train_tc": with_tf32(True, lambda: step_cuda("tc")),
                 "train_eager_fp32": with_tf32(False, step_eager), "train_eager_tf32": with_tf32(True, step_eager)}
+    variants["projection_tf32"] = with_tf32(True, projection)
     for fn in variants.values():
         fn()
     res = {k: [] for k in variants}
+    peak = {}
     for _ in range(3):
         for k, fn in variants.items():
+            torch.cuda.reset_peak_memory_stats()
             res[k].append(timed(fn, args.iters))
+            peak[k] = max(peak.get(k, 0), torch.cuda.max_memory_allocated())
     best = {k: min(v) for k, v in res.items()}
+    cuda_train = ("train_fp32", "train_tf32", "train_autocast", "train_tc")
+    splits = {k: [split(variants[k]) for _ in range(3)] for k in cuda_train}
     q = torch.cuda.get_device_properties(0).name
     try:
         import subprocess
@@ -94,7 +153,10 @@ def main():
         power = "unknown"
     print(json.dumps({"gpu": q, "power_limit": power, "frame_rays_per_s_fp32": round(H * W / best["render_fp32"]),
                       "frame_rays_per_s_tc": round(H * W / best["render_tc"]),
-                      **{f"{k}_step_ms": round(1e3 * v, 2) for k, v in best.items() if k.startswith("train")}}))
+                      **{f"{k}_step_ms": round(1e3 * v, 2) for k, v in best.items() if k.startswith("train")},
+                      "projection_fwd_bwd_ms_per_level": round(1e3 * best["projection_tf32"], 3),
+                      "split_encoder_vs_rest_ms": {k: min(v, key=sum) for k, v in splits.items()},
+                      "peak_mem_gib": {k: round(peak[k] / 2 ** 30, 2) for k in variants if k.startswith("train")}}))
 
 
 if __name__ == "__main__":
