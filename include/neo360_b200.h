@@ -558,8 +558,9 @@ int neo_tc_enc_column(int in_ch, int col);
  * (0,1), (1,0), (1,1).  out: n_rays * 64 bytes, 16-byte aligned. */
 int neo_tc_dir_fragments(const NeoScene* scene, const NeoRays* rays, void* out, void* stream);
 
-/* "" or a description of the mbarrier wait that timed out inside the NEO_PREC_TC field kernel (the kernel bounds its wait for the
- * weight copies and traps instead of hanging; the waiter's identity is recorded in host-mapped memory, which survives the failed context). */
+/* "" or a description of the mbarrier wait that timed out inside the NEO_PREC_TC field kernel (the kernel bounds its waits for the
+ * weight copies and for the hand-off between its producer and consumer warpgroups, and traps instead of hanging; the barrier and the
+ * waiter's identity are recorded in host-mapped memory, which survives the failed context). */
 const char* neo_tc_trap_info(void);
 const char* neo_last_error(void);
 /* "neo360_b200 <version> sm_90a" */

@@ -10,7 +10,10 @@
 //     i.e. the cross-view means become one register accumulator summed over the views.
 //   * b0 and b3 ride on a constant-one column of the positional encoding; b1, b2 and the head biases seed the accumulators.
 //
-// Layout: one persistent CTA per SM, two warpgroups, each working on its own tiles of 64 points (32 rays x 2 consecutive samples).
+// Layout: one persistent CTA per SM, three warpgroups.  Two consumer warpgroups each work on their own tiles of 64 points (32 rays x 2
+// consecutive samples); the producer warpgroup builds their geometry (points, camera-frame encodings, tap tables: 64 threads per
+// consumer, one point each) and hands it over through full / empty mbarrier pairs, so the consumers only blend and multiply.
+// setmaxnreg moves registers from the producer (56) to the consumers (224).
 // The rays of a tile are 32 consecutive slots of the ray order (one 8x4 pixel block of a frame, renderer._blocked_order): rays that
 // close together read the same texels at a sample, while consecutive samples move on to the next texel, so a tile that spans more
 // rays and fewer samples reads fewer distinct texels per point (on H100 the field launches are 1.11x faster than with 16 rays x 4
@@ -36,8 +39,14 @@ using namespace hopper;
 constexpr int kTileRays = 32;
 constexpr int kTileSamples = 2;
 constexpr int kTilePts = kTileRays * kTileSamples;  // = the M of one wgmma
-constexpr int kWarpgroups = 2;
-constexpr int kThreads = 128 * kWarpgroups;
+constexpr int kConsumers = 2;                        // MMA warpgroups 0, 1; warpgroup 2 is the producer
+constexpr int kThreads = 128 * (kConsumers + 1);
+// setmaxnreg only moves registers within the CTA's launch allocation (kLaunchRegs per thread, what __launch_bounds__ leaves ptxas:
+// 168 x 384 = 64 512, not the SM's 65 536): a split that asks for more leaves a consumer warp waiting for registers forever.
+constexpr int kLaunchRegs = 65536 / kThreads / 8 * 8;
+constexpr int kConsumerRegs = 224, kProducerRegs = 56;
+static_assert(kConsumers * 128 * kConsumerRegs + 128 * kProducerRegs == kThreads * kLaunchRegs, "setmaxnreg split must fill the CTA's registers");
+static_assert(kConsumers * kTilePts == 128, "the producer warpgroup has one thread per point of each consumer's tile");
 
 // head weights image (B operands, 128-byte swizzle): Whead_h 80 x 128 | Whead_dir 80 x 64 | Wv1 64 x 64 | Wrgb 16 x 64
 constexpr uint32_t WH_H = 0, WH_DIR = 20480, WH_V1 = 30720, WH_RGB = 38912, WH_BYTES = 40960;
@@ -45,10 +54,18 @@ constexpr int BIAS_FLOATS = 512 + 64 + 64 + 4 + 4;   // fp32: b0..b3 (512) | bq 
 constexpr uint32_t BIAS_BYTES = 2624;                // BIAS_FLOATS * 4 rounded up to 64
 constexpr uint32_t SLAB = 128 * 128;                 // one 64-column slab of a 128-row weight tile
 
-// trunk weights image: W0enc | W1 | W2 | W3h | W3enc, each 128 rows (neurons) x K, K-major in 64-column slabs
+// trunk weights image: W0enc | W1 | W2 | W3h | W3enc, each 128 rows (neurons) x K, K-major in 64-column slabs.  The background's
+// KE = 96 fills only half of each encoding segment's last slab, so W3enc's columns 64-95 are packed into columns 32-63 of W0enc's
+// last slab (w3enc_tail): W3enc takes one slab instead of two, and the 16 KB go to the encoding staging rows.
 __host__ __device__ constexpr int enc_slabs(int KE) { return (KE + 63) / 64; }
 __host__ __device__ constexpr uint32_t trunk_off(int KE, int seg) { return seg == 0 ? 0u : (uint32_t)(enc_slabs(KE) + 2 * (seg - 1)) * SLAB; }
-__host__ __device__ constexpr uint32_t trunk_bytes(int KE) { return trunk_off(KE, 4) + (uint32_t)enc_slabs(KE) * SLAB; }
+__host__ __device__ constexpr uint32_t trunk_bytes(int KE) { return trunk_off(KE, 4) + (uint32_t)(KE / 64) * SLAB; }
+__host__ __device__ constexpr uint32_t w3enc_tail(int KE) { return trunk_off(KE, 0) + (uint32_t)(KE / 64) * SLAB; }
+// byte offset of W3enc's 16-column k-step ks (a wgmma descriptor start address relative to the image)
+__host__ __device__ constexpr uint32_t w3enc_kstep(int KE, int ks) {
+    return ks < 4 * (KE / 64) ? trunk_off(KE, 4) + (uint32_t)(ks >> 2) * SLAB + (uint32_t)(ks & 3) * 32u
+                              : w3enc_tail(KE) + (uint32_t)(ks - 4 * (KE / 64) + 2) * 32u;
+}
 
 // channel order of the projected maps: physical channel p of a texel holds logical channel pmap_logical(p) of [P0 | P3], so that
 // thread t (lane % 4) of an accumulator fragment finds its channels 8 j + 2 t + e (j < 16, e < 2) of a half at
@@ -92,34 +109,42 @@ struct Params {
     MlpTc mlp;
     float* rgb_out;
     float* sigma_out;
-    int* trap;          // host-mapped int[8]: who timed out on the weight-load mbarrier
+    int* trap;          // host-mapped int[8]: who timed out on which mbarrier (wait_timeout)
 #ifdef NEO_FIELD_PHASES
     int phase_slot;     // row of g_phase_cycles this launch adds to
 #endif
 };
 
-// Phase clocks (diagnostic build only, -DNEO_FIELD_PHASES; read by tools/field_phases.py): thread 0 of every warpgroup adds the
-// clock64() cycles between consecutive marks to its phase, and at the end of the kernel the warpgroup's sums (and its tile count) go
-// into the launch's row of g_phase_cycles.  The marks bound the phases as the compiler scheduled them, which is close to, but not
-// exactly, the source order.  Without the macro the kernel has no marks at all.
+// Phase clocks (diagnostic build only, -DNEO_FIELD_PHASES; read by tools/field_phases.py): the first thread of every consumer
+// warpgroup and of every producer half adds the clock64() cycles between consecutive marks to its phase, and at the end of the
+// kernel the sums (and the consumers' tile counts) go into the launch's row of g_phase_cycles.  The marks bound the phases as the
+// compiler scheduled them, which is close to, but not exactly, the source order.  Without the macro the kernel has no marks at all.
 #ifdef NEO_FIELD_PHASES
-constexpr int kPhases = 9;          // tile setup | camera + encodings | tap table | blend P0 | layers 0-2 | blend P3 | layer 3 + head |
-                                    // direction term | colour head + stores
+enum Phase {
+    kPhWait, kPhRows, kPhBlend0, kPhLayers, kPhBlend3, kPhLayer3, kPhDir, kPhColour,          // consumers
+    kPhSetup, kPhEnc, kPhTaps, kPhSlot,                                                      // producer
+    kPhases
+};
 constexpr int kPhaseCols = kPhases + 2;                                  // the phases, then tiles, then taps of non-zero weight
-constexpr uint32_t kPhaseBytes = kWarpgroups * (kPhases + 1) * 8;        // per-warpgroup sums (phases, tiles) in shared memory
+constexpr int kPhaseUnits = 2 * kConsumers;                              // the consumers, then the producer halves
+constexpr uint32_t kPhaseBytes = kPhaseUnits * (kPhases + 1) * 8;        // per-unit sums (phases, tiles) in shared memory
 constexpr int kPhaseSlots = 64;
 __device__ unsigned long long g_phase_cycles[kPhaseSlots][kPhaseCols];    // [launch][column]
 static int g_phase_launches = 0;
-#define FIELD_PHASE_INIT() long long ph_t = clock64(); unsigned long long ph_taps = 0
-#define FIELD_PHASE(p)                                   \
-    do {                                                 \
-        const long long now_ = clock64();                \
-        if (wt == 0) ph_acc[wg][p] += now_ - ph_t;       \
-        ph_t = now_;                                     \
+#define FIELD_PHASE_INIT(unit, lead) \
+    long long ph_t = clock64();      \
+    unsigned long long ph_taps = 0;  \
+    const int ph_unit = (unit);      \
+    const bool ph_lead = (lead)
+#define FIELD_PHASE(p)                                        \
+    do {                                                      \
+        const long long now_ = clock64();                     \
+        if (ph_lead) ph_acc[ph_unit][p] += now_ - ph_t;       \
+        ph_t = now_;                                          \
     } while (0)
 #else
 constexpr uint32_t kPhaseBytes = 0;
-#define FIELD_PHASE_INIT() do {} while (0)
+#define FIELD_PHASE_INIT(unit, lead) do {} while (0)
 #define FIELD_PHASE(p) do {} while (0)
 #endif
 
@@ -168,9 +193,10 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
     return *reinterpret_cast<uint32_t*>(&h);
 }
 // trunk weights image (shared-memory bytes, 128-byte swizzle): element (neuron n, k) of segment s at trunk_off(KE, s) +
-// sw128_off(n, k, 128); segments W0enc (KE) | W1 | W2 | W3h (128 each) | W3enc (KE), encoding segments zero-padded to whole slabs
+// sw128_off(n, k, 128); segments W0enc (KE) | W1 | W2 | W3h (128 each) | W3enc (KE); W3enc's columns from 64 (KE / 64) on at
+// w3enc_tail(KE) + sw128_off(n, 32 + k - 64 (KE / 64), 128)
 __global__ void trunk_img_kernel(NeoMLPParams p, int enc_dim, int KE, unsigned char* __restrict__ img) {
-    const int es = enc_slabs(KE) * 64, KW = 2 * es + 384;
+    const int KW = 2 * KE + 384;
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= KW * 128) return;
     const int n = idx / KW, kk = idx % KW;
@@ -178,7 +204,6 @@ __global__ void trunk_img_kernel(NeoMLPParams p, int enc_dim, int KE, unsigned c
     const bool bg = (KE == 96);
     // encoding column `col` of the kernel's operand layout (enc_col<>): reference column, bias (constant-one column) or zero
     auto enc_w = [&](const float* w, size_t stride, size_t off0, const float* bias, int col) -> float {
-        if (col >= KE) return 0.f;
         const EncCol e = bg ? enc_col<4>(col) : enc_col<3>(col);
         if (e.kind == 1) return bias[n];
         const int ref = bg ? enc_col_ref_index<4>(col) : enc_col_ref_index<3>(col);
@@ -186,12 +211,14 @@ __global__ void trunk_img_kernel(NeoMLPParams p, int enc_dim, int KE, unsigned c
     };
     int seg, k;
     float x;
-    if (kk < es) { seg = 0; k = kk; x = enc_w(p.w0, in_dim, 0, p.b0, k); }
-    else if (kk < es + 128) { seg = 1; k = kk - es; x = p.w1[n * 128 + k]; }
-    else if (kk < es + 256) { seg = 2; k = kk - es - 128; x = p.w2[n * 128 + k]; }
-    else if (kk < es + 384) { seg = 3; k = kk - es - 256; x = p.w3[(size_t)n * (128 + in_dim) + k]; }
-    else { seg = 4; k = kk - es - 384; x = enc_w(p.w3, 128 + in_dim, 128, p.b3, k); }
-    *reinterpret_cast<__half*>(img + trunk_off(KE, seg) + sw128_off(n, k, 128)) = __float2half_rn(x);
+    if (kk < KE) { seg = 0; k = kk; x = enc_w(p.w0, in_dim, 0, p.b0, k); }
+    else if (kk < KE + 128) { seg = 1; k = kk - KE; x = p.w1[n * 128 + k]; }
+    else if (kk < KE + 256) { seg = 2; k = kk - KE - 128; x = p.w2[n * 128 + k]; }
+    else if (kk < KE + 384) { seg = 3; k = kk - KE - 256; x = p.w3[(size_t)n * (128 + in_dim) + k]; }
+    else { seg = 4; k = kk - KE - 384; x = enc_w(p.w3, 128 + in_dim, 128, p.b3, k); }
+    const int full = 64 * (KE / 64);
+    const uint32_t off = (seg == 4 && k >= full) ? w3enc_tail(KE) + sw128_off(n, 32 + k - full, 128) : trunk_off(KE, seg) + sw128_off(n, k, 128);
+    *reinterpret_cast<__half*>(img + off) = __float2half_rn(x);
 }
 
 // head weights (pre-swizzled smem image) + folded biases
@@ -290,23 +317,33 @@ __device__ __forceinline__ void tap_quad(float gx, float gy, int W, int H, TapQu
 // ------------------------------------------------------------------------------------------------
 // the field kernel
 // ------------------------------------------------------------------------------------------------
-__device__ __noinline__ void load_timeout(int* trapinfo, uint32_t bar) {
+// Hand-off between the producer and consumer c: mbarrier 1 + kChans c + k of the CTA (mbarrier 0: the weight copies).  A full
+// barrier completes when the consumer's 64 producer threads have written, an empty one when its 128 threads have read.
+enum Chan { kRowsFull, kRowsEmpty, kStageFull, kStageEmpty, kTapsFull, kTapsEmpty, kChans };
+constexpr int kBars = 1 + kChans * kConsumers;
+
+// records who timed out on which mbarrier (id: 0 the weight copies, 1 + kChans c + k channel k of consumer c), then traps
+__device__ __noinline__ void wait_timeout(int* trapinfo, uint32_t bar, int id) {
     if (trapinfo) {
         volatile int* t = trapinfo;
         if (t[0] == 0) {
-            t[1] = (int)blockIdx.x; t[2] = (int)threadIdx.x; t[3] = (int)bar; t[4] = 0; t[5] = (int)gridDim.x;
+            t[1] = (int)blockIdx.x; t[2] = (int)threadIdx.x; t[3] = (int)bar; t[4] = id; t[5] = (int)gridDim.x;
             t[0] = 1000;
         }
         __threadfence_system();
     }
     asm volatile("trap;");
 }
+// bounded wait for the phase of parity `parity` of mbarrier id (bar0: the address of mbarrier 0)
+__device__ __forceinline__ void bar_wait(int* trapinfo, uint32_t bar0, int id, uint32_t parity) {
+    const uint32_t b = bar0 + 8u * (uint32_t)id;
+    if (!mbar_wait_bounded(b, parity)) wait_timeout(trapinfo, b, id);
+}
 
 __device__ __forceinline__ float sel4(const float* x, int i) { return i == 0 ? x[0] : i == 1 ? x[1] : i == 2 ? x[2] : x[3]; }
 
-// Encoding staging: per (tile, view) a warpgroup computes its 64 points' encodings once, as a flat set of items, into one row of 64
-// fp16 per point (in the bytes of its tap table, before the table is built); then every thread loads its A-fragment columns from
-// the rows.  Row slot 21 j + k holds column k of staged coordinate j: k = 0 the coordinate, 1 + l sin(2^l x), 11 + l cos(2^l x), the
+// Encoding staging: per (tile, view) the producer computes a consumer's 64 points' encodings once, as a flat set of items, into one
+// row of 64 fp16 per point; then every thread of the consumer loads its A-fragment columns from the rows.  Row slot 21 j + k holds column k of staged coordinate j: k = 0 the coordinate, 1 + l sin(2^l x), 11 + l cos(2^l x), the
 // order of enc_col<3> (slot == column for the foreground).  The 32-bit words of a row are XOR-swizzled by the point (bits 2-4), so
 // that the 8 points x 4 words a warp loads per fragment register fall on 32 distinct banks.
 constexpr int kStageRow = 64;
@@ -417,14 +454,13 @@ __device__ __forceinline__ void seed_bias(float (&d)[NC / 2], const float* b, in
 // descriptor of k-step ks of a 128-byte-swizzled K-major weight tile whose 64-column slabs are `slab` bytes apart
 __device__ __forceinline__ uint64_t wdesc(uint32_t base, int ks, uint32_t slab) { return desc_sw128(base + (uint32_t)(ks >> 2) * slab + (uint32_t)(ks & 3) * 32u); }
 
-// Tap table of one (tile, view), per warpgroup in shared memory: for every point n of the tile and map m (latent, xz, xy, yz), the
+// Tap table of one (tile, view), per consumer in shared memory: for every point n of the tile and map m (latent, xz, xy, yz), the
 // texel indices (view included) of the four taps {nw, ne, sw, se} and their bilinear weights.  Split in two arrays of 16-byte
 // entries [m][n], so that the 8 points a warp reads at once fall on distinct banks.
 struct TapTable {
     int4 tex[4][kTilePts];
     float4 w[4][kTilePts];
 };
-static_assert(kTilePts * kStageRow * sizeof(__half) <= sizeof(TapTable), "the encoding staging rows live in the tap table's bytes");
 __device__ __forceinline__ int comp4(const int4& x, int k) { return k == 0 ? x.x : k == 1 ? x.y : k == 2 ? x.z : x.w; }
 __device__ __forceinline__ float comp4(const float4& x, int k) { return k == 0 ? x.x : k == 1 ? x.y : k == 2 ? x.z : x.w; }
 
@@ -492,8 +528,11 @@ __device__ __forceinline__ void blend_maps(float (&acc)[64], const Params& P, co
 template <int KE>
 struct SmemMap {
     static constexpr uint32_t HEAD = trunk_bytes(KE), BIAS = HEAD + WH_BYTES, VIEWS = BIAS + BIAS_BYTES,
-                              PTS = VIEWS + kMaxViews * 64, TAPS = PTS + kWarpgroups * kTilePts * (uint32_t)sizeof(PtsRow),
-                              BAR = TAPS + kWarpgroups * (uint32_t)sizeof(TapTable), PHASES = BAR + 16, TOTAL = PHASES + kPhaseBytes;
+                              PTS = VIEWS + kMaxViews * 64, TAPS = PTS + kConsumers * kTilePts * (uint32_t)sizeof(PtsRow),
+                              STAGE = TAPS + kConsumers * (uint32_t)sizeof(TapTable),
+                              BAR = STAGE + kConsumers * kTilePts * kStageRow * (uint32_t)sizeof(__half),
+                              PHASES = BAR + (kBars * 8 + 15) / 16 * 16, TOTAL = PHASES + kPhaseBytes;
+    static_assert(KE % 64 == 0 || KE % 64 == 32, "an encoding segment ends on a whole or a half slab (w3enc_tail)");
     static_assert(TOTAL + 1024 <= 227u * 1024u, "field kernel shared memory exceeds the 227 KB an sm_90 CTA can have");
 };
 
@@ -507,9 +546,11 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
     using SM = SmemMap<KE>;
     const uint32_t bar = sbase + SM::BAR;
 
-    // ---- one-time setup: every weight of the MLP -> shared memory (TMA bulk copies), source-camera transforms ----
+    // ---- one-time setup: every weight of the MLP -> shared memory (TMA bulk copies), source-camera transforms, hand-off barriers ----
     if (threadIdx.x == 0) {
         mbar_init(bar, 1);
+        for (int c = 0; c < kConsumers; ++c)
+            for (int k = 0; k < kChans; ++k) mbar_init(bar + 8u * (1 + kChans * c + k), (k & 1) ? 128 : kTilePts);   // empty: consumer
         mbar_init_fence();
         constexpr uint32_t TB = trunk_bytes(KE);
         mbar_expect_tx(bar, TB + WH_BYTES + BIAS_FLOATS * 4);
@@ -524,55 +565,131 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
     }
 #ifdef NEO_FIELD_PHASES
     auto ph_acc = reinterpret_cast<unsigned long long (*)[kPhases + 1]>(sgen + SM::PHASES);
-    if (threadIdx.x < kWarpgroups * (kPhases + 1)) (&ph_acc[0][0])[threadIdx.x] = 0ull;
+    if (threadIdx.x < kPhaseUnits * (kPhases + 1)) (&ph_acc[0][0])[threadIdx.x] = 0ull;
 #endif
     __syncthreads();
-    if (!mbar_wait_bounded(bar, 0)) load_timeout(P.trap, bar);
 
-    const int wg = threadIdx.x >> 7, wt = threadIdx.x & 127, warp = wt >> 5, lane = threadIdx.x & 31, t = lane & 3;
-    PtsRow* pts = reinterpret_cast<PtsRow*>(sgen + SM::PTS) + wg * kTilePts;
-    TapTable* tab = reinterpret_cast<TapTable*>(sgen + SM::TAPS) + wg;
+    const int wg = threadIdx.x >> 7;
     const ViewXform* vxs = reinterpret_cast<const ViewXform*>(sgen + SM::VIEWS);
+    const int nv = P.nv, N = P.N;
+
+    if (wg == kConsumers) {
+        // ================= producer: thread pt builds point n of consumer c's tiles =================
+        setmaxnreg_dec<kProducerRegs>();
+        const int pt = threadIdx.x - 128 * kConsumers, c = pt / kTilePts, n = pt % kTilePts;
+        PtsRow* pts = reinterpret_cast<PtsRow*>(sgen + SM::PTS) + c * kTilePts;
+        TapTable* tab = reinterpret_cast<TapTable*>(sgen + SM::TAPS) + c;
+        __half* stage = reinterpret_cast<__half*>(sgen + SM::STAGE) + c * kTilePts * kStageRow;
+        const int cb = 1 + kChans * c;                   // id of this consumer's first channel barrier
+        uint32_t k_rows = 0, k_stage = 0, k_taps = 0;   // fills so far: the producer's wait for fill k is on parity (k & 1) ^ 1
+        FIELD_PHASE_INIT(kConsumers + c, n == 0);
+        for (int tile = blockIdx.x * kConsumers + c; tile < P.n_tiles; tile += gridDim.x * kConsumers) {
+            const int g = tile / P.sg, q = tile % P.sg;
+            bar_wait(P.trap, bar, cb + kRowsEmpty, (k_rows & 1) ^ 1);        // the consumer has copied the previous tile's rows
+            FIELD_PHASE(kPhSlot);
+            {
+                const int rl = n % kTileRays, sl = n / kTileRays;
+                const int slot = g * kTileRays + rl, s = q * kTileSamples + sl;
+                const int slot_c = min(slot, P.n_rays - 1), s_c = min(s, N - 1);
+                const int rid = P.ray_order ? P.ray_order[slot_c] : slot_c;
+                PtsRow pr;
+                pr.rid = rid; pr.sidx = s_c; pr.valid = (slot < P.n_rays) && (s < N);
+                pr.tv = P.tvals[(long long)rid * N + s_c];
+                RayFast rg;
+                ray_fast(P.rays_o + 3 * rid, P.rays_d + 3 * rid, P.far[rid], rg, IS_BG);
+                if (IS_BG) bg_point_fast(rg, pr.tv, P.far_unc, pr.xe, pr.xl);
+                else for (int i = 0; i < 3; ++i) { pr.xe[i] = rg.o[i] + pr.tv * rg.d[i]; pr.xl[i] = pr.xe[i]; }
+                // quirk Q1: the direction of ray (j mod B) of the ray's chunk, j = flat (ray, sample) index inside the chunk
+                const int ch = P.chunk > 0 ? P.chunk : P.n_rays;
+                const int c0 = (rid / ch) * ch;
+                const int Bc = min(ch, P.n_rays - c0);
+                const long long jl = (long long)(rid - c0) * N + s_c;
+                pr.src = c0 + (int)(jl % Bc);
+                pr.pad = 0;
+                pts[n] = pr;
+            }
+            mbar_arrive(bar + 8u * (cb + kRowsFull));
+            ++k_rows;
+            FIELD_PHASE(kPhSetup);
+            if constexpr (IS_BG) {
+                // the s columns 72-92 do not depend on the view: staged as coordinate 0 once per tile
+                const float sx[3] = {pts[n].tv, 0.f, 0.f};
+                bar_wait(P.trap, bar, cb + kStageEmpty, (k_stage & 1) ^ 1);
+                FIELD_PHASE(kPhSlot);
+                stage[stage_slot(n, 0)] = __float2half_rn(sx[0]);
+                stage_items(stage, n, sx, 0, 10);
+                mbar_arrive(bar + 8u * (cb + kStageFull));
+                ++k_stage;
+                FIELD_PHASE(kPhEnc);
+            }
+#pragma unroll 1
+            for (int v = 0; v < nv; ++v) {
+                float ce[3];
+                to_camera(vxs[v], pts[n].xe, ce);
+                bar_wait(P.trap, bar, cb + kStageEmpty, (k_stage & 1) ^ 1);  // the consumer has loaded the previous encodings
+                FIELD_PHASE(kPhSlot);
+#pragma unroll
+                for (int j = 0; j < 3; ++j) stage[stage_slot(n, 21 * j)] = __float2half_rn(ce[j]);
+                stage_items(stage, n, ce, 0, 30);
+                mbar_arrive(bar + 8u * (cb + kStageFull));
+                ++k_stage;
+                FIELD_PHASE(kPhEnc);
+                float cl[3] = {ce[0], ce[1], ce[2]};            // foreground: xl == xe, the lookup point IS the encoded point
+                if constexpr (IS_BG) to_camera(vxs[v], pts[n].xl, cl);
+                bar_wait(P.trap, bar, cb + kTapsEmpty, (k_taps & 1) ^ 1);    // the consumer's blends have read the previous table
+                FIELD_PHASE(kPhSlot);
+#pragma unroll 1
+                for (int m = 0; m < 4; ++m) {
+                    tap_entry(*tab, P.sc, cl, v, n, m);
+#ifdef NEO_FIELD_PHASES
+                    for (int k = 0; k < 4; ++k) ph_taps += comp4(tab->w[m][n], k) != 0.f;
+#endif
+                }
+                mbar_arrive(bar + 8u * (cb + kTapsFull));
+                ++k_taps;
+                FIELD_PHASE(kPhTaps);
+            }
+        }
+#ifdef NEO_FIELD_PHASES
+        if (ph_lead)
+            for (int p = kPhSetup; p < kPhases; ++p) atomicAdd(&g_phase_cycles[P.phase_slot][p], ph_acc[ph_unit][p]);
+        atomicAdd(&g_phase_cycles[P.phase_slot][kPhases + 1], ph_taps);
+#endif
+        return;
+    }
+
+    // ================= consumer wg: blends and tensor-core MLP of its tiles =================
+    setmaxnreg_inc<kConsumerRegs>();
+    bar_wait(P.trap, bar, 0, 0);                         // the weight copies
+    const int wt = threadIdx.x & 127, warp = wt >> 5, lane = threadIdx.x & 31, t = lane & 3;
+    const PtsRow* pts = reinterpret_cast<const PtsRow*>(sgen + SM::PTS) + wg * kTilePts;
+    const TapTable* tab = reinterpret_cast<const TapTable*>(sgen + SM::TAPS) + wg;
+    const __half* stage = reinterpret_cast<const __half*>(sgen + SM::STAGE) + wg * kTilePts * kStageRow;
+    const int cb = 1 + kChans * wg;
+    uint32_t k_rows = 0, k_stage = 0, k_taps = 0;       // fills consumed so far: the wait for fill k is on parity k & 1
     const float* sb = reinterpret_cast<const float*>(sgen + SM::BIAS);
     const uint32_t sW = sbase, sH = sbase + SM::HEAD;
-    const int nv = P.nv, N = P.N;
     const int r0 = warp * 16 + (lane >> 2);          // this thread's accumulator rows (points) r0, r0 + 8
-    FIELD_PHASE_INIT();
+    FIELD_PHASE_INIT(wg, wt == 0);
 
-    for (int tile = blockIdx.x * kWarpgroups + wg; tile < P.n_tiles; tile += gridDim.x * kWarpgroups) {
-        const int g = tile / P.sg, q = tile % P.sg;
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");       // the previous tile's rows have been read
-        if (wt < kTilePts) {
-            const int n = wt, rl = n % kTileRays, sl = n / kTileRays;
-            const int slot = g * kTileRays + rl, s = q * kTileSamples + sl;
-            const int slot_c = min(slot, P.n_rays - 1), s_c = min(s, N - 1);
-            const int rid = P.ray_order ? P.ray_order[slot_c] : slot_c;
-            PtsRow pr;
-            pr.rid = rid; pr.sidx = s_c; pr.valid = (slot < P.n_rays) && (s < N);
-            pr.tv = P.tvals[(long long)rid * N + s_c];
-            RayFast rg;
-            ray_fast(P.rays_o + 3 * rid, P.rays_d + 3 * rid, P.far[rid], rg, IS_BG);
-            if (IS_BG) bg_point_fast(rg, pr.tv, P.far_unc, pr.xe, pr.xl);
-            else for (int i = 0; i < 3; ++i) { pr.xe[i] = rg.o[i] + pr.tv * rg.d[i]; pr.xl[i] = pr.xe[i]; }
-            // quirk Q1: the direction of ray (j mod B) of the ray's chunk, j = flat (ray, sample) index inside the chunk
-            const int ch = P.chunk > 0 ? P.chunk : P.n_rays;
-            const int c0 = (rid / ch) * ch;
-            const int Bc = min(ch, P.n_rays - c0);
-            const long long jl = (long long)(rid - c0) * N + s_c;
-            pr.src = c0 + (int)(jl % Bc);
-            pr.pad = 0;
-            pts[n] = pr;
+    for (int tile = blockIdx.x * kConsumers + wg; tile < P.n_tiles; tile += gridDim.x * kConsumers) {
+        // the tile's rows: what the direction term and the stores need, copied so that the producer can move on to the next tile
+        bar_wait(P.trap, bar, cb + kRowsFull, k_rows & 1);
+        FIELD_PHASE(kPhWait);
+        long long gp[2];                                 // output index rid * N + sidx of rows r0, r0 + 8, -1: padding row
+        int src[2];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const PtsRow& pr = pts[r0 + 8 * i];
+            gp[i] = pr.valid ? (long long)pr.rid * N + pr.sidx : -1;
+            src[i] = pr.src;
         }
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+        mbar_arrive(bar + 8u * (cb + kRowsEmpty));
+        ++k_rows;
 #ifdef NEO_FIELD_PHASES
         if (wt == 0) ph_acc[wg][kPhases] += 1ull;
 #endif
-        FIELD_PHASE(0);
-
-        // Encodings: thread wt stages point n = wt % 64, items 15 (wt / 64) .. + 14 of its 30 (3 coordinates x 10 levels) per view.
-        // A-fragment columns 16 ks + 8 h + 2 t + e of rows r0, r0 + 8, as enc_staged reads them (c0 = 16 ks + 8 h, u = 2 t + e).
-        __half* stage = reinterpret_cast<__half*>(tab);
-        const int sn = wt & (kTilePts - 1), shf = wt >> 6;
+        // A-fragment columns 16 ks + 8 h + 2 t + e of rows r0, r0 + 8, as enc_staged reads them (c0 = 16 ks + 8 h, u = 2 t + e)
         uint32_t enc[KS][4];
         auto load_enc = [&](int ks, int h, int j0) {
 #pragma unroll
@@ -581,57 +698,41 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
                                      enc_staged<ICH>(stage, r0 + 8 * i, 16 * ks + 8 * h, 2 * t + 1, j0) << 16;
         };
         if constexpr (IS_BG) {
-            // the s columns 72-92 (enc[4][2..3], enc[5][*]) do not depend on the view: staged as coordinate 0 once per tile
-            const float sx[3] = {pts[sn].tv, 0.f, 0.f};
-            if (shf == 0) stage[stage_slot(sn, 0)] = __float2half_rn(sx[0]);
-            stage_items(stage, sn, sx, 5 * shf, 5);
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+            // the s columns 72-92 (enc[4][2..3], enc[5][*]), staged as coordinate 0 once per tile
+            bar_wait(P.trap, bar, cb + kStageFull, k_stage & 1);
+            FIELD_PHASE(kPhWait);
             load_enc(KS - 2, 1, 3);
             load_enc(KS - 1, 0, 3);
             load_enc(KS - 1, 1, 3);
+            mbar_arrive(bar + 8u * (cb + kStageEmpty));
+            ++k_stage;
         }
+        FIELD_PHASE(kPhRows);
 
         float hacc[40];                                 // folded head: [q (64) | sigma | pad], summed over the views
 #pragma unroll
         for (int i = 0; i < 40; ++i) hacc[i] = 0.f;
 #pragma unroll 1
         for (int v = 0; v < nv; ++v) {
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // the previous view's table (or the s columns) has been read
-            float ce[3];
-            to_camera(vxs[v], pts[sn].xe, ce);
-            if (shf == 0)
-#pragma unroll
-                for (int j = 0; j < 3; ++j) stage[stage_slot(sn, 21 * j)] = __float2half_rn(ce[j]);
-            stage_items(stage, sn, ce, 15 * shf, 15);
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+            bar_wait(P.trap, bar, cb + kStageFull, k_stage & 1);
+            FIELD_PHASE(kPhWait);
 #pragma unroll
             for (int ks = 0; ks < 4; ++ks)
 #pragma unroll
                 for (int h = 0; h < 2; ++h) load_enc(ks, h, 0);
             if constexpr (IS_BG) load_enc(4, 0, 0);                                  // columns 64-71: the last levels of coordinate 2
-            FIELD_PHASE(1);
-            // tap table of this view, built once for both halves: thread wt does point wt % 64, maps 2 (wt / 64) and 2 (wt / 64) + 1
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // the staged encodings have been read
-            {
-                const int m0 = 2 * shf;
-                float cl[3] = {ce[0], ce[1], ce[2]};            // foreground: xl == xe, the lookup point IS the encoded point
-                if constexpr (IS_BG) to_camera(vxs[v], pts[sn].xl, cl);
-                tap_entry(*tab, P.sc, cl, v, sn, m0);
-                tap_entry(*tab, P.sc, cl, v, sn, m0 + 1);
-#ifdef NEO_FIELD_PHASES
-                for (int m = m0; m < m0 + 2; ++m)
-                    for (int k = 0; k < 4; ++k) ph_taps += comp4(tab->w[m][sn], k) != 0.f;
-#endif
-            }
-            asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-            FIELD_PHASE(2);
+            mbar_arrive(bar + 8u * (cb + kStageEmpty));
+            ++k_stage;
+            FIELD_PHASE(kPhRows);
+            bar_wait(P.trap, bar, cb + kTapsFull, k_taps & 1);
+            FIELD_PHASE(kPhWait);
             float acc[64];
             uint32_t a[8][4];
             // layer 0: blend of P0 + W0enc . enc (b0 on the constant-one column)
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;
             blend_maps<0>(acc, P, *tab, r0, t);
-            FIELD_PHASE(3);
+            FIELD_PHASE(kPhBlend0);
             wgmma_fence();
 #pragma unroll
             for (int ks = 0; ks < KS; ++ks) wgmma_rs_n128(acc, enc[ks], wdesc(sW + trunk_off(KE, 0), ks, SLAB));
@@ -652,14 +753,16 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
             // layer 3: blend of P3 + W3h . h2 + W3enc . enc (b3 on the constant-one column)
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-            FIELD_PHASE(4);
+            FIELD_PHASE(kPhLayers);
             blend_maps<1>(acc, P, *tab, r0, t);
-            FIELD_PHASE(5);
+            mbar_arrive(bar + 8u * (cb + kTapsEmpty));                              // the producer may build the next table
+            ++k_taps;
+            FIELD_PHASE(kPhBlend3);
             wgmma_fence();
 #pragma unroll
             for (int ks = 0; ks < 8; ++ks) wgmma_rs_n128(acc, a[ks], wdesc(sW + trunk_off(KE, 3), ks, SLAB));
 #pragma unroll
-            for (int ks = 0; ks < KS; ++ks) wgmma_rs_n128(acc, enc[ks], wdesc(sW + trunk_off(KE, 4), ks, SLAB));
+            for (int ks = 0; ks < KS; ++ks) wgmma_rs_n128(acc, enc[ks], desc_sw128(sW + w3enc_kstep(KE, ks)));
             wgmma_commit();
             wgmma_wait<0>();
             relu_to_frags<128>(acc, a);
@@ -669,11 +772,11 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
             for (int ks = 0; ks < 8; ++ks) wgmma_rs_n80(hacc, a[ks], wdesc(sH + WH_H, ks, 80 * 128));
             wgmma_commit();
             wgmma_wait<0>();
-            FIELD_PHASE(6);
+            FIELD_PHASE(kPhLayer3);
         }
         // direction term: hacc += mean_v(dir_enc_v) . Whead_dir^T, A = the direction fragments of the points' conditioning rays
         {
-            const uint4 d0 = __ldg(P.dir + 4LL * pts[r0].src + t), d1 = __ldg(P.dir + 4LL * pts[r0 + 8].src + t);
+            const uint4 d0 = __ldg(P.dir + 4LL * src[0] + t), d1 = __ldg(P.dir + 4LL * src[1] + t);
             const uint32_t dfr[2][4] = {{d0.x, d1.x, d0.y, d1.y}, {d0.z, d1.z, d0.w, d1.w}};
             wgmma_fence();
 #pragma unroll
@@ -681,15 +784,13 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
             wgmma_commit();
             wgmma_wait<0>();
         }
-        FIELD_PHASE(7);
+        FIELD_PHASE(kPhDir);
         // sigma (column 64: thread t = 0 of each quad), q = relu(hacc + bq) -> colour head 64 x 64 -> relu -> 64 x 3 -> sigmoid
-        const PtsRow pr0 = pts[r0], pr1 = pts[r0 + 8];
         if (t == 0) {
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
-                const PtsRow& pr = i ? pr1 : pr0;
                 const float xs = (hacc[32 + 2 * i] + sb[644]) - 1.0f;                   // model.py:392-393
-                if (pr.valid) P.sigma_out[(long long)pr.rid * N + pr.sidx] = softplus_(xs);
+                if (gp[i] >= 0) P.sigma_out[gp[i]] = softplus_(xs);
             }
         }
         uint32_t qa[4][4];
@@ -726,22 +827,21 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
         if (t < 2) {
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
-                const PtsRow& pr = i ? pr1 : pr0;
-                if (!pr.valid) continue;
-                const long long gp = (long long)pr.rid * N + pr.sidx;
+                if (gp[i] < 0) continue;
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const int c = 2 * t + e;
-                    if (c < 3) P.rgb_out[gp * 3 + c] = rgb_act(o[2 * i + e]);   // model.py:395-397
+                    if (c < 3) P.rgb_out[gp[i] * 3 + c] = rgb_act(o[2 * i + e]);   // model.py:395-397
                 }
             }
         }
-        FIELD_PHASE(8);
+        FIELD_PHASE(kPhColour);
     }
 #ifdef NEO_FIELD_PHASES
-    if (wt == 0)
-        for (int p = 0; p <= kPhases; ++p) atomicAdd(&g_phase_cycles[P.phase_slot][p], ph_acc[wg][p]);
-    atomicAdd(&g_phase_cycles[P.phase_slot][kPhases + 1], ph_taps);
+    if (ph_lead) {
+        for (int p = 0; p < kPhSetup; ++p) atomicAdd(&g_phase_cycles[P.phase_slot][p], ph_acc[ph_unit][p]);
+        atomicAdd(&g_phase_cycles[P.phase_slot][kPhases], ph_acc[ph_unit][kPhases]);
+    }
 #endif
 }
 
@@ -750,7 +850,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-static int* g_trap_host = nullptr;   // host-mapped int[8] written by load_timeout before a trap
+static int* g_trap_host = nullptr;   // host-mapped int[8] written by wait_timeout before a trap
 static int* g_trap_dev = nullptr;
 
 static int trap_buffer() {
@@ -768,8 +868,14 @@ const char* tc_trap_info() {
     static char buf[256];
     if (!g_trap_host || g_trap_host[0] == 0) return "";
     volatile int* t = g_trap_host;
-    snprintf(buf, sizeof(buf), " [TC field kernel: weight load timed out: CTA %d of %d, thread %d, barrier smem 0x%x]",
-             t[1], t[5], t[2], (unsigned)t[3]);
+    static const char* chans[tc::kChans] = {"rows full", "rows empty", "staging full", "staging empty", "tap table full", "tap table empty"};
+    const int id = t[4];
+    char what[64];
+    if (id == 0) snprintf(what, sizeof(what), "weight copies");
+    else if (id > 0 && id < tc::kBars) snprintf(what, sizeof(what), "%s, consumer %d", chans[(id - 1) % tc::kChans], (id - 1) / tc::kChans);
+    else snprintf(what, sizeof(what), "barrier %d", id);
+    snprintf(buf, sizeof(buf), " [TC field kernel: wait on the %s mbarrier timed out: CTA %d of %d, thread %d, barrier smem 0x%x]",
+             what, t[1], t[5], t[2], (unsigned)t[3]);
     return buf;
 }
 
@@ -823,7 +929,7 @@ int tc_scene_create(NeoScene* sc, const NeoMLPParams mlps[4], cudaStream_t s) {
         const uint32_t tbytes = trunk_bytes(m.KE);
         if ((rc = scene_alloc_bytes(sc, &q, tbytes))) return rc;
         m.trunkimg = (const unsigned char*)q;
-        const int nelem = (2 * enc_slabs(m.KE) * 64 + 384) * 128;
+        const int nelem = (2 * m.KE + 384) * 128;
         trunk_img_kernel<<<(nelem + 255) / 256, 256, 0, s>>>(p, m.enc_dim, m.KE, (unsigned char*)q);
         NEO_LAUNCH_CHECK("trunk_img_kernel");
         void* hb = nullptr; void* bb = nullptr;
@@ -900,9 +1006,15 @@ int launch_field_tc(const NeoScene* sc, const NeoRays* rays, const float* far, c
 #ifdef NEO_FIELD_PHASES
     P.phase_slot = g_phase_launches++ % kPhaseSlots;
 #endif
-    const long long ctas = (n_tiles + kWarpgroups - 1) / kWarpgroups;
+    const long long ctas = (n_tiles + kConsumers - 1) / kConsumers;
     const int grid = (int)(ctas < n_sm ? ctas : n_sm);
     auto launch = [&](auto kern, size_t smem) -> int {
+        cudaFuncAttributes fa;
+        NEO_CUDA(cudaFuncGetAttributes(&fa, kern));
+        if (fa.numRegs != kLaunchRegs) {              // the setmaxnreg split would not fit: refuse rather than hang
+            set_error("field_tc_kernel was compiled for %d registers per thread, its warpgroup split needs %d", fa.numRegs, kLaunchRegs);
+            return NEO_ERR_UNSUPPORTED;
+        }
         NEO_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         kern<<<grid, kThreads, smem, s>>>(P);
         return NEO_OK;

@@ -1,5 +1,5 @@
-// PTX wrappers for the sm_90a tensor-core paths (gemm_tc.cu, field_tc.cu): mbarriers, TMA (tensor and bulk copies) and
-// warpgroup MMA (wgmma.mma_async, fp16 operands, fp32 accumulators in registers).
+// PTX wrappers for the sm_90a tensor-core paths (gemm_tc.cu, field_tc.cu): mbarriers, TMA (tensor and bulk copies), warpgroup
+// register reallocation and warpgroup MMA (wgmma.mma_async, fp16 operands, fp32 accumulators in registers).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -37,6 +37,12 @@ __device__ __forceinline__ bool mbar_wait_bounded(uint32_t bar, uint32_t parity)
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if (!mbar_wait_bounded(bar, parity)) asm volatile("trap;");
 }
+// warpgroup register reallocation: every warp of the warpgroup executes the same call; N is a multiple of 8 in 24..256.  ptxas
+// allocates the code that follows within N registers per thread.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 // 2-D TMA tile load (128-byte swizzle set in the tensor map) completing on an mbarrier
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const void* tmap, int c0, int c1, uint32_t bar) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"

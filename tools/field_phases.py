@@ -2,9 +2,11 @@
 
 Builds a copy of the library with -DNEO_FIELD_PHASES (clock64() marks in field_tc_kernel, see csrc/field_tc.cu) into a temporary
 directory, loads it through NEO360_B200_LIB, renders the headline frame of bench.py (same scene, rays, img_wh block order and chunk)
-once to warm up and once measured, and prints for each field launch the cycles per tile (64 points, all views) of every phase,
-summed over the warpgroups, and the texel traffic the blends request: taps of non-zero weight per tile (each one 2 x 256 bytes,
-the P0 and P3 halves of a texel) over the cycles of the two blend phases.  Usage on a GPU box:
+once to warm up and once measured, and prints for each field launch the cycles per tile (64 points, all views) of every phase: the
+consumer warpgroups' phases (blends and MMAs, and their waits for geometry) summed over the two consumers, and the producer's
+phases (points, encodings, tap tables, and its waits for a free slot) summed over its two halves.  Whichever side waits less bounds
+the tile.  It also prints the texel traffic the blends request: taps of non-zero weight per tile (each one 2 x 256 bytes, the P0
+and P3 halves of a texel) over the cycles of the two blend phases.  Usage on a GPU box:
 
   python tools/field_phases.py [--lib PATH] [--clock-mhz F]
       --lib: an instrumented library built beforehand, e.g. from another source tree
@@ -21,8 +23,10 @@ import tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-PHASES = ("tile setup", "camera + encodings", "tap table", "blend P0", "layers 0-2", "blend P3", "layer 3 + head", "direction term",
-          "colour head + stores")
+CONSUMER = ("waiting for geometry", "rows + encodings", "blend P0", "layers 0-2", "blend P3", "layer 3 + head", "direction term",
+            "colour head + stores")
+PRODUCER = ("setup", "encodings", "tap table", "waiting for a free slot")
+PHASES = CONSUMER + PRODUCER                                         # column order of neo_field_phases_read (csrc/field_tc.cu)
 LAUNCHES = ("fg coarse", "bg coarse", "fg fine", "bg fine")      # order of the field launches of one frame (render.cu)
 MAX_LAUNCHES = 64
 
@@ -82,23 +86,28 @@ def main():
     name = torch.cuda.get_device_name(0)
     n_sm = torch.cuda.get_device_properties(0).multi_processor_count
     print(f"{name}; library {os.environ['NEO360_B200_LIB']}; {n} field launches; cycles per tile (64 points x {Bm.NV} views) per phase")
-    print(f"{'launch':<12}{'tiles':>9}" + "".join(f"{p:>22}" for p in PHASES) + f"{'total':>12}")
     rows = []
-    for li in range(n):
-        row = buf[li * cols:(li + 1) * cols]
-        tiles = max(row[-2], 1)
-        per = [c / tiles for c in row[:-2]]
-        rows.append((tiles, per, row[-1] / tiles))
-        print(f"{LAUNCHES[li % 4]:<12}{row[-2]:>9}" + "".join(f"{x:>14.0f} ({x / sum(per):4.0%})" for x in per) + f"{sum(per):>12.0f}")
+    for side, names, lo in (("consumers", CONSUMER, 0), ("producer", PRODUCER, len(CONSUMER))):
+        print(f"{side}:")
+        print(f"{'launch':<12}{'tiles':>9}" + "".join(f"{p:>24}" for p in names) + f"{'total':>12}")
+        for li in range(n):
+            row = buf[li * cols:(li + 1) * cols]
+            tiles = max(row[-2], 1)
+            per = [c / tiles for c in row[lo:lo + len(names)]]
+            if lo == 0:
+                rows.append((tiles, [c / tiles for c in row[:-2]], row[-1] / tiles))
+            print(f"{LAUNCHES[li % 4]:<12}{row[-2]:>9}" + "".join(f"{x:>16.0f} ({x / max(sum(per), 1):4.0%})" for x in per)
+                  + f"{sum(per):>12.0f}")
     # request rate of the blends: a warpgroup's texel bytes per tile over its blend cycles per tile; the GPU figure assumes both
     # warpgroups of every SM blend at once (an upper bound), the launch figure spreads the bytes over the whole tile
-    print(f"texel requests ({n_sm} SMs, 2 warpgroups each, SM clock {args.clock_mhz:.0f} MHz):")
+    print(f"texel requests ({n_sm} SMs, 2 consumer warpgroups each, SM clock {args.clock_mhz:.0f} MHz):")
     print(f"{'launch':<12}{'taps/tile':>10}{'KB/tile':>9}{'B/cycle in blends':>19}{'GPU TB/s in blends':>20}{'GPU TB/s over tile':>20}")
     for li, (tiles, per, taps) in enumerate(rows):
         by = taps * 512
         blend = per[PHASES.index("blend P0")] + per[PHASES.index("blend P3")]
         scale = 2 * n_sm * args.clock_mhz * 1e6 / 1e12
-        print(f"{LAUNCHES[li % 4]:<12}{taps:>10.0f}{by / 1024:>9.0f}{by / blend:>19.1f}{by / blend * scale:>20.2f}{by / sum(per) * scale:>20.2f}")
+        tile = sum(per[:len(CONSUMER)])
+        print(f"{LAUNCHES[li % 4]:<12}{taps:>10.0f}{by / 1024:>9.0f}{by / blend:>19.1f}{by / blend * scale:>20.2f}{by / tile * scale:>20.2f}")
 
 
 if __name__ == "__main__":
