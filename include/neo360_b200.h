@@ -274,6 +274,42 @@ int neo_index_local_bwd(const NeoScene* scene, const float* pts, int M, const fl
 int neo_field_eval(const NeoScene* scene, const NeoRays* rays, const float* far, const float* t_vals, int N,
                    int mlp_index, int precision, float* rgb, float* sigma, void* stream);
 
+/* ---- geometry export: density grid, marching tetrahedra, normals (csrc/mesh.cu, neo360_b200/mesh.py) ----
+ * A lattice of nx * ny * nz points, each axis >= 2 points, at most 2^28 points in all.  Point (i, j, k) lies at
+ * (origin[0] + i * step[0], origin[1] + j * step[1], origin[2] + k * step[2]), each product and sum rounded to nearest in fp32.
+ * Grid values (sigma) are fp32, laid out (nz, ny, nx) with x fastest; row r = k * ny + j is the x-row of points (*, j, k).
+ * Every call validates its arguments before any launch and returns NEO_ERR_INVALID on a bad one. */
+typedef struct {
+    int nx, ny, nz;
+    float origin[3];          /* x, y, z of point (0, 0, 0): finite */
+    float step[3];            /* spacing along x, y, z: finite and > 0 */
+} NeoGrid;
+/* Rays that make neo_field_eval evaluate a foreground MLP at the lattice points of rows [row0, row0 + n_rows): row r gets
+ * rays_o = (origin[0], y_j, z_k), dirs = (1, 0, 0) (pass it as rays_d and viewdirs) and t_vals (n_rows, nx) = i * step[0], so that
+ * o + t d is the lattice point bit for bit.  rays_o and dirs are (n_rows, 3). */
+int neo_grid_rays(const NeoGrid* grid, long long row0, int n_rows, float* rays_o, float* dirs, float* t_vals, void* stream);
+/* sigma_rows (n_rows, nx), rows [row0, row0 + n_rows) of a grid: sets sigma = 0 at every point with x*x + y*y + z*z > 1 (fp32, in that
+ * order).  The foreground branch is only sampled inside the unit sphere, so the density grid defines sigma = 0 outside it. */
+int neo_grid_mask_sphere(const NeoGrid* grid, long long row0, int n_rows, float* sigma_rows, void* stream);
+/* Marching tetrahedra over a grid (sigma, (nz, ny, nx)).  Inside means sigma >= iso (a NaN is outside).  Every cell is split into the 6
+ * Kuhn tetrahedra sharing its main diagonal; point p owns the 7 edges from p to p + e, e in type order (1,0,0) (0,1,0) (0,0,1) (1,1,0)
+ * (1,0,1) (0,1,1) (1,1,1).  A vertex lies on each owned edge whose end points are on different sides, at
+ * w = (iso - s_a) / (s_b - s_a), x = p_a + w * (p_b - p_a) per coordinate (a = p, b = p + e; fp32, each operation rounded to nearest).
+ * Vertex ids follow (point, edge type) order; faces (int32 vertex ids) follow (cell, tetrahedron, triangle) order, cells in point order,
+ * and wind counter-clockwise seen from outside (lower sigma).  No atomics: two calls give identical bits.
+ * Workspace: neo_mt_workspace_bytes(grid) bytes (0 = bad grid), 256-byte aligned, caller-owned.  neo_mt_count writes V and F to
+ * *n_verts / *n_faces (HOST ints) and synchronises `stream` once; NEO_ERR_UNSUPPORTED when either exceeds 2^31 - 1.
+ * neo_mt_emit reads the block offsets neo_mt_count left in the workspace (same sigma, grid, iso and workspace, same stream), writes
+ * verts (n_verts, 3) and faces (n_faces, 3), and never writes past n_verts / n_faces. */
+size_t neo_mt_workspace_bytes(const NeoGrid* grid);
+int neo_mt_count(const float* sigma, const NeoGrid* grid, float iso, void* workspace, size_t workspace_bytes, int* n_verts, int* n_faces,
+                 void* stream);
+int neo_mt_emit(const float* sigma, const NeoGrid* grid, float iso, void* workspace, size_t workspace_bytes, float* verts, int n_verts,
+                int* faces, int n_faces, void* stream);
+/* normals (n_verts, 3) = -grad sigma / |grad sigma| at each vertex (0 where the gradient is 0): the gradient at the lattice points by central
+ * differences (one-sided on the grid's faces), trilinearly interpolated in the cell that holds the vertex (clamped into the grid). */
+int neo_grid_normals(const float* sigma, const NeoGrid* grid, const float* verts, int n_verts, float* normals, void* stream);
+
 /* ---- vanilla two-level NeRF (SURVEY.md section 8(a) row a17): models/vanilla_nerf/model.py:44-216 ---- */
 typedef struct {
     const float* w[8];        /* pts_linears.{0..7}.weight: (256,63) (256,256)x4 (256,319) (256,256)x2 */

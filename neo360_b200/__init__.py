@@ -2,7 +2,7 @@
 `model(rays, randomized, white_bkgd, near, far, out_depth)` call surface.  See DESIGN.md / INTEGRATION.md."""
 from . import synth  # noqa: F401
 
-__all__ = ["NeRF_TP", "NeRFPPMLP", "PixelNeRF", "ops", "synth", "release_cached"]
+__all__ = ["NeRF_TP", "NeRFPPMLP", "PixelNeRF", "ops", "mesh", "synth", "release_cached"]
 
 
 def release_cached() -> None:
@@ -18,7 +18,7 @@ def __getattr__(name):
     if name == "PixelNeRF":
         from . import pixelnerf
         return pixelnerf.PixelNeRF
-    if name == "ops":
+    if name in ("ops", "mesh"):
         import importlib
-        return importlib.import_module(".ops", __name__)
+        return importlib.import_module("." + name, __name__)
     raise AttributeError(name)

@@ -89,6 +89,10 @@ class NeoMipOut(C.Structure):
     _fields_ = [(n, C.c_void_p * 3) for n in MIP_OUT_FIELDS]
 
 
+class NeoGrid(C.Structure):
+    _fields_ = [("nx", C.c_int), ("ny", C.c_int), ("nz", C.c_int), ("origin", C.c_float * 3), ("step", C.c_float * 3)]
+
+
 class NeoGridEncoderParams(C.Structure):
     _fields_ = [("fc_w", C.c_void_p * 3), ("fc_b", C.c_void_p * 3)] + \
                [(f"agg_{pl}_{n}", C.c_void_p) for pl in ("xz", "yz", "xy") for n in ("w0", "b0", "w1", "b1")]
@@ -130,6 +134,14 @@ SYMBOLS = {
     "neo_index_grid_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_index_local_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_field_eval": (C.c_int, [C.c_void_p, C.POINTER(NeoRays), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "neo_grid_rays": (C.c_int, [C.POINTER(NeoGrid), C.c_longlong, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "neo_grid_mask_sphere": (C.c_int, [C.POINTER(NeoGrid), C.c_longlong, C.c_int, C.c_void_p, C.c_void_p]),
+    "neo_mt_workspace_bytes": (C.c_size_t, [C.POINTER(NeoGrid)]),
+    "neo_mt_count": (C.c_int, [C.c_void_p, C.POINTER(NeoGrid), C.c_float, C.c_void_p, C.c_size_t, C.POINTER(C.c_int), C.POINTER(C.c_int),
+                               C.c_void_p]),
+    "neo_mt_emit": (C.c_int, [C.c_void_p, C.POINTER(NeoGrid), C.c_float, C.c_void_p, C.c_size_t, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                              C.c_void_p]),
+    "neo_grid_normals": (C.c_int, [C.c_void_p, C.POINTER(NeoGrid), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "neo_vanilla_create": (C.c_int, [C.POINTER(NeoVanillaMLPParams), C.POINTER(C.c_void_p), C.c_void_p]),
     "neo_vanilla_free": (None, [C.c_void_p]),
     "neo_vanilla_workspace_bytes": (C.c_size_t, [C.c_int, C.POINTER(NeoVanillaCfg)]),

@@ -231,3 +231,36 @@ def store_depth_raw(dirpath: str, depths: Sequence[torch.Tensor], name: str) -> 
         np.savez_compressed(path, d.detach().cpu().numpy())
         paths.append(path)
     return paths
+
+
+def write_ply(path: str, mesh: dict) -> str:
+    """A mesh dict (extract_mesh: verts (V,3), faces (F,3), optional normals (V,3) and colors (V,3) in [0, 1]) as a binary little-endian
+    PLY: vertex x y z [nx ny nz] float32, [red green blue] uchar = round(255 * clip(color, 0, 1)), faces as a uchar-counted list of int32
+    vertex_indices."""
+    v = mesh["verts"].detach().cpu().numpy().astype("<f4").reshape(-1, 3)
+    f = mesh["faces"].detach().cpu().numpy().astype("<i4").reshape(-1, 3)
+    fields = [("x", "<f4"), ("y", "<f4"), ("z", "<f4")]
+    cols = {"x": v[:, 0], "y": v[:, 1], "z": v[:, 2]}
+    if mesh.get("normals") is not None:
+        n = mesh["normals"].detach().cpu().numpy().astype("<f4").reshape(-1, 3)
+        fields += [("nx", "<f4"), ("ny", "<f4"), ("nz", "<f4")]
+        cols.update(nx=n[:, 0], ny=n[:, 1], nz=n[:, 2])
+    if mesh.get("colors") is not None:
+        c = np.rint(np.clip(mesh["colors"].detach().cpu().numpy().reshape(-1, 3), 0.0, 1.0) * 255.0).astype(np.uint8)
+        fields += [("red", "u1"), ("green", "u1"), ("blue", "u1")]
+        cols.update(red=c[:, 0], green=c[:, 1], blue=c[:, 2])
+    vert = np.empty(v.shape[0], dtype=fields)
+    for k, col in cols.items():
+        vert[k] = col
+    face = np.empty(f.shape[0], dtype=[("n", "u1"), ("i", "<i4", (3,))])
+    face["n"] = 3
+    face["i"] = f
+    ply_type = {"<f4": "float", "u1": "uchar"}
+    header = ["ply", "format binary_little_endian 1.0", f"element vertex {v.shape[0]}"]
+    header += [f"property {ply_type[t]} {k}" for k, t in fields]
+    header += [f"element face {f.shape[0]}", "property list uchar int vertex_indices", "end_header"]
+    with open(path, "wb") as fh:
+        fh.write(("\n".join(header) + "\n").encode("ascii"))
+        fh.write(vert.tobytes())
+        fh.write(face.tobytes())
+    return path

@@ -174,7 +174,8 @@ class NeRF_TP(nn.Module):
         return (src is not None and len(src[0]) == len(tensors) and all(a is b for a, b in zip(src[0], tensors))
                 and src[1] == tuple(t._version for t in tensors))
 
-    def _ensure_scene(self, rays):
+    def _ensure_scene(self, rays, precision: Optional[str] = None):
+        precision = precision or self.precision
         if all(k in rays for k in ("planes_xz", "planes_xy", "planes_yz", "latent")):
             keyed = tuple(rays[k] for k in ("planes_xz", "planes_xy", "planes_yz", "latent", "src_poses"))
             if not self._same_source(keyed):
@@ -193,15 +194,17 @@ class NeRF_TP(nn.Module):
                 self._scene_src = (keyed, tuple(t._version for t in keyed))
         if self._scene is None:
             raise RuntimeError("no scene: call set_scene(...) or pass planes_*/latent in `rays`, or give an encoder")
-        need = 1 << PRECISIONS[self.precision]
+        need = 1 << PRECISIONS[precision]
         if self._param_key != self._params_version() or not (self._scene.mask & need):
             # the packed weights (fp32 transposes, swizzled weight images, W0/W3-projected feature maps) are stale, or the scene was last built for
             # another use (a training step leaves a cameras-only scene): re-pack from the kept inputs
             src = self._scene_src
             a = self._scene_inputs
             prec = a[8]
-            if prec is not None and not any(PRECISIONS[p] == PRECISIONS[self.precision] for p in prec):
-                prec = list(prec) + [self.precision]
+            if prec is None and precision != self.precision:
+                prec = [self.precision]
+            if prec is not None and not any(PRECISIONS[p] == PRECISIONS[precision] for p in prec):
+                prec = list(prec) + [precision]
             self.set_scene(*a[:8], precisions=prec)
             self._scene_src = src
         return self._scene
@@ -350,6 +353,12 @@ class NeRF_TP(nn.Module):
                                             PRECISIONS[precision or self.precision], L.ptr(rgb), L.ptr(sig),
                                             torch.cuda.current_stream().cuda_stream))
         return rgb, sig
+
+    def density_grid(self, resolution, bbox=((-1.0, -1.0, -1.0), (1.0, 1.0, 1.0)), level: int = 1, precision: Optional[str] = None,
+                     slab_rays: int = 16384, batch: Optional[Dict[str, torch.Tensor]] = None) -> torch.Tensor:
+        """sigma of the foreground MLP of `level` on an (R_z, R_y, R_x) lattice over `bbox`; see neo360_b200.mesh.density_grid."""
+        from . import mesh
+        return mesh.density_grid(self, resolution, bbox, level, precision, slab_rays, batch)
 
     def check(self):
         """Synchronise and surface deferred device-side errors (the reference's asserts, helper.py:271,426)."""
