@@ -10,6 +10,7 @@ seeded run picks the same pixels; it is the only per-step host-to-device copy (8
 Disk I/O, PIL/cv2 decoding and scene bookkeeping are out of scope (SURVEY.md section 2 row 19: OUT); callers hand in decoded tensors."""
 from __future__ import annotations
 
+import random
 from typing import Dict, Optional
 
 import numpy as np
@@ -85,3 +86,41 @@ def patch_batch(views: TargetViews, src: Dict[str, torch.Tensor], view: int, x: 
     if y is None:
         y = np.random.randint(0, views.W - PATCH + 1)
     return train_batch(views, src, pix_inds=patch_pix_inds(view, int(x), int(y), views.H, views.W))
+
+
+def draw_source_view(n_views: int, H: int, W: int, view: Optional[int] = None, finetune_lpips: bool = False,
+                     ray_batch_size: int = RAY_BATCH_SIZE, generator: Optional[torch.Generator] = None):
+    """The host draws of one test-time optimisation sample, in the reference's order (nerds360_ae.py:540-551, 598-673): the target
+    view's position among the NV source views with `random.sample(ids, 1)[0]` from Python's global generator (skipped when `view` is
+    given), then either `torch.randint(0, H * W, (ray_batch_size,))` pixels of that view, returned as flat indices into the (NV,H,W)
+    stack, or with `finetune_lpips` the 30x30 patch origin (x, y) drawn as `patch_batch` draws it.  `random.sample` consumes the
+    generator the same way for any population of NV items, so the position drawn is the one the reference draws from its ids.
+    Returns (view, pix_inds) or (view, (x, y))."""
+    if view is None:
+        view = random.sample(range(n_views), 1)[0]
+    elif not 0 <= view < n_views:
+        raise ValueError(f"view {view} of {n_views}")
+    if finetune_lpips:
+        x = np.random.randint(0, H - PATCH + 1)
+        y = np.random.randint(0, W - PATCH + 1)
+        return view, (int(x), int(y))
+    return view, view * H * W + torch.randint(0, H * W, (ray_batch_size,), generator=generator)
+
+
+def source_view_batch(views: TargetViews, src: Dict[str, torch.Tensor], view: Optional[int] = None, finetune_lpips: bool = False,
+                      ray_batch_size: int = RAY_BATCH_SIZE, generator: Optional[torch.Generator] = None) -> Dict[str, torch.Tensor]:
+    """One test-time optimisation sample (--is_optimize, nerds360_ae.py:540-551, 598-673) with the keys of `train_batch`: rays and colours
+    of one of the scene's own source views.  `views` holds the NV source images in [0,1] (not normalised) with their poses; `src` the
+    source-view entries as the dataset produces them (src_imgs normalised).  The view and its pixels (or, with `finetune_lpips`, its
+    30x30 patch) are drawn by `draw_source_view`.  NeRDS360's source views share one focal, as `TargetViews` has one: a `src_focal`
+    with another value raises."""
+    if views.T != src["src_poses"].shape[0]:
+        raise ValueError(f"{views.T} source images for {src['src_poses'].shape[0]} source poses")
+    focal = float(torch.tensor(views.focal, dtype=torch.float32))
+    focals = src["src_focal"].reshape(-1).tolist()
+    if any(f != focal for f in focals):
+        raise ValueError(f"the source views must share one focal ({views.focal}), got {focals}")
+    view, draw = draw_source_view(views.T, views.H, views.W, view, finetune_lpips, ray_batch_size, generator)
+    if finetune_lpips:
+        return patch_batch(views, src, view, *draw)
+    return train_batch(views, src, pix_inds=draw)

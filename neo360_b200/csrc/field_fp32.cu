@@ -7,8 +7,13 @@
 
 namespace neo {
 
-constexpr int kP = 8;          // points per CTA
 constexpr int kThreads = 128;  // one thread per hidden unit
+constexpr int kMaxInDim = 4 * (2 * kPosDeg + 1) + kLocalCh + kWorldCh;   // background MLP: [pos_enc(xyz, 1/r) | local | world]
+constexpr size_t kSmemLimit = 227 * 1024;                               // opt-in dynamic shared memory per block on sm_90
+
+// Points per CTA.  Each point has one row per view in shared memory, so the tile shrinks from 8 to 4 points above 6 views to stay
+// within kSmemLimit.  A point's arithmetic does not depend on the tile: only which CTA evaluates it changes.
+__host__ __device__ constexpr int points_per_cta(int nv) { return nv <= 6 ? 8 : 4; }
 
 struct RowGeo {
     float enc_in[4];    // camera-frame position fed to pos_enc (+ 1/r for bg)
@@ -24,6 +29,7 @@ field_fp32_kernel(SceneDev sc, MLPFp32 mlp, const float* __restrict__ rays_o, co
                   const float* __restrict__ viewdirs, const float* __restrict__ far, const float* __restrict__ tvals,
                   int n_rays, int N, int chunk, int is_bg, float far_unc, float* __restrict__ rgb_out,
                   float* __restrict__ sigma_out) {
+    constexpr int kP = points_per_cta(NV);
     constexpr int ROWS = NV * kP;
     extern __shared__ __align__(16) float smem[];
     const int in_dim = mlp.in_dim;                 // enc + 512 + 128
@@ -214,16 +220,20 @@ field_fp32_kernel(SceneDev sc, MLPFp32 mlp, const float* __restrict__ rays_o, co
     }
 }
 
-static size_t field_fp32_smem(int nv, int in_dim) {
-    int rows = nv * kP;
-    int ldx = (in_dim + 3) / 4 * 4 + 4;
-    size_t fl = (size_t)rows * ldx + 2 * (size_t)rows * (kHidden + 4) + (size_t)rows * 28 + 2 * kP * 68;
+static constexpr size_t field_fp32_smem(int nv, int in_dim) {
+    const int kP = points_per_cta(nv);
+    const int rows = nv * kP;
+    const int ldx = (in_dim + 3) / 4 * 4 + 4;
+    const size_t fl = (size_t)rows * ldx + 2 * (size_t)rows * (kHidden + 4) + (size_t)rows * 28 + 2 * kP * 68;
     return fl * sizeof(float) + (size_t)rows * sizeof(RowGeo);
 }
 
 template <int NV>
 static int launch_nv(const NeoScene* sc, const NeoRays* rays, const float* far, const float* t, int N, int mi,
                      float* rgb, float* sigma, cudaStream_t s) {
+    constexpr int kP = points_per_cta(NV);
+    static_assert(field_fp32_smem(NV, kMaxInDim) <= kSmemLimit, "field_fp32_kernel tile exceeds shared memory");
+    static_assert(NV * kP <= kThreads && 3 * kP <= kThreads, "phase A and the rgb head need one thread per row");
     const MLPFp32& m = sc->mlp32[mi];
     size_t smem = field_fp32_smem(NV, m.in_dim);
     NEO_CUDA(cudaFuncSetAttribute(field_fp32_kernel<NV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -243,8 +253,13 @@ int launch_field_fp32(const NeoScene* sc, const NeoRays* rays, const float* far,
         case 2: return launch_nv<2>(sc, rays, far, t, N, mlp_index, rgb, sigma, s);
         case 3: return launch_nv<3>(sc, rays, far, t, N, mlp_index, rgb, sigma, s);
         case 4: return launch_nv<4>(sc, rays, far, t, N, mlp_index, rgb, sigma, s);
+        case 5: return launch_nv<5>(sc, rays, far, t, N, mlp_index, rgb, sigma, s);
+        case 6: return launch_nv<6>(sc, rays, far, t, N, mlp_index, rgb, sigma, s);
+        case 7: return launch_nv<7>(sc, rays, far, t, N, mlp_index, rgb, sigma, s);
+        case 8: return launch_nv<8>(sc, rays, far, t, N, mlp_index, rgb, sigma, s);
     }
-    set_error("NEO_PREC_FP32 supports 1..4 source views (got %d)", sc->dev.nv);
+    static_assert(kMaxViews == 8, "instantiate field_fp32_kernel for every view count up to kMaxViews");
+    set_error("NEO_PREC_FP32 supports 1..%d source views (got %d)", kMaxViews, sc->dev.nv);
     return NEO_ERR_UNSUPPORTED;
 }
 

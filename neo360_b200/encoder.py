@@ -354,6 +354,7 @@ class GridEncoder(nn.Module):
                   self.pillar_aggregator_xz, self.pillar_aggregator_yz, self.pillar_aggregator_xy):
             m.apply(_init_linear_kaiming)
         self._ws = None
+        self._latent_key = None         # (images, their version, the ResNet's tensor versions, latent, latent_scaling) of the cached latent
 
     @property
     def train_precision(self) -> str:
@@ -458,10 +459,31 @@ class GridEncoder(nn.Module):
                                                self._ws.data_ptr(), self._ws.numel(), torch.cuda.current_stream().cuda_stream))
         return out[0], out[1], out[2]
 
+    def _spatial_latent(self, images):
+        """spatial_encoder(images).  A frozen spatial encoder in eval mode (test-time optimisation, `training.test_time_optimizer`) is a
+        fixed function of its input, so it runs once per set of `images`: compared by identity and in-place version, as
+        NeRF_TP._same_source compares its sources, and by the version of every ResNet parameter and buffer (load_state_dict).  The
+        cached latent is put back in `spatial_encoder.latent`, where the renderer reads it."""
+        se = self.spatial_encoder
+        frozen = not se.training and not images.requires_grad and not any(p.requires_grad for p in se.parameters())
+        if not frozen:
+            self._latent_key = None
+            return se(images)
+        key = (images, images._version, tuple((t.data_ptr(), t._version) for t in list(se.parameters()) + list(se.buffers())
+                                              if t is not se.latent and t is not se.latent_scaling))
+        old = self._latent_key
+        if old is not None and old[0] is images and old[1:3] == key[1:3]:
+            se.latent, se.latent_scaling = old[3], old[4]
+            return old[3]
+        with torch.no_grad():
+            latent = se(images)
+        self._latent_key = key + (latent, se.latent_scaling)
+        return latent
+
     def forward(self, images, poses, focal, c):
         """images (NV,3,H,W), poses (NV,4,4) camera-to-world, focal (NV,), c (NV,2) -> scene_grid_xz, scene_grid_xy, scene_grid_yz (NV,128,120,160)."""
         NV, _, H, W = images.shape
-        latent = self.spatial_encoder(images)
+        latent = self._spatial_latent(images)
         trained = [self.depth_fc, self.pillar_aggregator_xz, self.pillar_aggregator_yz, self.pillar_aggregator_xy]
         needs_grad = torch.is_grad_enabled() and (latent.requires_grad or any(q.requires_grad for m in trained for q in m.parameters()))
         if needs_grad:

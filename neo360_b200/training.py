@@ -644,6 +644,40 @@ def setup_finetune_lpips(net) -> List[torch.nn.Parameter]:
     return [p for p in net.parameters() if p.requires_grad]
 
 
+TEST_TIME_LR = 5e-6      # model.py:960-967: 5e-6 when the run resumes from a checkpoint, which run.py:84-92 always does
+
+
+def test_time_optimizer(net, lr: float = TEST_TIME_LR, eval_modules: bool = True) -> torch.optim.Adam:
+    """configure_optimizers for --is_optimize, the reference's test-time optimisation of a trained model on the source views of a new scene
+    (model.py:957-981): the encoder's spatial_encoder (ResNet-34) is frozen, and Adam with betas (0.9, 0.999) runs over every parameter of
+    `net` (the frozen ones never get a gradient).  optimizer_step then steps it with no learning-rate schedule and no gradient clipping
+    (model.py:999-1000): see `test_time_step`.
+    `eval_modules` (default True, configure_optimizers' evident intent) puts the spatial_encoder and every BatchNorm2d in eval mode, so
+    their running statistics stay as trained and GridEncoder runs the frozen ResNet once per set of source images.  False leaves the
+    modes alone: that is what the reference gets if its training loop calls `model.train()` after configure_optimizers (DESIGN.md
+    section 8)."""
+    if getattr(net, "encoder", None) is not None:
+        net.encoder.spatial_encoder.requires_grad_(False)
+    if eval_modules:
+        setup_finetune_lpips(net)
+    return torch.optim.Adam(net.parameters(), lr=lr, betas=(0.9, 0.999))
+
+
+def test_time_step(net, opt: torch.optim.Optimizer, batch: Dict[str, Tensor], lpips_model=None) -> Tensor:
+    """One step of the reference's test-time optimisation (training_step, model.py:697-820, and the --is_optimize branch of
+    optimizer_step, model.py:999-1000): randomized forward, `training_loss` (with `lpips_model` for a --finetune_lpips patch batch),
+    backward and a plain optimiser step: no schedule, no clip.  Returns the loss."""
+    ret = net(batch, True, False, None, None, out_depth=False)
+    loss = training_loss(ret, batch["target"], lpips_model=lpips_model)
+    opt.zero_grad(set_to_none=True)
+    loss.backward()
+    opt.step()
+    return loss.detach()
+
+
+test_time_optimizer.__test__ = test_time_step.__test__ = False      # library functions, not pytest tests, when a test module imports them
+
+
 def training_loss(ret, target: Tensor, dist_weight: float = 0.01, lpips_model=None) -> Tensor:
     """MSE of both levels + distortion regulariser on the fine level (model.py:740-748, 1246-1260).  With `lpips_model` (the
     --finetune_lpips variant, model.py:750-755) the LPIPS loss of both levels' patch colours is added before the regulariser."""
