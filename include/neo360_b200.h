@@ -344,6 +344,15 @@ size_t neo_vanilla_workspace_bytes(int n_rays, const NeoVanillaCfg* cfg);
 /* NeRF.forward (models/vanilla_nerf/model.py:154-216); rays->chunk is ignored (no cross-ray coupling in this model) */
 int neo_vanilla_render_fwd(const NeoVanilla* v, const NeoRays* rays, const NeoVanillaCfg* cfg, NeoVanillaOut* out,
                            void* workspace, size_t workspace_bytes, void* stream);
+/* The NeRFMLP of one level (0 coarse, 1 fine) at caller-given points: sample s of ray b is rays_o[b] + t_vals[b, s] * viewdirs[b], as the
+ * render casts it (rays_d is not read), and its direction input is viewdirs[b].  t_vals (n_rays, N) -> activated rgb (n_rays, N, 3) and
+ * sigma (n_rays, N), the render's `rgb_s` / `sigma` at its own samples.  The render runs the same code per level, so the two give the same
+ * bits.  precision NEO_PREC_FP32 (the fused field kernel) or NEO_PREC_TC (the fp16 layer chain).  Workspace: 256-byte aligned,
+ * neo_vanilla_field_workspace_bytes(n_rays * N, precision) bytes; NEO_PREC_FP32 needs none (0 bytes, ws may be NULL).
+ * n_rays * N < 2^31.  sigma does not depend on viewdirs. */
+size_t neo_vanilla_field_workspace_bytes(long long n_points, int precision);
+int neo_vanilla_field_eval(const NeoVanilla* v, const NeoRays* rays, const float* t_vals, int N, int level, int precision, float* rgb,
+                           float* sigma, void* ws, size_t ws_bytes, void* stream);
 /* Stages of the differentiable NeRF.forward (training, models/vanilla_nerf/model.py:154-216 under autograd; neo360_b200/vanilla.py).
  * Hand-written: sampling, encodings, compositing forward and backward; the NeRFMLP dense layers are differentiated by the host framework.
  * The fine level resamples with neo_sample_pdf(rays_o, viewdirs, NULL, t0, weights0, n, n_coarse+1, n_fine, 1, 0, u1, t1, NULL, NULL)
@@ -473,6 +482,16 @@ int neo_mip_composite(const float* raw_density, const float* raw_rgb, const floa
 int neo_mip_composite_bwd(const float* raw_density, const float* raw_rgb, const float* tdist, const float* rays_d, int n_rays, int N,
                           const float* g_rgb, const float* g_weights, const float* g_density, const float* g_rgb_s, float* d_raw_density,
                           float* d_raw_rgb, void* stream);
+/* One MLP of Mip-NeRF 360 (level 0, 1: PropMLP; 2: NeRFMLP) at caller-given points.  The MLP reads a Gaussian: here its mean is the point
+ * rays_o[b] + t_vals[b, s] * viewdirs[b] (fp32, each operation rounded; rays_d is not read) and its covariance diag(var), var >= 0 per
+ * axis.  The Gaussian goes through the render's own encoding (contraction with its Jacobian, 21-direction lift, 12-octave IPE), then the
+ * render's layer chain in `precision` (fp32 SGEMMs or fp16 tensor-core GEMMs) with viewdirs[b] as the direction input.  Outputs: density
+ * (n_rays, N) = softplus(raw - 1) and, at level 2 only, rgb (n_rays, N, 3) = 1.002 sigmoid(raw) - 0.001, or NULL.  A non-NULL rgb at a
+ * proposal level is an error: those MLPs have no colour head.  mlps[3] as for neo_mip_render_fwd; only mlps[level] is read.  Workspace:
+ * neo_mip_field_workspace_bytes(n_rays * N, mlps[level].width, precision) bytes, 256-byte aligned (0 = invalid sizes).  n_rays * N < 2^31. */
+size_t neo_mip_field_workspace_bytes(long long n_points, int width, int precision);
+int neo_mip_field_eval(const NeoMipMLPParams mlps[3], int level, const NeoRays* rays, const float* t_vals, int N, const float var[3],
+                       int precision, float* rgb, float* density, void* ws, size_t ws_bytes, void* stream);
 
 /* ---- tri-plane builder, dense part (SURVEY.md section 8(f1)): models/neo360/encoder_tp_fusion_conv.py:472-597 between the ResNet feature
  * extractor and the floor-plan conv stacks (both stay in the host framework).  64^3 world grid x nv views: latent lookup, DepthPillarEncoder

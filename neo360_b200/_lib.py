@@ -146,6 +146,9 @@ SYMBOLS = {
     "neo_vanilla_free": (None, [C.c_void_p]),
     "neo_vanilla_workspace_bytes": (C.c_size_t, [C.c_int, C.POINTER(NeoVanillaCfg)]),
     "neo_vanilla_render_fwd": (C.c_int, [C.c_void_p, C.POINTER(NeoRays), C.POINTER(NeoVanillaCfg), C.POINTER(NeoVanillaOut), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "neo_vanilla_field_workspace_bytes": (C.c_size_t, [C.c_longlong, C.c_int]),
+    "neo_vanilla_field_eval": (C.c_int, [C.c_void_p, C.POINTER(NeoRays), C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_size_t, C.c_void_p]),
     "neo_vanilla_sample_along_rays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_vanilla_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_pixelnerf_field": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(NeoPixelMLPParams), C.POINTER(NeoRays), C.c_void_p, C.c_int, C.c_void_p,
@@ -163,6 +166,9 @@ SYMBOLS = {
     "neo_mip_encode": (C.c_int, [C.c_void_p] * 6 + [C.c_int] * 2 + [C.c_void_p] * 3),
     "neo_mip_composite": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 2 + [C.c_void_p] * 5),
     "neo_mip_composite_bwd": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 2 + [C.c_void_p] * 7),
+    "neo_mip_field_workspace_bytes": (C.c_size_t, [C.c_longlong, C.c_int, C.c_int]),
+    "neo_mip_field_eval": (C.c_int, [C.POINTER(NeoMipMLPParams), C.c_int, C.POINTER(NeoRays), C.c_void_p, C.c_int, C.POINTER(C.c_float), C.c_int,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "neo_grid_encoder_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "neo_grid_encoder_dense": (C.c_int, [C.POINTER(NeoGridEncoderParams), C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                          C.c_float, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

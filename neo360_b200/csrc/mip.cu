@@ -164,27 +164,47 @@ __global__ void resample_kernel(const float* __restrict__ s_prev, const float* _
 // ------------------------------------------------------------------------------------------------
 // conical frustum -> Gaussian -> contraction -> 21-direction lift -> integrated positional encoding (one warp per sample)
 // ------------------------------------------------------------------------------------------------
-// conical frustum [t0, t1] of ray b -> Gaussian (helper.py:293-339) -> contraction with its Jacobian (helper.py:33-66): z[3], zc[3][3]
-__device__ __forceinline__ void frustum_gaussian(const float* __restrict__ rays_o, const float* __restrict__ rays_d,
-                                                 const float* __restrict__ radii, const float* __restrict__ tdist, int b, int k, int n,
-                                                 float (&z)[3], float (&zc)[3][3]) {
-    const float t0 = tdist[(size_t)b * (n + 1) + k], t1 = tdist[(size_t)b * (n + 1) + k + 1];
-    const float d[3] = {rays_d[3 * b], rays_d[3 * b + 1], rays_d[3 * b + 2]};
-    const float o[3] = {rays_o[3 * b], rays_o[3 * b + 1], rays_o[3 * b + 2]};
-    const float rad = radii[b];
-    const float mu = (t0 + t1) / 2.f, hw = (t1 - t0) / 2.f;
-    const float denom = fmaxf(3.f * mu * mu + hw * hw, kEps);
-    const float t_mean = mu + (2.f * mu * hw * hw) / denom;
-    const float hw4 = hw * hw * hw * hw;
-    const float t_var = (hw * hw) / 3.f - (4.f / 15.f) * hw4 * (12.f * mu * mu - hw * hw) / (denom * denom);
-    const float r_var = ((mu * mu) / 4.f + (5.f / 12.f) * hw * hw - (4.f / 15.f) * hw4 / denom) * rad * rad;
-    const float dmag = fmaxf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2], 1e-10f);
-    float mean[3], cov[3][3];
-    for (int i = 0; i < 3; ++i) {
-        mean[i] = d[i] * t_mean + o[i];
-        for (int j = 0; j < 3; ++j) cov[i][j] = t_var * d[i] * d[j] + r_var * ((i == j ? 1.f : 0.f) - d[i] * (d[j] / dmag));
+// Sources of the Gaussian (mean, cov) of sample m that the IPE features encode.  The encoding itself (contraction, lift, IPE) is
+// the same code for both: features_kernel and features16_kernel take the source as a template parameter.
+// conical frustum [t0, t1] of sample k of ray b, m = b * n + k (helper.py:293-339): the render's samples
+struct FrustumSrc {          // read-only inputs: loaded through the non-coherent path (__ldg), as the kernels' __restrict__ arguments were
+    const float *rays_o, *rays_d, *radii, *tdist;
+    int n;
+    __device__ __forceinline__ void operator()(long long m, float (&mean)[3], float (&cov)[3][3]) const {
+        const int b = (int)(m / n), k = (int)(m % n);
+        const float t0 = __ldg(tdist + (size_t)b * (n + 1) + k), t1 = __ldg(tdist + (size_t)b * (n + 1) + k + 1);
+        const float d[3] = {__ldg(rays_d + 3 * b), __ldg(rays_d + 3 * b + 1), __ldg(rays_d + 3 * b + 2)};
+        const float o[3] = {__ldg(rays_o + 3 * b), __ldg(rays_o + 3 * b + 1), __ldg(rays_o + 3 * b + 2)};
+        const float rad = __ldg(radii + b);
+        const float mu = (t0 + t1) / 2.f, hw = (t1 - t0) / 2.f;
+        const float denom = fmaxf(3.f * mu * mu + hw * hw, kEps);
+        const float t_mean = mu + (2.f * mu * hw * hw) / denom;
+        const float hw4 = hw * hw * hw * hw;
+        const float t_var = (hw * hw) / 3.f - (4.f / 15.f) * hw4 * (12.f * mu * mu - hw * hw) / (denom * denom);
+        const float r_var = ((mu * mu) / 4.f + (5.f / 12.f) * hw * hw - (4.f / 15.f) * hw4 / denom) * rad * rad;
+        const float dmag = fmaxf(d[0] * d[0] + d[1] * d[1] + d[2] * d[2], 1e-10f);
+        for (int i = 0; i < 3; ++i) {
+            mean[i] = d[i] * t_mean + o[i];
+            for (int j = 0; j < 3; ++j) cov[i][j] = t_var * d[i] * d[j] + r_var * ((i == j ? 1.f : 0.f) - d[i] * (d[j] / dmag));
+        }
     }
-    // contraction z = x (r<=1) | ((2r-1)/r^2) x ; J = f I + ((2-2r)/r^4) x x^T
+};
+// a point o + t viewdirs of sample k of ray b (fp32, each operation rounded) with covariance diag(var): neo_mip_field_eval
+struct PointSrc {
+    const float *rays_o, *viewdirs, *t;
+    int n;
+    float var[3];
+    __device__ __forceinline__ void operator()(long long m, float (&mean)[3], float (&cov)[3][3]) const {
+        const int b = (int)(m / n);
+        const float tm = __ldg(t + m);
+        for (int i = 0; i < 3; ++i) {
+            mean[i] = add_(__ldg(rays_o + 3 * b + i), mul_(tm, __ldg(viewdirs + 3 * b + i)));
+            for (int j = 0; j < 3; ++j) cov[i][j] = i == j ? var[i] : 0.f;
+        }
+    }
+};
+// contraction with its Jacobian (helper.py:33-66): z = x (r<=1) | ((2r-1)/r^2) x ; J = f I + ((2-2r)/r^4) x x^T ; zc = J cov J^T
+__device__ __forceinline__ void contract_gaussian(const float (&mean)[3], const float (&cov)[3][3], float (&z)[3], float (&zc)[3][3]) {
     const float r2 = fmaxf(mean[0] * mean[0] + mean[1] * mean[1] + mean[2] * mean[2], 1e-32f);
     if (r2 <= 1.f) {
         for (int i = 0; i < 3; ++i) { z[i] = mean[i]; for (int j = 0; j < 3; ++j) zc[i][j] = cov[i][j]; }
@@ -196,16 +216,21 @@ __device__ __forceinline__ void frustum_gaussian(const float* __restrict__ rays_
         for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) zc[i][j] = Tm[i][0] * J[j][0] + Tm[i][1] * J[j][1] + Tm[i][2] * J[j][2];
     }
 }
+template <class Src>
+__device__ __forceinline__ void contracted_gaussian(const Src& src, long long m, float (&z)[3], float (&zc)[3][3]) {
+    float mean[3], cov[3][3];
+    src(m, mean, cov);
+    contract_gaussian(mean, cov, z, zc);
+}
 
 // fp32 path (tight parity): one warp per sample, the reference's own sin(x), sin(x + pi/2) formulation
-__global__ void features_kernel(const float* __restrict__ rays_o, const float* __restrict__ rays_d, const float* __restrict__ radii,
-                                const float* __restrict__ tdist, const float* __restrict__ basis, long long M, int n,
-                                float* __restrict__ X) {
+template <class Src>
+__global__ void features_kernel(Src src, const float* __restrict__ basis, long long M, float* __restrict__ X) {
     const long long m = (long long)blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32;
     const int lane = threadIdx.x % 32;
     if (m >= M) return;
     float z[3], zc[3][3];
-    frustum_gaussian(rays_o, rays_d, radii, tdist, (int)(m / n), (int)(m % n), n, z, zc);
+    contracted_gaussian(src, m, z, zc);
     if (lane < kBasis) {
         const float p[3] = {basis[lane], basis[kBasis + lane], basis[2 * kBasis + lane]};
         const float lm = z[0] * p[0] + z[1] * p[1] + z[2] * p[2];
@@ -231,10 +256,9 @@ __global__ void features_kernel(const float* __restrict__ rays_o, const float* _
 // the row is assembled in shared memory and leaves as 16-byte coalesced stores (the 2-byte scattered stores of the warp-per-sample
 // kernel were the bottleneck: r2 launch list, 15.9 % of the Mip-NeRF 360 frame).
 constexpr int kFeatSamples = 12, kFeatThreads = kFeatSamples * kBasis;     // 252
-__global__ void __launch_bounds__(kFeatThreads) features16_kernel(const float* __restrict__ rays_o, const float* __restrict__ rays_d,
-                                                                  const float* __restrict__ radii, const float* __restrict__ tdist,
-                                                                  const float* __restrict__ basis, long long M, int n,
-                                                                  __half* __restrict__ X16, long long ld16) {
+template <class Src>
+__global__ void __launch_bounds__(kFeatThreads) features16_kernel(Src src, const float* __restrict__ basis, long long M, __half* __restrict__ X16,
+                                                                  long long ld16) {
     __shared__ float zs[kFeatSamples][12];
     __shared__ __align__(16) __half row[kFeatSamples][kFeat + 8];
     const int tid = threadIdx.x;
@@ -242,8 +266,7 @@ __global__ void __launch_bounds__(kFeatThreads) features16_kernel(const float* _
     const int nrows = (int)((M - m0) < kFeatSamples ? (M - m0) : kFeatSamples);
     if (tid < nrows) {
         float z[3], zc[3][3];
-        const long long m = m0 + tid;
-        frustum_gaussian(rays_o, rays_d, radii, tdist, (int)(m / n), (int)(m % n), n, z, zc);
+        contracted_gaussian(src, m0 + tid, z, zc);
         for (int i = 0; i < 3; ++i) { zs[tid][i] = z[i]; for (int j = 0; j < 3; ++j) zs[tid][3 + 3 * i + j] = zc[i][j]; }
     }
     if (tid < kFeatSamples * 8) row[tid / 8][kFeat + (tid % 8)] = __float2half_rn(0.f);
@@ -341,6 +364,17 @@ __global__ void __launch_bounds__(256) sgemm_kernel(const float* __restrict__ A1
             out[(size_t)mrow * N + nn] = v;
         }
     }
+}
+
+// composite_kernel's head activations without the compositing (neo_mip_field_eval): density = softplus(raw - 1), rgb = 1.002 sigmoid - 0.001
+__global__ void field_act_kernel(const float* __restrict__ raw_density, const float* __restrict__ raw_rgb, long long M, float* __restrict__ density,
+                                 float* __restrict__ rgb) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= M * 4) return;
+    const long long m = i >> 2;
+    const int c = (int)(i & 3);
+    if (c == 3) density[m] = softplus_(raw_density[m] - 1.0f);
+    else if (rgb) rgb[m * 3 + c] = rgb_act(raw_rgb[m * 3 + c]);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -490,23 +524,25 @@ constexpr int kFeatPad = 512, kDirPad = 64;
 size_t tc_weight_halves(int width) {      // fp16 elements of one MLP's packed weights (upper bound: the 8-layer NeRF MLP)
     return (size_t)width * kFeatPad + 6 * (size_t)width * width + (size_t)width * (width + kFeatPad) + 256 * (size_t)width + 128 * (256 + kDirPad);
 }
-size_t carve(Carve& c, int n, const NeoMipCfg* cfg, int width, WSM& w) {
-    const int ns[3] = {cfg->n_prop, cfg->n_prop, cfg->n_nerf};
-    int nmax = cfg->n_prop > cfg->n_nerf ? cfg->n_prop : cfg->n_nerf;
-    for (int l = 0; l < 3; ++l) { w.s[l] = c.take<float>((size_t)n * (ns[l] + 1)); w.w[l] = c.take<float>((size_t)n * ns[l]); }
-    w.t = c.take<float>((size_t)n * (nmax + 1));
-    const size_t M = (size_t)n * nmax;
-    const bool tcp = cfg->precision == NEO_PREC_TC;          // the fp32 activation buffers are not needed on the tensor-core path
-    w.X = c.take<float>(tcp ? 0 : M * mip::kFeat);
+// the buffers of one MLP evaluation over M samples (features, activations, raw heads; the packed fp16 weights on the tensor-core path)
+void carve_mlp(Carve& c, size_t M, int width, bool tcp, WSM& w) {
+    w.X = c.take<float>(tcp ? 0 : M * mip::kFeat);          // the fp32 activation buffers are not needed on the tensor-core path
     w.Ha = c.take<float>(tcp ? 0 : M * width); w.Hb = c.take<float>(tcp ? 0 : M * width);
     w.beta = c.take<float>(tcp ? 0 : M * 256); w.DE = c.take<float>(tcp ? 0 : M * 27); w.V = c.take<float>(tcp ? 0 : M * 128);
     w.rawd = c.take<float>(M); w.rawc = c.take<float>(M * 3);
-    if (cfg->precision == NEO_PREC_TC) {
+    if (tcp) {
         for (int i = 0; i < 2; ++i) w.A16[i] = c.take<__half>(M * (size_t)(width + kFeatPad));
         w.B16 = c.take<__half>(M * (256 + kDirPad));
         w.V16 = c.take<__half>(M * 128);
         w.W16 = c.take<__half>(tc_weight_halves(width));
     }
+}
+size_t carve(Carve& c, int n, const NeoMipCfg* cfg, int width, WSM& w) {
+    const int ns[3] = {cfg->n_prop, cfg->n_prop, cfg->n_nerf};
+    int nmax = cfg->n_prop > cfg->n_nerf ? cfg->n_prop : cfg->n_nerf;
+    for (int l = 0; l < 3; ++l) { w.s[l] = c.take<float>((size_t)n * (ns[l] + 1)); w.w[l] = c.take<float>((size_t)n * ns[l]); }
+    w.t = c.take<float>((size_t)n * (nmax + 1));
+    carve_mlp(c, (size_t)n * nmax, width, cfg->precision == NEO_PREC_TC, w);
     return c.used;
 }
 int check(const NeoMipCfg* c) {
@@ -594,6 +630,46 @@ int mlp_tc(const NeoMipMLPParams& p, const WSM& w, long long M, int n, const flo
     }
     return NEO_OK;
 }
+
+// One MLP of Mip-NeRF 360 as the chain of fp32 SGEMMs with fused bias / ReLU / concatenation (the reference formulation).
+int mlp_fp32(const NeoMipMLPParams& p, const WSM& w, long long M, int n, const float* viewdirs, float* rawd, float* rawc, cudaStream_t s) {
+    int rc;
+    float* src = w.Ha;
+    float* dst = w.Hb;
+    if ((rc = gemm(w.X, mip::kFeat, nullptr, 0, p.w[0], p.b[0], M, p.width, 1, src, s))) return rc;
+    for (int l = 1; l < p.depth; ++l) {
+        const bool skip_in = (l == 5);                      // cat([h, inputs]) after layer 4 feeds layer 5
+        if ((rc = gemm(src, p.width, skip_in ? w.X : nullptr, skip_in ? mip::kFeat : 0, p.w[l], p.b[l], M, p.width, 1, dst, s))) return rc;
+        float* tmp = src; src = dst; dst = tmp;
+    }
+    if ((rc = gemm(src, p.width, nullptr, 0, p.wsig, p.bsig, M, 1, 0, rawd, s))) return rc;
+    if (p.wrgb) {
+        if ((rc = gemm(src, p.width, nullptr, 0, p.wb, p.bb, M, 256, 0, w.beta, s))) return rc;
+        mip::dir_kernel<<<(unsigned)((M * 27 + 255) / 256), 256, 0, s>>>(viewdirs, M, n, w.DE, 27, 27);
+        NEO_LAUNCH_CHECK("mip dir_kernel");
+        if ((rc = gemm(w.beta, 256, w.DE, 27, p.wv0, p.bv0, M, 128, 1, w.V, s))) return rc;
+        if ((rc = gemm(w.V, 128, nullptr, 0, p.wrgb, p.brgb, M, 3, 0, rawc, s))) return rc;
+    }
+    return NEO_OK;
+}
+// features (of the Gaussians of `src`) and then the MLP of one level, in either precision: raw density (M), raw rgb (M, 3) if p has a colour head
+template <class Src>
+int features_mlp(const NeoMipMLPParams& p, Src src, const WSM& w, long long M, int n, const float* viewdirs, int precision, cudaStream_t s) {
+    if (precision == NEO_PREC_TC) {
+        mip::features16_kernel<<<(unsigned)((M + mip::kFeatSamples - 1) / mip::kFeatSamples), mip::kFeatThreads, 0, s>>>(
+            src, p.basis, M, w.A16[0] + p.width, p.width + kFeatPad);
+        NEO_LAUNCH_CHECK("mip features16_kernel");
+        return mlp_tc(p, w, M, n, viewdirs, w.rawd, w.rawc, s);
+    }
+    mip::features_kernel<<<(unsigned)((M + 7) / 8), 256, 0, s>>>(src, p.basis, M, w.X);
+    NEO_LAUNCH_CHECK("mip features_kernel");
+    return mlp_fp32(p, w, M, n, viewdirs, w.rawd, w.rawc, s);
+}
+int check_mlp(const NeoMipMLPParams& p, int l) {
+    if (p.depth < 1 || p.depth > 8 || p.width < 64 || p.width % 4 || !p.basis) { set_error("mip mlp %d: bad depth/width", l); return NEO_ERR_INVALID; }
+    if ((l == 2) != (p.wrgb != nullptr)) { set_error("mip: mlps must be {prop, prop, nerf}"); return NEO_ERR_INVALID; }
+    return NEO_OK;
+}
 }  // namespace
 
 extern "C" size_t neo_mip_workspace_bytes(int n_rays, const NeoMipCfg* cfg, int nerf_width) {
@@ -609,11 +685,8 @@ extern "C" int neo_mip_render_fwd(const NeoMipMLPParams mlps[3], const float* ra
     if (!mlps || !rays_o || !rays_d || !viewdirs || !radii || !out || n_rays <= 0) { set_error("neo_mip_render_fwd: bad arguments"); return NEO_ERR_INVALID; }
     int rc = check(cfg);
     if (rc) return rc;
-    for (int l = 0; l < 3; ++l) {
-        const NeoMipMLPParams& p = mlps[l];
-        if (p.depth < 1 || p.depth > 8 || p.width < 64 || p.width % 4 || !p.basis) { set_error("mip mlp %d: bad depth/width", l); return NEO_ERR_INVALID; }
-        if ((l == 2) != (p.wrgb != nullptr)) { set_error("mip: mlps must be {prop, prop, nerf}"); return NEO_ERR_INVALID; }
-    }
+    for (int l = 0; l < 3; ++l)
+        if ((rc = check_mlp(mlps[l], l))) return rc;
     cudaStream_t s = (cudaStream_t)stream;
     const int width = mlps[2].width > 256 ? mlps[2].width : 256;
     Carve c{static_cast<unsigned char*>(workspace), 0};
@@ -630,38 +703,10 @@ extern "C" int neo_mip_render_fwd(const NeoMipMLPParams mlps[3], const float* ra
         if ((rc = launch_resample(lvl ? w.s[lvl - 1] : nullptr, lvl ? w.w[lvl - 1] : nullptr, n_rays, n_prev, lvl, dilation, anneal, n, cfg->near_plane,
                                   cfg->far_plane, cfg->jitter[lvl], w.s[lvl], w.t, s))) return rc;
         const long long M = (long long)n_rays * n;
-        const bool tcp = cfg->precision == NEO_PREC_TC;
-        if (tcp) mip::features16_kernel<<<(unsigned)((M + mip::kFeatSamples - 1) / mip::kFeatSamples), mip::kFeatThreads, 0, s>>>(
-                     rays_o, rays_d, radii, w.t, mlps[lvl].basis, M, n, w.A16[0] + mlps[lvl].width, mlps[lvl].width + kFeatPad);
-        else mip::features_kernel<<<(unsigned)((M + 7) / 8), 256, 0, s>>>(rays_o, rays_d, radii, w.t, mlps[lvl].basis, M, n, w.X);
-        NEO_LAUNCH_CHECK("mip features_kernel");
         const NeoMipMLPParams& p = mlps[lvl];
-        const float* rawc = nullptr;
-        if (cfg->precision == NEO_PREC_TC) {
-            if ((rc = mlp_tc(p, w, M, n, viewdirs, w.rawd, w.rawc, s))) return rc;
-            if (p.wrgb) rawc = w.rawc;
-            else if (out->rgb_s[lvl]) NEO_CUDA(cudaMemsetAsync(out->rgb_s[lvl], 0, (size_t)M * 3 * sizeof(float), s));
-        } else {
-            float* src = w.Ha;
-            float* dst = w.Hb;
-            if ((rc = gemm(w.X, mip::kFeat, nullptr, 0, p.w[0], p.b[0], M, p.width, 1, src, s))) return rc;
-            for (int l = 1; l < p.depth; ++l) {
-                const bool skip_in = (l == 5);                      // cat([h, inputs]) after layer 4 feeds layer 5
-                if ((rc = gemm(src, p.width, skip_in ? w.X : nullptr, skip_in ? mip::kFeat : 0, p.w[l], p.b[l], M, p.width, 1, dst, s))) return rc;
-                float* tmp = src; src = dst; dst = tmp;
-            }
-            if ((rc = gemm(src, p.width, nullptr, 0, p.wsig, p.bsig, M, 1, 0, w.rawd, s))) return rc;
-                    if (p.wrgb) {
-                if ((rc = gemm(src, p.width, nullptr, 0, p.wb, p.bb, M, 256, 0, w.beta, s))) return rc;
-                mip::dir_kernel<<<(unsigned)((M * 27 + 255) / 256), 256, 0, s>>>(viewdirs, M, n, w.DE, 27, 27);
-                NEO_LAUNCH_CHECK("mip dir_kernel");
-                if ((rc = gemm(w.beta, 256, w.DE, 27, p.wv0, p.bv0, M, 128, 1, w.V, s))) return rc;
-                if ((rc = gemm(w.V, 128, nullptr, 0, p.wrgb, p.brgb, M, 3, 0, w.rawc, s))) return rc;
-                rawc = w.rawc;
-            } else {
-                if (out->rgb_s[lvl]) NEO_CUDA(cudaMemsetAsync(out->rgb_s[lvl], 0, (size_t)M * 3 * sizeof(float), s));     // disable_rgb: zeros
-            }
-        }
+        if ((rc = features_mlp(p, mip::FrustumSrc{rays_o, rays_d, radii, w.t, n}, w, M, n, viewdirs, cfg->precision, s))) return rc;
+        const float* rawc = p.wrgb ? w.rawc : nullptr;
+        if (!p.wrgb && out->rgb_s[lvl]) NEO_CUDA(cudaMemsetAsync(out->rgb_s[lvl], 0, (size_t)M * 3 * sizeof(float), s));     // disable_rgb: zeros
         const int cw = kCompWarps;
         mip::composite_kernel<<<(n_rays + cw - 1) / cw, cw * 32, 0, s>>>(w.rawd, rawc, w.t, rays_d, n_rays, n, out->density[lvl],
                                                                         rawc ? out->rgb_s[lvl] : nullptr, w.w[lvl], out->rgb[lvl]);
@@ -669,6 +714,40 @@ extern "C" int neo_mip_render_fwd(const NeoMipMLPParams mlps[3], const float* ra
         if ((rc = copy_out(out->sdist[lvl], w.s[lvl], (size_t)n_rays * (n + 1), s))) return rc;
         if ((rc = copy_out(out->weights[lvl], w.w[lvl], (size_t)M, s))) return rc;
     }
+    return NEO_OK;
+}
+
+extern "C" size_t neo_mip_field_workspace_bytes(long long n_points, int width, int precision) {
+    if (n_points <= 0 || width < 64 || (precision != NEO_PREC_FP32 && precision != NEO_PREC_TC)) return 0;
+    Carve c{nullptr, 0};
+    WSM w;
+    carve_mlp(c, (size_t)n_points, width > 256 ? width : 256, precision == NEO_PREC_TC, w);
+    return c.used;
+}
+
+extern "C" int neo_mip_field_eval(const NeoMipMLPParams mlps[3], int level, const NeoRays* rays, const float* t_vals, int N, const float var[3],
+                                  int precision, float* rgb, float* density, void* ws, size_t ws_bytes, void* stream) {
+    if (!mlps || !rays || !t_vals || !var || !density) { set_error("neo_mip_field_eval: null argument"); return NEO_ERR_INVALID; }
+    if (level < 0 || level > 2) { set_error("neo_mip_field_eval: level must be 0, 1 or 2 (got %d)", level); return NEO_ERR_INVALID; }
+    if (rgb && level < 2) { set_error("neo_mip_field_eval: proposal level %d has no colour head (pass rgb = NULL)", level); return NEO_ERR_INVALID; }
+    if (precision != NEO_PREC_FP32 && precision != NEO_PREC_TC) { set_error("neo_mip_field_eval: bad precision %d", precision); return NEO_ERR_INVALID; }
+    if (rays->n_rays <= 0 || !rays->rays_o || !rays->viewdirs || N < 1) { set_error("neo_mip_field_eval: empty rays or N < 1"); return NEO_ERR_INVALID; }
+    for (int i = 0; i < 3; ++i)
+        if (!(var[i] >= 0.f && var[i] <= 3.4e38f)) { set_error("neo_mip_field_eval: var must be finite and >= 0"); return NEO_ERR_INVALID; }
+    int rc = check_mlp(mlps[level], level);
+    if (rc) return rc;
+    const NeoMipMLPParams& p = mlps[level];
+    const long long M = (long long)rays->n_rays * N;
+    if (M > ((long long)1 << 31) - 1) { set_error("neo_mip_field_eval: n_rays * N must be below 2^31"); return NEO_ERR_INVALID; }
+    Carve c{static_cast<unsigned char*>(ws), 0};
+    WSM w;
+    carve_mlp(c, (size_t)M, p.width > 256 ? p.width : 256, precision == NEO_PREC_TC, w);
+    if (!ws || ws_bytes < c.used) { set_error("workspace too small: need %zu bytes, got %zu", c.used, ws_bytes); return NEO_ERR_WORKSPACE; }
+    cudaStream_t s = (cudaStream_t)stream;
+    const mip::PointSrc src{rays->rays_o, rays->viewdirs, t_vals, N, {var[0], var[1], var[2]}};
+    if ((rc = features_mlp(p, src, w, M, N, rays->viewdirs, precision, s))) return rc;
+    mip::field_act_kernel<<<(unsigned)((M * 4 + 255) / 256), 256, 0, s>>>(w.rawd, p.wrgb ? w.rawc : nullptr, M, density, rgb);
+    NEO_LAUNCH_CHECK("mip field_act_kernel");
     return NEO_OK;
 }
 
@@ -698,7 +777,7 @@ extern "C" int neo_mip_encode(const float* rays_o, const float* rays_d, const fl
     }
     cudaStream_t s = (cudaStream_t)stream;
     const long long M = (long long)n_rays * N;
-    mip::features_kernel<<<(unsigned)((M + 7) / 8), 256, 0, s>>>(rays_o, rays_d, radii, tdist, basis, M, N, feats);
+    mip::features_kernel<<<(unsigned)((M + 7) / 8), 256, 0, s>>>(mip::FrustumSrc{rays_o, rays_d, radii, tdist, N}, basis, M, feats);
     NEO_LAUNCH_CHECK("mip features_kernel");
     mip::dir_kernel<<<(unsigned)(((long long)n_rays * kDirEnc + 255) / 256), 256, 0, s>>>(viewdirs, (long long)n_rays, 1, dir_enc, kDirEnc, kDirEnc);
     NEO_LAUNCH_CHECK("mip dir_kernel");

@@ -229,19 +229,53 @@ __global__ void encode_kernel(const float* __restrict__ rays_o, const float* __r
 using namespace neo;
 
 namespace {
-struct WSV { float *t0, *w0, *t1, *w1, *sig, *rgb; __half *A16[2], *B16, *V16; float *rawd, *rawc; };
+// Scratch of one level's field: the tensor-core chain's fp16 activation rows and raw head outputs (the fp32 field kernel needs none)
+struct WSF { __half *A16[2], *B16, *V16; float *rawd, *rawc; };
+struct WSV { float *t0, *w0, *t1, *w1, *sig, *rgb; WSF f; };
 constexpr int kLdA = 256 + 64, kLdB = 256 + 64;      // activation rows: [h (256) | padded encoding (64)], [bottleneck (256) | padded direction encoding (64)]
+void carve_field(Carve& c, size_t M, WSF& w, int precision) {
+    if (precision != NEO_PREC_TC) return;
+    for (int i = 0; i < 2; ++i) w.A16[i] = c.take<__half>(M * kLdA);
+    w.B16 = c.take<__half>(M * kLdB);
+    w.V16 = c.take<__half>(M * 128);
+    w.rawd = c.take<float>(M); w.rawc = c.take<float>(M * 3);
+}
 size_t carve(Carve& c, int n, int N0, int N1, WSV& w, int precision) {
     w.t0 = c.take<float>((size_t)n * N0); w.w0 = c.take<float>((size_t)n * N0); w.t1 = c.take<float>((size_t)n * N1); w.w1 = c.take<float>((size_t)n * N1);
     w.sig = c.take<float>((size_t)n * N1); w.rgb = c.take<float>((size_t)n * N1 * 3);
-    if (precision == NEO_PREC_TC) {
-        const size_t M = (size_t)n * N1;
-        for (int i = 0; i < 2; ++i) w.A16[i] = c.take<__half>(M * kLdA);
-        w.B16 = c.take<__half>(M * kLdB);
-        w.V16 = c.take<__half>(M * 128);
-        w.rawd = c.take<float>(M); w.rawc = c.take<float>(M * 3);
-    }
+    carve_field(c, (size_t)n * N1, w.f, precision);
     return c.used;
+}
+// One level's NeRFMLP at the points o + t viewdirs of t (n, N): activated rgb (n, N, 3) and sigma (n, N).  The render and
+// neo_vanilla_field_eval both run this, so the two give the same bits.
+int field(const NeoVanilla::Mlp& m, const float* rays_o, const float* viewdirs, const float* t, int n, int N, int precision, const WSF& w,
+          float* rgb, float* sig, cudaStream_t s) {
+    const long long total = (long long)n * N;
+    int rc;
+    if (precision == NEO_PREC_TC) {
+        // NeRFMLP (models/vanilla_nerf/model.py:44-125) layer by layer on the tensor cores (csrc/gemm_tc.cu), fp16 activations; the skip concatenation
+        // by keeping h4 and the encoding in ONE buffer (layer 5 is a single K = 320 GEMM)
+        __half* buf[2] = {w.A16[0], w.A16[1]};
+        __half* B = w.B16;
+        van::enc16_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(rays_o, viewdirs, t, total, N, buf[0] + 256, kLdA, B + 256, kLdB);
+        NEO_LAUNCH_CHECK("vanilla enc16_kernel");
+        if ((rc = gemm_f16(buf[0] + 256, kLdA, m.w16[0], 64, m.b[0], buf[0], kLdA, total, 256, 64, 1, s))) return rc;
+        for (int l = 1; l < 8; ++l) {
+            const int K = l == 5 ? 320 : 256;
+            if ((rc = gemm_f16(buf[(l - 1) & 1], kLdA, m.w16[l], K, m.b[l], buf[l & 1], kLdA, total, 256, K, 1, s))) return rc;
+        }
+        const __half* h = buf[1];
+        if ((rc = launch_rowdot_f16(h, kLdA, 256, m.wsig, m.bsig, 1, total, w.rawd, s))) return rc;
+        if ((rc = gemm_f16(h, kLdA, m.wb16, 256, m.bb, B, kLdB, total, 256, 256, 0, s))) return rc;
+        if ((rc = gemm_f16(B, kLdB, m.wv016, 320, m.bv0, w.V16, 128, total, 128, 320, 1, s))) return rc;
+        if ((rc = launch_rowdot_f16(w.V16, 128, 128, m.wrgb, m.brgb, 3, total, w.rawc, s))) return rc;
+        van::head_act_kernel<<<(unsigned)((total * 4 + 255) / 256), 256, 0, s>>>(w.rawd, w.rawc, total, sig, rgb);
+        NEO_LAUNCH_CHECK("vanilla head_act_kernel");
+    } else {
+        van::field_kernel<<<(unsigned)((total + van::kP - 1) / van::kP), van::kThreads, 0, s>>>(m, rays_o, viewdirs, t, n, N, rgb, sig);
+        NEO_LAUNCH_CHECK("vanilla field_kernel");
+    }
+    return NEO_OK;
 }
 int check(const NeoVanillaCfg* c) {
     if (!c || c->n_coarse < 3 || c->n_fine < 1 || c->n_coarse > 4096 || c->n_fine > 4096) { set_error("vanilla: bad sample counts"); return NEO_ERR_INVALID; }
@@ -353,32 +387,7 @@ extern "C" int neo_vanilla_render_fwd(const NeoVanilla* v, const NeoRays* rays, 
             // sample_pdf: bins = mids(t), weights[1:-1]; same ascending-bin inverse CDF + merge as the NeO-360 foreground branch
             if ((rc = launch_resample(rays->rays_o, rays->viewdirs, nullptr, w.t0, w.w0, n, N0, cfg->n_fine, 1, 0.f, cfg->u1, t, nullptr, nullptr, s))) return rc;
         }
-        long long total = (long long)n * N;
-        if (cfg->precision == NEO_PREC_TC) {
-            // NeRFMLP (models/vanilla_nerf/model.py:44-125) layer by layer on the tensor cores (csrc/gemm_tc.cu), fp16 activations; the skip concatenation
-            // by keeping h4 and the encoding in ONE buffer (layer 5 is a single K = 320 GEMM)
-            const NeoVanilla::Mlp& m = v->mlp[lvl];
-            __half* buf[2] = {w.A16[0], w.A16[1]};
-            __half* B = w.B16;
-            van::enc16_kernel<<<(unsigned)((total + 255) / 256), 256, 0, s>>>(rays->rays_o, rays->viewdirs, t, total, N, buf[0] + 256, kLdA, B + 256, kLdB);
-            NEO_LAUNCH_CHECK("vanilla enc16_kernel");
-            if ((rc = gemm_f16(buf[0] + 256, kLdA, m.w16[0], 64, m.b[0], buf[0], kLdA, total, 256, 64, 1, s))) return rc;
-            for (int l = 1; l < 8; ++l) {
-                const int K = l == 5 ? 320 : 256;
-                if ((rc = gemm_f16(buf[(l - 1) & 1], kLdA, m.w16[l], K, m.b[l], buf[l & 1], kLdA, total, 256, K, 1, s))) return rc;
-            }
-            const __half* h = buf[1];
-            if ((rc = launch_rowdot_f16(h, kLdA, 256, m.wsig, m.bsig, 1, total, w.rawd, s))) return rc;
-            if ((rc = gemm_f16(h, kLdA, m.wb16, 256, m.bb, B, kLdB, total, 256, 256, 0, s))) return rc;
-            if ((rc = gemm_f16(B, kLdB, m.wv016, 320, m.bv0, w.V16, 128, total, 128, 320, 1, s))) return rc;
-            if ((rc = launch_rowdot_f16(w.V16, 128, 128, m.wrgb, m.brgb, 3, total, w.rawc, s))) return rc;
-            van::head_act_kernel<<<(unsigned)((total * 4 + 255) / 256), 256, 0, s>>>(w.rawd, w.rawc, total, w.sig, w.rgb);
-            NEO_LAUNCH_CHECK("vanilla head_act_kernel");
-        } else {
-            van::field_kernel<<<(unsigned)((total + van::kP - 1) / van::kP), van::kThreads, 0, s>>>(v->mlp[lvl], rays->rays_o, rays->viewdirs, t, n, N,
-                                                                                                      w.rgb, w.sig);
-            NEO_LAUNCH_CHECK("vanilla field_kernel");
-        }
+        if ((rc = field(v->mlp[lvl], rays->rays_o, rays->viewdirs, t, n, N, cfg->precision, w.f, w.rgb, w.sig, s))) return rc;
         // mode 2: ascending t, last interval 1e10, scaled by |rays_d|, depth nan_to_num(inf)
         if ((rc = launch_composite(w.rgb, w.sig, t, rays->rays_d, nullptr, n, N, cfg->white_bkgd, 2, out->comp_rgb[lvl], out->acc[lvl], wt, nullptr,
                                    out->depth[lvl], s))) return rc;
@@ -388,6 +397,29 @@ extern "C" int neo_vanilla_render_fwd(const NeoVanilla* v, const NeoRays* rays, 
         if ((rc = copy_out(out->weights[lvl], wt, (size_t)n * N, s))) return rc;
     }
     return NEO_OK;
+}
+
+extern "C" size_t neo_vanilla_field_workspace_bytes(long long n_points, int precision) {
+    if (n_points <= 0) return 0;
+    Carve c{nullptr, 0};
+    WSF w;
+    carve_field(c, (size_t)n_points, w, precision);
+    return c.used;
+}
+
+extern "C" int neo_vanilla_field_eval(const NeoVanilla* v, const NeoRays* rays, const float* t_vals, int N, int level, int precision, float* rgb,
+                                      float* sigma, void* ws, size_t ws_bytes, void* stream) {
+    if (!v || !rays || !t_vals || !rgb || !sigma) { set_error("neo_vanilla_field_eval: null argument"); return NEO_ERR_INVALID; }
+    if (rays->n_rays <= 0 || !rays->rays_o || !rays->viewdirs || N < 1) { set_error("neo_vanilla_field_eval: empty rays or N < 1"); return NEO_ERR_INVALID; }
+    if (level != 0 && level != 1) { set_error("neo_vanilla_field_eval: level must be 0 (coarse) or 1 (fine), got %d", level); return NEO_ERR_INVALID; }
+    if (precision != NEO_PREC_FP32 && precision != NEO_PREC_TC) { set_error("neo_vanilla_field_eval: bad precision %d", precision); return NEO_ERR_INVALID; }
+    const long long M = (long long)rays->n_rays * N;
+    if (M > ((long long)1 << 31) - 1) { set_error("neo_vanilla_field_eval: n_rays * N must be below 2^31"); return NEO_ERR_INVALID; }
+    Carve c{static_cast<unsigned char*>(ws), 0};
+    WSF w;
+    carve_field(c, (size_t)M, w, precision);
+    if (c.used && (!ws || ws_bytes < c.used)) { set_error("workspace too small: need %zu bytes, got %zu", c.used, ws_bytes); return NEO_ERR_WORKSPACE; }
+    return field(v->mlp[level], rays->rays_o, rays->viewdirs, t_vals, rays->n_rays, N, precision, w, rgb, sigma, (cudaStream_t)stream);
 }
 
 // ---- stage-level entry points of the training path (neo360_b200/vanilla.py): sampling and encodings have no backward; the compositing

@@ -16,7 +16,7 @@ dense layers are framework fp32 GEMMs under autograd, or with `train_precision="
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, List, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import torch
 import torch.nn as nn
@@ -125,6 +125,46 @@ class MipNeRF360(nn.Module):
             L.check(lib.neo_mip_render_fwd(arr, L.ptr(o), L.ptr(d), L.ptr(vd), L.ptr(radii), n, C.byref(cfg), C.byref(out), self._ws.data_ptr(),
                                            self._ws.numel(), torch.cuda.current_stream().cuda_stream))
         return ren, hist
+
+    @torch.no_grad()
+    def field(self, rays: Dict[str, torch.Tensor], t: torch.Tensor, level: int, var, precision: Optional[str] = None, rgb: bool = True):
+        """MLP `level` (0, 1: PropMLP; 2: NeRFMLP) at Gaussians with mean rays_o + t viewdirs and covariance diag(var), var a 3-sequence
+        of per-axis variances; viewdirs is the direction input (neo_mip_field_eval).  t (n_rays, N) -> (rgb (n_rays, N, 3) or None,
+        density (n_rays, N)) after their activations, in `precision` (default: the module's).  rgb is None at the proposal levels,
+        which have no colour head, and when rgb=False."""
+        o, vd = rays["rays_o"].contiguous().float(), rays["viewdirs"].contiguous().float()
+        if not o.is_cuda:
+            raise RuntimeError("neo360_b200 needs CUDA tensors (no CPU fallback)")
+        prec = precision or self.precision
+        if prec not in ("fp32", "tc"):
+            raise ValueError(f"precision must be 'fp32' or 'tc', got {prec!r}")
+        lib = L.load()
+        t = t.contiguous().float()
+        n, N = t.shape
+        dev = o.device
+        keep = []
+        arr = (L.NeoMipMLPParams * 3)(*[m.to(dev).c_params(keep) for m in self.mlps])
+        P = {"fp32": L.NEO_PREC_FP32, "tc": L.NEO_PREC_TC}[prec]
+        need = lib.neo_mip_field_workspace_bytes(n * N, self.mlps[level].netwidth if 0 <= level < 3 else 0, P)
+        if need == 0:
+            raise ValueError(f"Mip-NeRF 360 field: bad level {level} or size {n} x {N}")
+        ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        r = L.NeoRays()
+        r.n_rays, r.chunk = n, 0
+        r.rays_o, r.rays_d, r.viewdirs = L.ptr(o), L.ptr(vd), L.ptr(vd)
+        v = (C.c_float * 3)(*[float(x) for x in var])
+        out_rgb = torch.empty(n, N, 3, device=dev) if rgb and level == 2 else None
+        density = torch.empty(n, N, device=dev)
+        with torch.cuda.device(dev):
+            L.check(lib.neo_mip_field_eval(arr, int(level), C.byref(r), L.ptr(t), N, v, P, L.ptr(out_rgb), L.ptr(density), L.ptr(ws), need,
+                                           torch.cuda.current_stream().cuda_stream))
+        return out_rgb, density
+
+    def density_grid(self, resolution, bbox=((-1.0, -1.0, -1.0), (1.0, 1.0, 1.0)), level: int = 2, precision: Optional[str] = None,
+                     slab_rays: Optional[int] = None, var=None) -> torch.Tensor:
+        """density of MLP `level` on an (R_z, R_y, R_x) lattice over `bbox`; see neo360_b200.mesh.density_grid."""
+        from . import mesh
+        return mesh.density_grid(self, resolution, bbox, level, precision, slab_rays, var=var)
 
     def _forward_train(self, batch: Dict[str, torch.Tensor], train_frac: float, randomized: bool, near, far) -> Tuple[List[dict], List[dict]]:
         """MipNeRF360.forward under autograd (what LitMipNeRF360.training_step calls, model.py:427-456).  Per level: `neo_mip_resample` on the

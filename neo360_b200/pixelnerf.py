@@ -172,13 +172,13 @@ class PixelNeRF(nn.Module):
     def _key(tensors):
         return tuple((id(t), t._version) for t in tensors)
 
-    def _ensure_weights(self):
+    def _ensure_weights(self, precision: str):
         params = list(self.coarse_mlp.parameters()) + list(self.fine_mlp.parameters())
         key = tuple((p.data_ptr(), p._version) for p in params)
-        if self._packed is None or self._packed[0] != key or self._packed[1] != self.precision:
+        if self._packed is None or self._packed[0] != key or self._packed[1] != precision:
             keep = []
-            pack = (lambda m: m.c_params(keep)) if self.precision == "fp32" else (lambda m: m.tc_params(keep))
-            self._packed = (key, self.precision, keep, [pack(self.coarse_mlp), pack(self.fine_mlp)])
+            pack = (lambda m: m.c_params(keep)) if precision == "fp32" else (lambda m: m.tc_params(keep))
+            self._packed = (key, precision, keep, [pack(self.coarse_mlp), pack(self.fine_mlp)])
         return self._packed[3]
 
     def _ensure_scene(self, rays, lat_hw):
@@ -245,12 +245,12 @@ class PixelNeRF(nn.Module):
                                        1, 0.0, L.ptr(u), L.ptr(t1), None, None, _stream()))
         return t1
 
-    def _field(self, r, sc, lat, t, lvl):
+    def _field(self, r, sc, lat, t, lvl, precision: str):
         lib, dev = L.load(), t.device
         n, N = t.shape
-        mlp = self._ensure_weights()[lvl]
+        mlp = self._ensure_weights(precision)[lvl]
         rgb, sigma = torch.empty(n, N, 3, device=dev), torch.empty(n, N, device=dev)
-        if self.precision == "fp32":
+        if precision == "fp32":
             L.check(lib.neo_pixelnerf_field(sc.handle, L.ptr(lat), C.byref(mlp), C.byref(r), L.ptr(t), N, L.ptr(rgb), L.ptr(sigma), _stream()))
         else:
             need = lib.neo_pixelnerf_tc_workspace_bytes(sc.nv, n * N)
@@ -261,14 +261,25 @@ class PixelNeRF(nn.Module):
         return rgb, sigma
 
     @torch.no_grad()
-    def field(self, rays: Dict[str, torch.Tensor], t: torch.Tensor, level: int, chunk: Optional[int] = None):
-        """The field of one level at the caller's sample distances t (n_rays, N), in `self.precision`: rgb (n_rays, N, 3), sigma
-        (n_rays, N) after their activations (model_pixel.py:207-246).  For stage tests."""
+    def field(self, rays: Dict[str, torch.Tensor], t: torch.Tensor, level: int, chunk: Optional[int] = None, precision: Optional[str] = None):
+        """The field of one level at the caller's sample distances t (n_rays, N), in `precision` (default: `self.precision`): rgb
+        (n_rays, N, 3), sigma (n_rays, N) after their activations (model_pixel.py:207-246).  `rays` also holds the src_* entries of
+        `forward`'s batch; `chunk` is `forward`'s (quirk Q1)."""
+        prec = precision or self.precision
+        if prec not in ("fp32", "tc"):
+            raise ValueError(f"PixelNeRF precision must be 'fp32' or 'tc', got {prec!r}")
         r, (o, _, _) = self._rays(rays, chunk)
         with torch.cuda.device(o.device):
             lat = self._hoisted_latent(rays["src_imgs"])
             sc = self._ensure_scene(rays, lat.shape[1:3])
-            return self._field(r, sc, lat, t.contiguous().float(), level)
+            return self._field(r, sc, lat, t.contiguous().float(), level, prec)
+
+    def density_grid(self, resolution, bbox=((-1.0, -1.0, -1.0), (1.0, 1.0, 1.0)), level: int = 1, precision: Optional[str] = None,
+                     slab_rays: Optional[int] = None, batch: Optional[Dict[str, torch.Tensor]] = None) -> torch.Tensor:
+        """sigma of the MLP of `level` on an (R_z, R_y, R_x) lattice over `bbox`, seen by the source views of `batch` (its src_*
+        entries, as `forward` takes them); see neo360_b200.mesh.density_grid."""
+        from . import mesh
+        return mesh.density_grid(self, resolution, bbox, level, precision, slab_rays, batch)
 
     def forward(self, rays: Dict[str, torch.Tensor], randomized: bool, white_bkgd: bool, near, far, chunk: Optional[int] = None) -> List[tuple]:
         """model_pixel.py:174-258.  `chunk` (default: the whole call) is the caller's chunk size for quirk Q1: a sample's direction
@@ -288,7 +299,7 @@ class PixelNeRF(nn.Module):
             for lvl in range(2):
                 t = self._sample(lvl, o, d, t, w, n, near, far, u[lvl])
                 N = t.shape[1]
-                rgb, sigma = self._field(r, sc, lat, t, lvl)
+                rgb, sigma = self._field(r, sc, lat, t, lvl, self.precision)
                 comp, acc, w, depth = torch.empty(n, 3, device=dev), torch.empty(n, device=dev), torch.empty(n, N, device=dev), torch.empty(n, device=dev)
                 L.check(lib.neo_volumetric_rendering(L.ptr(rgb), L.ptr(sigma), L.ptr(t), L.ptr(d), None, n, N, int(bool(white_bkgd)), 2,
                                                      L.ptr(comp), L.ptr(acc), L.ptr(w), None, L.ptr(depth), _stream()))

@@ -13,7 +13,7 @@ parameter's storage and version)."""
 from __future__ import annotations
 
 import ctypes as C
-from typing import Dict, List
+from typing import Dict, List, Optional
 
 import torch
 import torch.nn as nn
@@ -164,6 +164,41 @@ class NeRF(nn.Module):
         if debug:
             self.last_debug = T
         return [(T["comp_rgb"][lvl], T["acc"][lvl], T["depth"][lvl]) for lvl in range(2)]
+
+    @torch.no_grad()
+    def field(self, rays: Dict[str, torch.Tensor], t: torch.Tensor, level: int, precision: Optional[str] = None):
+        """The NeRFMLP of `level` (0 coarse, 1 fine) at the points rays_o + t viewdirs of t (n_rays, N), viewdirs its direction input:
+        rgb (n_rays, N, 3), sigma (n_rays, N) after their activations (neo_vanilla_field_eval), in `precision` (default: the module's).
+        The same code as `forward`'s per-level field: at the render's own t the same bits as its `rgb_s` / `sigma`."""
+        o, vd = rays["rays_o"].contiguous().float(), rays["viewdirs"].contiguous().float()
+        if not o.is_cuda:
+            raise RuntimeError("neo360_b200 needs CUDA tensors (no CPU fallback)")
+        prec = precision or getattr(self, "precision", "fp32")
+        if prec not in ("fp32", "tc"):
+            raise ValueError(f"precision must be 'fp32' or 'tc', got {prec!r}")
+        lib = L.load()
+        t = t.contiguous().float()
+        n, N = t.shape
+        dev = o.device
+        h = self._ensure(dev)
+        P = {"fp32": L.NEO_PREC_FP32, "tc": L.NEO_PREC_TC}[prec]
+        need = lib.neo_vanilla_field_workspace_bytes(n * N, P)
+        if need and (self._ws is None or self._ws.numel() < need or self._ws.device != dev):
+            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        r = L.NeoRays()
+        r.n_rays, r.chunk = n, 0
+        r.rays_o, r.rays_d, r.viewdirs = L.ptr(o), L.ptr(vd), L.ptr(vd)
+        rgb, sigma = torch.empty(n, N, 3, device=dev), torch.empty(n, N, device=dev)
+        with torch.cuda.device(dev):
+            L.check(lib.neo_vanilla_field_eval(h, C.byref(r), L.ptr(t), N, int(level), P, L.ptr(rgb), L.ptr(sigma),
+                                               self._ws.data_ptr() if need else None, need, torch.cuda.current_stream().cuda_stream))
+        return rgb, sigma
+
+    def density_grid(self, resolution, bbox=((-1.0, -1.0, -1.0), (1.0, 1.0, 1.0)), level: int = 1, precision: Optional[str] = None,
+                     slab_rays: Optional[int] = None) -> torch.Tensor:
+        """sigma of the NeRFMLP of `level` on an (R_z, R_y, R_x) lattice over `bbox`; see neo360_b200.mesh.density_grid."""
+        from . import mesh
+        return mesh.density_grid(self, resolution, bbox, level, precision, slab_rays)
 
     def _forward_train(self, rays: Dict[str, torch.Tensor], randomized: bool, white_bkgd: bool, near, far, debug: bool = False) -> List[tuple]:
         """NeRF.forward under autograd (what LitNeRF.training_step calls, models/vanilla_nerf/model.py:273-299): the same tuples,
