@@ -164,6 +164,15 @@ int neo_get_rays(int H, int W, float focal, const float* c2w, float* rays_o, flo
 int neo_sample_rays(int n, const long long* pix_inds, int n_views, int H, int W, float focal, const float* c2w,
                     const float* images, float* rays_o, float* viewdirs, float* rays_d, float* radii, float* target,
                     int* err_flag, void* stream);
+/* Backward of neo_sample_rays (and of neo_get_rays: pix_inds = 0..H*W-1, n_views = 1) w.r.t. the camera-to-world matrices: upstream
+ * gradients g_rays_o, g_viewdirs, g_rays_d (n,3), any may be NULL, -> g_c2w (n_views,3,4), overwritten.  Chain: d = R dir_cam,
+ * viewdirs = rays_d = d / |d| (quirk Q3), rays_o = t.  radii is a norm of a difference of rotated directions, unchanged by any rotation
+ * R exp([w]x) and by t, so it takes no gradient here and a pose correction loses nothing by it.  Fixed-order reduction (per-ray terms, per-block partials of each
+ * view, then the partials summed per view in block order), no atomics: bit-identical run to run.  Out-of-range indices contribute
+ * nothing.  Workspace of neo_sample_rays_bwd_workspace_bytes(n, n_views). */
+size_t neo_sample_rays_bwd_workspace_bytes(int n, int n_views);
+int neo_sample_rays_bwd(int n, const long long* pix_inds, int n_views, int H, int W, float focal, const float* c2w, const float* g_rays_o,
+                        const float* g_viewdirs, const float* g_rays_d, float* g_c2w, void* workspace, size_t workspace_bytes, void* stream);
 /* models/neo360/helper.py:253-273 */
 int neo_intersect_sphere(const float* rays_o, const float* rays_d, int n_rays, float* far, int* err_flag,
                          void* stream);
@@ -362,9 +371,15 @@ int neo_vanilla_field_eval(const NeoVanilla* v, const NeoRays* rays, const float
 int neo_vanilla_sample_along_rays(const float* rays_o, const float* viewdirs, int n_rays, int n_coarse, float near_plane, float far_plane,
                                   const float* u_rand, float* t_vals, void* stream);
 /* fp32 positional encodings (helper.py:445-449 column order) of the points o + t viewdirs: enc (n_rays*N, 63), and of the view
- * directions: dir_enc (n_rays, 27).  The same arithmetic as the NEO_PREC_FP32 field kernel (bit-identical).  No backward. */
+ * directions: dir_enc (n_rays, 27).  The same arithmetic as the NEO_PREC_FP32 field kernel (bit-identical).  Backward w.r.t. the rays:
+ * neo_vanilla_encode_bwd. */
 int neo_vanilla_encode(const float* rays_o, const float* viewdirs, const float* t_vals, int n_rays, int N, float* enc, float* dir_enc,
                        void* stream);
+/* Backward of neo_vanilla_encode w.r.t. the rays (t_vals carries no gradient): upstream g_enc (n_rays*N, 63) and g_dir_enc (n_rays, 27)
+ * -> g_rays_o (n_rays,3) = sum over the ray's samples of dL/dx, g_viewdirs (n_rays,3) = sum of t dL/dx plus the direction encoding's
+ * term.  One warp per ray, fixed-order sums, no atomics: bit-identical run to run. */
+int neo_vanilla_encode_bwd(const float* rays_o, const float* viewdirs, const float* t_vals, int n_rays, int N, const float* g_enc,
+                           const float* g_dir_enc, float* g_rays_o, float* g_viewdirs, void* stream);
 /* Backward of neo_volumetric_rendering in mode 2 (helper.py:521-559): upstream gradients of comp_rgb (n,3), acc (n), weights (n,N),
  * depth (n) -- any may be NULL -- -> d_rgb (n,N,3), d_sigma (n,N).  The depth gradient passes where sum w t was finite (nan_to_num +
  * clamp, quirk Q10) and is zero elsewhere.  Same rgb / sigma / t / rays_d as the forward call. */
@@ -467,9 +482,13 @@ int neo_mip_resample(const float* sdist_prev, const float* weights_prev, int n_r
                      float far_plane, float train_frac, const float* jitter, float* sdist, float* tdist, void* stream);
 /* fp32 integrated positional encoding of the conical frustums of tdist (n_rays, N+1) (cast_rays + contract + lift_and_diagonalize +
  * integrated_pos_enc): feats (n_rays*N, 504); and the direction encoding of viewdirs, one row per ray: dir_enc (n_rays, 27).  basis is
- * pos_basis_t (3,21).  The NEO_PREC_FP32 path's own kernels (bit-identical).  No backward. */
+ * pos_basis_t (3,21).  The NEO_PREC_FP32 path's own kernels (bit-identical).  Backward: neo_mip_encode_bwd. */
 int neo_mip_encode(const float* rays_o, const float* rays_d, const float* viewdirs, const float* radii, const float* tdist, const float* basis,
                    int n_rays, int N, float* feats, float* dir_enc, void* stream);
+/* Backward of neo_mip_encode w.r.t. the rays as the reference differentiates it: its `contract` returns detached Gaussians
+ * (models/mipnerf360/helper.py:63-66), so the IPE features give rays_o, rays_d and radii no gradient, and the direction encoding
+ * (model.py:152) gives viewdirs g_viewdirs (n_rays,3) from g_dir_enc (n_rays,27).  One thread per ray and coordinate, no atomics. */
+int neo_mip_encode_bwd(const float* viewdirs, int n_rays, const float* g_dir_enc, float* g_viewdirs, void* stream);
 /* Head activations + compute_alpha_weights(opaque_background) + volumetric_rendering with a white background (helper.py:234-274) of raw
  * density (n_rays,N) and raw rgb (n_rays,N,3) at tdist (n_rays,N+1): rgb (n_rays,3), weights (n_rays,N), density (n_rays,N), rgb_s
  * (n_rays,N,3).  raw_rgb NULL = a proposal level (rgb_s is written as zeros).  Outputs may be NULL.  The eval path's compositing kernel. */
@@ -482,6 +501,12 @@ int neo_mip_composite(const float* raw_density, const float* raw_rgb, const floa
 int neo_mip_composite_bwd(const float* raw_density, const float* raw_rgb, const float* tdist, const float* rays_d, int n_rays, int N,
                           const float* g_rgb, const float* g_weights, const float* g_density, const float* g_rgb_s, float* d_raw_density,
                           float* d_raw_rgb, void* stream);
+/* neo_mip_composite_bwd (the same d_raw_density / d_raw_rgb bits) that also returns g_rays_d (n,3): the intervals are scaled by |rays_d|,
+ * so dL/d|d| = sum_k dL/dx_k x_k / |d| over x_k = density_k (t_{k+1} - t_k) |d| of the finite intervals, g_rays_d = dL/d|d| d / |d|.
+ * Fixed-order per-ray sum, no atomics. */
+int neo_mip_composite_bwd_rays_d(const float* raw_density, const float* raw_rgb, const float* tdist, const float* rays_d, int n_rays, int N,
+                                 const float* g_rgb, const float* g_weights, const float* g_density, const float* g_rgb_s, float* d_raw_density,
+                                 float* d_raw_rgb, float* g_rays_d, void* stream);
 /* One MLP of Mip-NeRF 360 (level 0, 1: PropMLP; 2: NeRFMLP) at caller-given points.  The MLP reads a Gaussian: here its mean is the point
  * rays_o[b] + t_vals[b, s] * viewdirs[b] (fp32, each operation rounded; rays_d is not read) and its covariance diag(var), var >= 0 per
  * axis.  The Gaussian goes through the render's own encoding (contraction with its Jacobian, 21-direction lift, 12-octave IPE), then the

@@ -114,6 +114,8 @@ SYMBOLS = {
                                      C.c_void_p]),
     "neo_index_maps_bwd_det_workspace_bytes": (C.c_size_t, [C.c_void_p, C.c_int, C.c_int]),
     "neo_index_maps_bwd_det": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 7 + [C.c_size_t, C.c_void_p]),
+    "neo_sample_rays_bwd_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "neo_sample_rays_bwd": (C.c_int, [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float] + [C.c_void_p] * 6 + [C.c_size_t, C.c_void_p]),
     "neo_get_rays": (C.c_int, [C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_intersect_sphere": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_sample_along_rays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -151,6 +153,7 @@ SYMBOLS = {
                                          C.c_size_t, C.c_void_p]),
     "neo_vanilla_sample_along_rays": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_vanilla_encode": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "neo_vanilla_encode_bwd": (C.c_int, [C.c_void_p] * 3 + [C.c_int] * 2 + [C.c_void_p] * 5),
     "neo_pixelnerf_field": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(NeoPixelMLPParams), C.POINTER(NeoRays), C.c_void_p, C.c_int, C.c_void_p,
                                       C.c_void_p, C.c_void_p]),
     "neo_pixelnerf_tc_workspace_bytes": (C.c_size_t, [C.c_int, C.c_longlong]),
@@ -166,6 +169,8 @@ SYMBOLS = {
     "neo_mip_encode": (C.c_int, [C.c_void_p] * 6 + [C.c_int] * 2 + [C.c_void_p] * 3),
     "neo_mip_composite": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 2 + [C.c_void_p] * 5),
     "neo_mip_composite_bwd": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 2 + [C.c_void_p] * 7),
+    "neo_mip_composite_bwd_rays_d": (C.c_int, [C.c_void_p] * 4 + [C.c_int] * 2 + [C.c_void_p] * 8),
+    "neo_mip_encode_bwd": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "neo_mip_field_workspace_bytes": (C.c_size_t, [C.c_longlong, C.c_int, C.c_int]),
     "neo_mip_field_eval": (C.c_int, [C.POINTER(NeoMipMLPParams), C.c_int, C.POINTER(NeoRays), C.c_void_p, C.c_int, C.POINTER(C.c_float), C.c_int,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -190,6 +190,18 @@ __device__ __forceinline__ float pos_enc_col(const float* x, int ich, int deg, i
     const float xb = mul_(x[q % ich], (float)(1 << (q / ich)));
     return sinf(shifted ? add_(xb, 1.57079637f) : xb);
 }
+// dL/dx_j of one row of pos_enc_col's encoding of x (ich coordinates, deg octaves) whose upstream gradient is g: the identity
+// column, then 2^k cos(2^k x_j) for sin(2^k x_j) and -2^k sin(2^k x_j) for its shifted twin sin(2^k x_j + pi/2).  2^k x_j is exact.
+__device__ __forceinline__ float pos_enc_grad(float xj, const float* __restrict__ g, int j, int ich, int deg) {
+    float s = g[j];
+    for (int k = 0; k < deg; ++k) {
+        const float sc = (float)(1 << k);
+        float sn, cs;
+        sincosf(mul_(xj, sc), &sn, &cs);
+        s += sc * (g[ich + ich * k + j] * cs - g[ich + ich * deg + ich * k + j] * sn);
+    }
+    return s;
+}
 
 // Head activations of the reference MLPs: density = softplus_(raw - 1), rgb = rgb_act(raw)   (models/neo360/model.py:392-397)
 __device__ __forceinline__ float softplus_(float x) { return x > 20.f ? x : log1pf(expf(x)); }
@@ -294,6 +306,9 @@ int launch_sample_rays(int n, const long long* pix, int T, int H, int W, float f
                        float* o, float* vd, float* rd, float* radii, float* target, int* err, cudaStream_t s);
 int launch_get_rays(int H, int W, float focal, const float* c2w, float* o, float* vd, float* rd, float* radii,
                     cudaStream_t s);
+size_t sample_rays_bwd_workspace(int n, int T);
+int launch_sample_rays_bwd(int n, const long long* pix, int T, int H, int W, float focal, const float* c2w, const float* g_o, const float* g_vd,
+                           const float* g_rd, float* g_c2w, void* ws, cudaStream_t s);
 // field_fp32.cu
 int launch_field_fp32(const NeoScene* sc, const NeoRays* rays, const float* far, const float* t, int N, int mlp_index,
                       float* rgb, float* sigma, cudaStream_t s);

@@ -434,7 +434,7 @@ __global__ void composite_kernel(const float* __restrict__ raw_density, const fl
 __global__ void composite_bwd_kernel(const float* __restrict__ raw_density, const float* __restrict__ raw_rgb, const float* __restrict__ tdist,
                                      const float* __restrict__ rays_d, int n_rays, int n, const float* __restrict__ g_rgb,
                                      const float* __restrict__ g_w, const float* __restrict__ g_density, const float* __restrict__ g_rgb_s,
-                                     float* __restrict__ d_raw_density, float* __restrict__ d_raw_rgb) {
+                                     float* __restrict__ d_raw_density, float* __restrict__ d_raw_rgb, float* __restrict__ g_rays_d) {
     const int warps = blockDim.x / 32, wid = threadIdx.x / 32, lane = threadIdx.x % 32;
     const int b = blockIdx.x * warps + wid;
     if (b >= n_rays) return;
@@ -468,12 +468,14 @@ __global__ void composite_bwd_kernel(const float* __restrict__ raw_density, cons
     const float gc[3] = {g_rgb ? g_rgb[3 * b] : 0.f, g_rgb ? g_rgb[3 * b + 1] : 0.f, g_rgb ? g_rgb[3 * b + 2] : 0.f};
     const float gbg = (1.f - acc >= 0.f) ? gc[0] + gc[1] + gc[2] : 0.f;
     float S = 0.f;                                              // sum_{j >= next chunk} G_j w_j
+    float gdn = 0.f;                                            // sum_k dL/dx_k x_k (g_rays_d only)
     for (int base = ((n - 1) / 32) * 32; base >= 0; base -= 32) {
         const int k = base + lane;
         const bool ok = k < n;
-        float v = 0.f, dx = 0.f, delta = 0.f, w = 0.f, T = 0.f, e = 0.f, s[3] = {0.f, 0.f, 0.f};
+        float v = 0.f, dx = 0.f, delta = 0.f, w = 0.f, T = 0.f, e = 0.f, s[3] = {0.f, 0.f, 0.f}, xk = 0.f;
         if (ok) {
             const float dd = x_of(k, delta);
+            xk = (k == n - 1) ? 0.f : dd;
             T = expf(-gd[k]);
             e = expf(-dd);
             w = (1.f - e) * T;
@@ -494,6 +496,7 @@ __global__ void composite_bwd_kernel(const float* __restrict__ raw_density, cons
         const float chunk = __shfl_sync(0xffffffffu, incl, 0);
         if (ok) {
             dx = (k == n - 1) ? 0.f : dx - (after + S);
+            gdn += dx * xk;
             const float z = rd[k] - 1.0f;
             const float sp = z > 20.f ? 1.f : 1.f / (1.f + expf(-z));            // softplus'(z), threshold 20 as F.softplus
             gd[k] = (delta * dx + (g_density ? g_density[(size_t)b * n + k] : 0.f)) * sp;
@@ -506,6 +509,20 @@ __global__ void composite_bwd_kernel(const float* __restrict__ raw_density, cons
         }
         S += chunk;
     }
+    if (g_rays_d) {
+        // x_k = density_k (t_{k+1} - t_k) |d| (k < N-1): dL/d|d| = sum_k dL/dx_k x_k / |d|, and g_d = dL/d|d| d / |d|
+        gdn = warp_sum(gdn);
+        if (lane < 3) g_rays_d[3 * b + lane] = gdn / dn * (dd3[lane] / dn);
+    }
+}
+
+// Backward of dir_kernel's encoding (the reference differentiates viewdirs through dir_enc_fn, model.py:152): one thread per ray and
+// coordinate, g_viewdirs = d pos_enc(viewdirs, 0, 4) / d viewdirs applied to g_dir_enc
+__global__ void dir_enc_bwd_kernel(const float* __restrict__ viewdirs, int n, const float* __restrict__ g_dir, float* __restrict__ g_vd) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n * 3) return;
+    const int b = i / 3, j = i % 3;
+    g_vd[i] = pos_enc_grad(viewdirs[i], g_dir + (size_t)b * kDirEnc, j, 3, 4);
 }
 
 }  // namespace mip
@@ -751,9 +768,10 @@ extern "C" int neo_mip_field_eval(const NeoMipMLPParams mlps[3], int level, cons
     return NEO_OK;
 }
 
-// ---- stage-level entry points of the training path (neo360_b200/mip.py): resampling and encodings have no backward (the sample positions
-// are detached, model.py:309-310, and contract returns detached values, helper.py:63-66); compositing forward is composite_kernel itself and
-// its backward composite_bwd_kernel; the dense layers are differentiated by the host framework ----
+// ---- stage-level entry points of the training path (neo360_b200/mip.py): resampling and the IPE features have no backward (the sample
+// positions are detached, model.py:309-310, and contract returns detached values, helper.py:63-66); the direction encoding's backward
+// w.r.t. viewdirs is dir_enc_bwd_kernel; compositing forward is composite_kernel itself and its backward composite_bwd_kernel (with the
+// |rays_d| term on request); the dense layers are differentiated by the host framework ----
 extern "C" int neo_mip_resample(const float* sdist_prev, const float* weights_prev, int n_rays, int n_prev, int level, int n_new, float near_plane,
                                 float far_plane, float train_frac, const float* jitter, float* sdist, float* tdist, void* stream) {
     if (level < 0 || level > 2) { set_error("neo_mip_resample: level must be 0, 1 or 2 (got %d)", level); return NEO_ERR_INVALID; }
@@ -801,7 +819,27 @@ extern "C" int neo_mip_composite_bwd(const float* raw_density, const float* raw_
         return NEO_ERR_INVALID;
     }
     mip::composite_bwd_kernel<<<(n_rays + kCompWarps - 1) / kCompWarps, kCompWarps * 32, 0, (cudaStream_t)stream>>>(
-        raw_density, raw_rgb, tdist, rays_d, n_rays, N, g_rgb, g_weights, g_density, g_rgb_s, d_raw_density, d_raw_rgb);
+        raw_density, raw_rgb, tdist, rays_d, n_rays, N, g_rgb, g_weights, g_density, g_rgb_s, d_raw_density, d_raw_rgb, nullptr);
     NEO_LAUNCH_CHECK("mip composite_bwd_kernel");
+    return NEO_OK;
+}
+
+extern "C" int neo_mip_composite_bwd_rays_d(const float* raw_density, const float* raw_rgb, const float* tdist, const float* rays_d, int n_rays,
+                                            int N, const float* g_rgb, const float* g_weights, const float* g_density, const float* g_rgb_s,
+                                            float* d_raw_density, float* d_raw_rgb, float* g_rays_d, void* stream) {
+    if (!raw_density || !tdist || !rays_d || !d_raw_density || (raw_rgb && !d_raw_rgb) || !g_rays_d || n_rays <= 0 || N < 1) {
+        set_error("neo_mip_composite_bwd_rays_d: bad arguments");
+        return NEO_ERR_INVALID;
+    }
+    mip::composite_bwd_kernel<<<(n_rays + kCompWarps - 1) / kCompWarps, kCompWarps * 32, 0, (cudaStream_t)stream>>>(
+        raw_density, raw_rgb, tdist, rays_d, n_rays, N, g_rgb, g_weights, g_density, g_rgb_s, d_raw_density, d_raw_rgb, g_rays_d);
+    NEO_LAUNCH_CHECK("mip composite_bwd_kernel");
+    return NEO_OK;
+}
+
+extern "C" int neo_mip_encode_bwd(const float* viewdirs, int n_rays, const float* g_dir_enc, float* g_viewdirs, void* stream) {
+    if (!viewdirs || !g_dir_enc || !g_viewdirs || n_rays <= 0) { set_error("neo_mip_encode_bwd: bad arguments"); return NEO_ERR_INVALID; }
+    mip::dir_enc_bwd_kernel<<<(n_rays * 3 + 255) / 256, 256, 0, (cudaStream_t)stream>>>(viewdirs, n_rays, g_dir_enc, g_viewdirs);
+    NEO_LAUNCH_CHECK("mip dir_enc_bwd_kernel");
     return NEO_OK;
 }

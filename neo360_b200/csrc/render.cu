@@ -172,6 +172,24 @@ extern "C" int neo_sample_rays(int n, const long long* pix_inds, int n_views, in
     return launch_sample_rays(n, pix_inds, n_views, H, W, focal, c2w, images, rays_o, viewdirs, rays_d, radii, target, err_flag,
                               (cudaStream_t)stream);
 }
+extern "C" size_t neo_sample_rays_bwd_workspace_bytes(int n, int n_views) {
+    if (n < 0 || n_views < 1) { set_error("neo_sample_rays_bwd_workspace_bytes: need n >= 0 and n_views >= 1"); return 0; }
+    return sample_rays_bwd_workspace(n, n_views);
+}
+extern "C" int neo_sample_rays_bwd(int n, const long long* pix_inds, int n_views, int H, int W, float focal, const float* c2w, const float* g_rays_o,
+                                   const float* g_viewdirs, const float* g_rays_d, float* g_c2w, void* workspace, size_t workspace_bytes,
+                                   void* stream) {
+    if (n < 0 || n_views < 1 || H < 2 || W < 1 || !c2w || !g_c2w || (n > 0 && !pix_inds)) {
+        set_error("neo_sample_rays_bwd: bad arguments");
+        return NEO_ERR_INVALID;
+    }
+    const size_t need = sample_rays_bwd_workspace(n, n_views);
+    if (n > 0 && (!workspace || workspace_bytes < need)) {
+        set_error("neo_sample_rays_bwd: workspace of %zu bytes, %zu needed", workspace_bytes, need);
+        return NEO_ERR_WORKSPACE;
+    }
+    return launch_sample_rays_bwd(n, pix_inds, n_views, H, W, focal, c2w, g_rays_o, g_viewdirs, g_rays_d, g_c2w, workspace, (cudaStream_t)stream);
+}
 extern "C" int neo_intersect_sphere(const float* o, const float* d, int n, float* far, int* err_flag, void* stream) {
     if (n <= 0) { set_error("neo_intersect_sphere: n_rays <= 0"); return NEO_ERR_INVALID; }
     return launch_far(o, d, n, far, err_flag, (cudaStream_t)stream);

@@ -84,6 +84,100 @@ int launch_sample_rays(int n, const long long* pix, int T, int H, int W, float f
     return NEO_OK;
 }
 
+// Backward of ray_at w.r.t. the 3x4 camera-to-world matrix m = [R | t]: pass 1 writes each ray's 12 terms and its view, pass 2 sums
+// each block's chunk of rays per view, pass 3 sums the block partials per view in block order (no atomics).  With c the camera-frame
+// direction, d = R c, v = d / |d| (viewdirs and rays_d):
+//   g_d = (g_v - v (v . g_v)) / |d|,   g_R[r][k] = g_d[r] c[k],   g_t = g_rays_o.
+__global__ void sample_rays_bwd_terms_kernel(int n, const long long* __restrict__ pix, int T, int H, int W, float focal,
+                                             const float* __restrict__ c2w, const float* __restrict__ g_o, const float* __restrict__ g_vd,
+                                             const float* __restrict__ g_rd, float* __restrict__ terms, int* __restrict__ view) {
+    const int q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= n) return;
+    const long long p = pix[q];
+    if (p < 0 || p >= (long long)T * H * W) { view[q] = -1; return; }
+    const int t = (int)(p / ((long long)H * W)), r = (int)(p % ((long long)H * W)), i = r % W, j = r / W;
+    const float* m = c2w + t * 12;
+    const float c[3] = {__fdiv_rn(sub_((float)i, (float)W / 2.f), focal), -__fdiv_rn(sub_((float)j, (float)H / 2.f), focal), -1.0f};
+    float d[3], v[3], gv[3];
+    raw_dir(i, j, H, W, focal, m, d);
+    const float nrm = __fsqrt_rn(dot3_(d, d));
+    for (int k = 0; k < 3; ++k) {
+        v[k] = __fdiv_rn(d[k], nrm);
+        gv[k] = (g_vd ? g_vd[(size_t)q * 3 + k] : 0.f) + (g_rd ? g_rd[(size_t)q * 3 + k] : 0.f);
+    }
+    const float vg = v[0] * gv[0] + v[1] * gv[1] + v[2] * gv[2];
+    float* out = terms + (size_t)q * 12;
+    for (int rr = 0; rr < 3; ++rr) {
+        const float gd = (gv[rr] - v[rr] * vg) / nrm;
+        for (int k = 0; k < 3; ++k) out[rr * 4 + k] = gd * c[k];
+        out[rr * 4 + 3] = g_o ? g_o[(size_t)q * 3 + rr] : 0.f;
+    }
+    view[q] = t;
+}
+
+constexpr int kRaysBwdThreads = 256, kRaysBwdPerThread = 8, kRaysBwdChunk = kRaysBwdThreads * kRaysBwdPerThread;
+// Pass 2: block b sums, for every view, the terms of its chunk of rays (thread k: rays k, k + 256, ... of the chunk in order, then a
+// fixed tree) into part[b][view][12].
+__global__ void __launch_bounds__(kRaysBwdThreads) sample_rays_bwd_partial_kernel(int n, int T, const float* __restrict__ terms,
+                                                                                  const int* __restrict__ view, float* __restrict__ part) {
+    __shared__ float red[kRaysBwdThreads][13];
+    const int tid = threadIdx.x, q0 = blockIdx.x * kRaysBwdChunk;
+    for (int t = 0; t < T; ++t) {
+        float acc[12];
+#pragma unroll
+        for (int e = 0; e < 12; ++e) acc[e] = 0.f;
+#pragma unroll
+        for (int k = 0; k < kRaysBwdPerThread; ++k) {
+            const int q = q0 + k * kRaysBwdThreads + tid;
+            if (q < n && view[q] == t)
+#pragma unroll
+                for (int e = 0; e < 12; ++e) acc[e] += terms[(size_t)q * 12 + e];
+        }
+#pragma unroll
+        for (int e = 0; e < 12; ++e) red[tid][e] = acc[e];
+        __syncthreads();
+        for (int s = kRaysBwdThreads / 2; s > 0; s >>= 1) {
+            if (tid < s)
+                for (int e = 0; e < 12; ++e) red[tid][e] += red[tid + s][e];
+            __syncthreads();
+        }
+        if (tid < 12) part[((size_t)blockIdx.x * T + t) * 12 + tid] = red[0][tid];
+        __syncthreads();
+    }
+}
+// Pass 3: g_c2w[view][e] = the blocks' partials summed in block order.
+__global__ void sample_rays_bwd_sum_kernel(int nb, int T, const float* __restrict__ part, float* __restrict__ g_c2w) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= T * 12) return;
+    float s = 0.f;
+    for (int b = 0; b < nb; ++b) s += part[(size_t)b * T * 12 + i];
+    g_c2w[i] = s;
+}
+
+static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+static int rays_bwd_blocks(int n) { return n > 0 ? (n + kRaysBwdChunk - 1) / kRaysBwdChunk : 0; }
+size_t sample_rays_bwd_workspace(int n, int T) {
+    return align256((size_t)n * 12 * sizeof(float)) + align256((size_t)n * sizeof(int)) + (size_t)rays_bwd_blocks(n) * T * 12 * sizeof(float);
+}
+
+int launch_sample_rays_bwd(int n, const long long* pix, int T, int H, int W, float focal, const float* c2w, const float* g_o, const float* g_vd,
+                           const float* g_rd, float* g_c2w, void* ws, cudaStream_t s) {
+    unsigned char* p = (unsigned char*)ws;
+    float* terms = (float*)p;
+    int* view = (int*)(p + align256((size_t)n * 12 * sizeof(float)));
+    float* part = (float*)(p + align256((size_t)n * 12 * sizeof(float)) + align256((size_t)n * sizeof(int)));
+    const int nb = rays_bwd_blocks(n);
+    if (n > 0) {
+        sample_rays_bwd_terms_kernel<<<(n + 255) / 256, 256, 0, s>>>(n, pix, T, H, W, focal, c2w, g_o, g_vd, g_rd, terms, view);
+        NEO_LAUNCH_CHECK("sample_rays_bwd_terms_kernel");
+        sample_rays_bwd_partial_kernel<<<nb, kRaysBwdThreads, 0, s>>>(n, T, terms, view, part);
+        NEO_LAUNCH_CHECK("sample_rays_bwd_partial_kernel");
+    }
+    sample_rays_bwd_sum_kernel<<<(T * 12 + 255) / 256, 256, 0, s>>>(nb, T, part, g_c2w);
+    NEO_LAUNCH_CHECK("sample_rays_bwd_sum_kernel");
+    return NEO_OK;
+}
+
 // ------------------------------------------------------------------------------------------------
 // a3  intersect_sphere   (helper.py:253-273)
 // ------------------------------------------------------------------------------------------------

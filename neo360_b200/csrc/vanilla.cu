@@ -223,6 +223,36 @@ __global__ void encode_kernel(const float* __restrict__ rays_o, const float* __r
     }
 }
 
+// Backward of encode_kernel w.r.t. the ray: one warp per ray, lane l takes samples l, l + 32, ... in order, then a fixed butterfly.
+// x = o + t viewdirs (field_kernel's own rounding), so g_o = sum dL/dx and g_viewdirs = sum t dL/dx + the direction encoding's term.
+constexpr int kBwdRays = 8;
+__global__ void __launch_bounds__(kBwdRays * 32) encode_bwd_kernel(const float* __restrict__ rays_o, const float* __restrict__ viewdirs,
+                                                                   const float* __restrict__ tvals, int n, int N, const float* __restrict__ g_enc,
+                                                                   const float* __restrict__ g_dir, float* __restrict__ g_o, float* __restrict__ g_vd) {
+    const int b = blockIdx.x * kBwdRays + threadIdx.x / 32, lane = threadIdx.x % 32;
+    if (b >= n) return;
+    float o[3], v[3], go[3] = {0.f, 0.f, 0.f}, gv[3] = {0.f, 0.f, 0.f};
+    for (int j = 0; j < 3; ++j) { o[j] = rays_o[3 * b + j]; v[j] = viewdirs[3 * b + j]; }
+    for (int k = lane; k < N; k += 32) {
+        const long long m = (long long)b * N + k;
+        const float t = tvals[m];
+        const float* g = g_enc + m * kEnc;
+        for (int j = 0; j < 3; ++j) {
+            const float gx = pos_enc_grad(add_(o[j], mul_(t, v[j])), g, j, 3, 10);
+            go[j] += gx;
+            gv[j] += t * gx;
+        }
+    }
+    for (int j = 0; j < 3; ++j) { go[j] = warp_sum(go[j]); gv[j] = warp_sum(gv[j]); }
+    if (lane < 3) {
+        const float vj = lane == 0 ? v[0] : (lane == 1 ? v[1] : v[2]);
+        const float goj = lane == 0 ? go[0] : (lane == 1 ? go[1] : go[2]);
+        const float gvj = lane == 0 ? gv[0] : (lane == 1 ? gv[1] : gv[2]);
+        g_o[3 * b + lane] = goj;
+        g_vd[3 * b + lane] = gvj + pos_enc_grad(vj, g_dir + (size_t)b * kDirEnc, lane, 3, 4);
+    }
+}
+
 }  // namespace van
 }  // namespace neo
 
@@ -422,7 +452,8 @@ extern "C" int neo_vanilla_field_eval(const NeoVanilla* v, const NeoRays* rays, 
     return field(v->mlp[level], rays->rays_o, rays->viewdirs, t_vals, rays->n_rays, N, precision, w, rgb, sigma, (cudaStream_t)stream);
 }
 
-// ---- stage-level entry points of the training path (neo360_b200/vanilla.py): sampling and encodings have no backward; the compositing
+// ---- stage-level entry points of the training path (neo360_b200/vanilla.py): sampling has no backward, the encodings' backward w.r.t. the
+// rays is encode_bwd_kernel (pose refinement); the compositing
 // backward is composite_bwd_kernel in mode 2 (csrc/sampling.cu); the dense layers are differentiated by the host framework ----
 extern "C" int neo_vanilla_sample_along_rays(const float* rays_o, const float* viewdirs, int n_rays, int n_coarse, float near_plane, float far_plane,
                                              const float* u_rand, float* t_vals, void* stream) {
@@ -440,6 +471,18 @@ extern "C" int neo_vanilla_encode(const float* rays_o, const float* viewdirs, co
     const long long total = (long long)n_rays * N * van::kEnc + (long long)n_rays * kDirEnc;
     van::encode_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(rays_o, viewdirs, t_vals, n_rays, N, enc, dir_enc);
     NEO_LAUNCH_CHECK("vanilla encode_kernel");
+    return NEO_OK;
+}
+
+extern "C" int neo_vanilla_encode_bwd(const float* rays_o, const float* viewdirs, const float* t_vals, int n_rays, int N, const float* g_enc,
+                                      const float* g_dir_enc, float* g_rays_o, float* g_viewdirs, void* stream) {
+    if (!rays_o || !viewdirs || !t_vals || !g_enc || !g_dir_enc || !g_rays_o || !g_viewdirs || n_rays <= 0 || N < 1) {
+        set_error("neo_vanilla_encode_bwd: bad arguments");
+        return NEO_ERR_INVALID;
+    }
+    van::encode_bwd_kernel<<<(unsigned)((n_rays + van::kBwdRays - 1) / van::kBwdRays), van::kBwdRays * 32, 0, (cudaStream_t)stream>>>(
+        rays_o, viewdirs, t_vals, n_rays, N, g_enc, g_dir_enc, g_rays_o, g_viewdirs);
+    NEO_LAUNCH_CHECK("vanilla encode_bwd_kernel");
     return NEO_OK;
 }
 

@@ -12,7 +12,12 @@ and `weights` of every level and each level's rendered `rgb` carry gradients, `s
 levels' `rgb` are zeros.  Resampling, IPE features, direction encoding and compositing forward and backward are hand-written CUDA; the
 dense layers are framework fp32 GEMMs under autograd, or with `train_precision="tc"` bf16 tensor-core GEMMs forward and backward
 (training._MLPTrainTC, csrc/dense_train.cu).  `precision` applies to inference only.
-`training_loss` is the reference's training loss on those outputs."""
+`training_loss` is the reference's training loss on those outputs.
+Ray gradients, as the reference's plain-PyTorch module has them: when grad is enabled and a ray tensor requires grad, `forward` takes the
+autograd path (also with frozen parameters or in eval mode).  `viewdirs` gets the gradient of its direction encoding (`neo_mip_encode_bwd`)
+and `rays_d` that of the |rays_d| scaling of the intervals (`neo_mip_composite_bwd_rays_d`).  The reference's `contract` returns detached
+Gaussians (models/mipnerf360/helper.py:63-66), so, as there, `rays_o` and `radii` get no gradient and `rays_d` none through the frustums
+(DESIGN.md section 12)."""
 from __future__ import annotations
 
 import ctypes as C
@@ -24,7 +29,7 @@ import torch.nn.functional as F
 
 from . import _lib as L
 from .mip_basis import POS_BASIS_T
-from .training import check_train_precision, distortion_loss, mlp_train_tc
+from .training import check_train_precision, distortion_loss, mlp_train_tc, rays_need_grad
 
 
 class MipNeRF360MLP(nn.Module):
@@ -85,7 +90,7 @@ class MipNeRF360(nn.Module):
         self._ws = None
 
     def forward(self, batch: Dict[str, torch.Tensor], train_frac: float, randomized: bool, is_train: bool, near, far) -> Tuple[List[dict], List[dict]]:
-        if torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters()):
+        if torch.is_grad_enabled() and ((self.training and any(p.requires_grad for p in self.parameters())) or rays_need_grad(batch)):
             return self._forward_train(batch, train_frac, randomized, near, far)
         o = batch["rays_o"].contiguous().float()
         if not o.is_cuda:
@@ -194,10 +199,13 @@ class MipNeRF360(nn.Module):
                 L.check(lib.neo_mip_resample(L.ptr(sdist), L.ptr(wp), n, ns[lvl - 1] if lvl else 1, lvl, N, float(near), float(far),
                                              float(train_frac), L.ptr(jit[lvl]), L.ptr(s1), L.ptr(t1), stream))
                 sdist = s1
-                feats, denc = torch.empty(n * N, 504, device=dev), torch.empty(n, 27, device=dev)
                 basis = mlp.pos_basis_t.to(dev).contiguous().float()
-                L.check(lib.neo_mip_encode(L.ptr(o), L.ptr(d), L.ptr(vd), L.ptr(radii), L.ptr(t1), L.ptr(basis), n, N, L.ptr(feats), L.ptr(denc),
-                                           stream))
+                if vd.requires_grad:
+                    feats, denc = _MipEncode.apply(o, d, vd, radii, t1, basis)
+                else:
+                    feats, denc = torch.empty(n * N, 504, device=dev), torch.empty(n, 27, device=dev)
+                    L.check(lib.neo_mip_encode(L.ptr(o), L.ptr(d), L.ptr(vd), L.ptr(radii), L.ptr(t1), L.ptr(basis), n, N, L.ptr(feats),
+                                               L.ptr(denc), stream))
             if tc:
                 raw_density, raw_rgb = mlp_train_tc(mlp, feats, denc, n, N)
                 raw_density = raw_density.reshape(n, N)
@@ -230,6 +238,36 @@ def _mlp_train(m: MipNeRF360MLP, feats: torch.Tensor, denc: torch.Tensor, n: int
     return raw_density, lin(m.rgb_layer, torch.relu(y))
 
 
+class _MipEncode(torch.autograd.Function):
+    """neo_mip_encode under autograd: (rays_o, rays_d, viewdirs (n,3), radii (n), tdist (n,N+1), basis) -> feats (n*N, 504), dir_enc (n, 27).
+    The backward (neo_mip_encode_bwd) gives viewdirs the gradient of its direction encoding; the IPE features give the rays none, as the
+    reference's detached `contract` (helper.py:63-66)."""
+
+    @staticmethod
+    def forward(ctx, o, d, vd, radii, tdist, basis):
+        lib = L.load()
+        o, d, vd, radii, tdist = (x.detach().contiguous().float() for x in (o, d, vd, radii, tdist))
+        n, N = tdist.shape[0], tdist.shape[1] - 1
+        feats, denc = torch.empty(n * N, 504, device=o.device), torch.empty(n, 27, device=o.device)
+        with torch.cuda.device(o.device):
+            L.check(lib.neo_mip_encode(L.ptr(o), L.ptr(d), L.ptr(vd), L.ptr(radii), L.ptr(tdist), L.ptr(basis), n, N, L.ptr(feats), L.ptr(denc),
+                                       torch.cuda.current_stream(o.device).cuda_stream))
+        ctx.save_for_backward(vd)
+        return feats, denc
+
+    @staticmethod
+    def backward(ctx, g_feats, g_denc):
+        lib = L.load()
+        (vd,) = ctx.saved_tensors
+        n = vd.shape[0]
+        g_vd = torch.zeros(n, 3, device=vd.device)
+        if g_denc is not None:
+            with torch.cuda.device(vd.device):
+                L.check(lib.neo_mip_encode_bwd(L.ptr(vd), n, L.ptr(g_denc.contiguous().float()), L.ptr(g_vd),
+                                               torch.cuda.current_stream(vd.device).cuda_stream))
+        return None, None, g_vd, None, None, None
+
+
 class _MipComposite(torch.autograd.Function):
     """Head activations + compute_alpha_weights(opaque_background) + volumetric_rendering, white background (helper.py:234-274):
     raw density (n,N), raw rgb (n,N,3) or None (proposal level), tdist (n,N+1), rays_d (n,3) -> rgb (n,3), weights (n,N), density (n,N),
@@ -248,6 +286,7 @@ class _MipComposite(torch.autograd.Function):
             L.check(lib.neo_mip_composite(L.ptr(rd), L.ptr(rc), L.ptr(t), L.ptr(d), n, N, L.ptr(rgb), L.ptr(w), L.ptr(dens), L.ptr(rgb_s),
                                           torch.cuda.current_stream(dev).cuda_stream))
         ctx.save_for_backward(rd, rc, t, d)
+        ctx.want_d = rays_d.requires_grad
         if rc is None:
             ctx.mark_non_differentiable(rgb_s)
         return rgb, w, dens, rgb_s
@@ -261,11 +300,17 @@ class _MipComposite(torch.autograd.Function):
         d_rd = torch.empty(n, N, device=dev)
         d_rc = torch.empty(n, N, 3, device=dev) if rc is not None else None
         f = lambda g: None if g is None else g.contiguous().float()
+        gs = [L.ptr(f(g_rgb)), L.ptr(f(g_w)), L.ptr(f(g_dens)), L.ptr(f(g_rgb_s) if rc is not None else None)]
+        g_d = None
         with torch.cuda.device(dev):
-            L.check(lib.neo_mip_composite_bwd(L.ptr(rd), L.ptr(rc), L.ptr(t), L.ptr(d), n, N, L.ptr(f(g_rgb)), L.ptr(f(g_w)), L.ptr(f(g_dens)),
-                                              L.ptr(f(g_rgb_s) if rc is not None else None), L.ptr(d_rd), L.ptr(d_rc),
-                                              torch.cuda.current_stream(dev).cuda_stream))
-        return d_rd, d_rc, None, None
+            if ctx.needs_input_grad[3]:
+                g_d = torch.empty(n, 3, device=dev)
+                L.check(lib.neo_mip_composite_bwd_rays_d(L.ptr(rd), L.ptr(rc), L.ptr(t), L.ptr(d), n, N, *gs, L.ptr(d_rd), L.ptr(d_rc), L.ptr(g_d),
+                                                         torch.cuda.current_stream(dev).cuda_stream))
+            else:
+                L.check(lib.neo_mip_composite_bwd(L.ptr(rd), L.ptr(rc), L.ptr(t), L.ptr(d), n, N, *gs, L.ptr(d_rd), L.ptr(d_rc),
+                                                  torch.cuda.current_stream(dev).cuda_stream))
+        return d_rd, d_rc, None, g_d
 
 
 def _outer_weights(t: torch.Tensor, t_env: torch.Tensor, w_env: torch.Tensor) -> torch.Tensor:

@@ -5,8 +5,8 @@
     sample_along_rays       models/neo360/helper.py:24-75
     sample_pdf              models/neo360/helper.py:218-249
     volumetric_rendering    models/neo360/helper.py:128-171
-    get_rays                datasets/ray_utils.py:84-104,133-176
-    sample_rays             datasets/nerds360_ae.py:730-748 (pixel sampling of a training batch)
+    get_rays                datasets/ray_utils.py:84-104,133-176 (differentiable w.r.t. c2w when it requires grad)
+    sample_rays             datasets/nerds360_ae.py:730-748 (pixel sampling of a training batch; differentiable w.r.t. c2w likewise)
     index_grid / get_local_feats / field_eval   need a Scene (see renderer.py)
 
 CUDA only; there is no CPU fallback."""
@@ -39,8 +39,61 @@ def _f32(t):
     return t.contiguous().float()
 
 
+class _RaysFromPoses(torch.autograd.Function):
+    """neo_sample_rays under autograd w.r.t. c2w (T,3,4): the same kernel and the same bits forward, `neo_sample_rays_bwd` backward (a
+    fixed-order reduction per view).  radii and target carry no gradient: radii does not change under a rotation of the pose or a
+    translation, so a pose correction loses nothing by it."""
+
+    @staticmethod
+    def forward(ctx, c2w, pix, H, W, focal, img, check):
+        lib = L.load()
+        m = c2w.detach().contiguous().float()
+        n, T = pix.numel(), m.shape[0]
+        o = torch.empty(n, 3, device=m.device); vd = torch.empty_like(o); rd = torch.empty_like(o)
+        rad = torch.empty(n, 1, device=m.device)
+        tgt = torch.empty(n, 3, device=m.device) if img is not None else None
+        err = torch.zeros(1, dtype=torch.int32, device=m.device)
+        with _on(m):
+            L.check(lib.neo_sample_rays(n, pix.data_ptr(), T, H, W, float(focal), L.ptr(m), L.ptr(img), L.ptr(o), L.ptr(vd), L.ptr(rd),
+                                        L.ptr(rad), L.ptr(tgt), L.ptr(err), _stream()))
+        if check and int(err.item()):   # the reference's fancy indexing raises IndexError synchronously
+            raise IndexError("sample_rays: pix_inds out of range")
+        ctx.save_for_backward(m, pix)
+        ctx.dims = (H, W, float(focal))
+        ctx.mark_non_differentiable(rad)
+        if tgt is None:
+            return o, vd, rd, rad
+        ctx.mark_non_differentiable(tgt)
+        return o, vd, rd, rad, tgt
+
+    @staticmethod
+    def backward(ctx, g_o, g_vd, g_rd, *_):
+        lib = L.load()
+        m, pix = ctx.saved_tensors
+        H, W, focal = ctx.dims
+        n, T = pix.numel(), m.shape[0]
+        f = lambda g: None if g is None else g.contiguous().float()
+        need = lib.neo_sample_rays_bwd_workspace_bytes(n, T)
+        ws = torch.empty(max(need, 1), dtype=torch.uint8, device=m.device)
+        g_c2w = torch.empty(T, 3, 4, device=m.device)
+        with _on(m):
+            L.check(lib.neo_sample_rays_bwd(n, pix.data_ptr(), T, H, W, focal, L.ptr(m), L.ptr(f(g_o)), L.ptr(f(g_vd)), L.ptr(f(g_rd)),
+                                            L.ptr(g_c2w), L.ptr(ws), need, _stream()))
+        return g_c2w, None, None, None, None, None, None
+
+
+def _pose_grad(c2w) -> bool:
+    return torch.is_grad_enabled() and c2w.requires_grad
+
+
 def get_rays(H, W, focal, c2w, output_radii=True):
-    """c2w (3,4) or (4,4) CUDA -> rays_o, viewdirs, rays_d, radii  (quirk Q3: rays_d == viewdirs, unit norm)."""
+    """c2w (3,4) or (4,4) CUDA -> rays_o, viewdirs, rays_d, radii  (quirk Q3: rays_d == viewdirs, unit norm).  When c2w requires grad
+    the rays are differentiable w.r.t. it (neo_sample_rays_bwd over the frame's pixels; the same bits forward); radii is not."""
+    if _pose_grad(c2w):
+        m = _f32(c2w[:3, :4])
+        pix = torch.arange(H * W, dtype=torch.int64, device=m.device)
+        o, vd, rd, rad = _RaysFromPoses.apply(m[None], pix, H, W, focal, None, False)
+        return (o, vd, rd, rad.reshape(-1)) if output_radii else (o, vd, rd)
     lib = L.load()
     m = _f32(c2w[:3, :4])
     n = H * W
@@ -53,7 +106,8 @@ def get_rays(H, W, focal, c2w, output_radii=True):
 
 def sample_rays(pix_inds, H, W, focal, c2w, images=None, check=True):
     """The `pix_inds`-selected rays of the (T, H, W) stack of target views (nerds360_ae.py:730-748) without building the stack.
-    pix_inds (n) int64 CUDA, c2w (T,3,4) CUDA, images (T,H,W,3) fp32 CUDA or None -> rays_o, viewdirs, rays_d, radii (n,1), target."""
+    pix_inds (n) int64 CUDA, c2w (T,3,4) CUDA, images (T,H,W,3) fp32 CUDA or None -> rays_o, viewdirs, rays_d, radii (n,1), target.
+    When c2w requires grad, rays_o, viewdirs and rays_d are differentiable w.r.t. it (neo_sample_rays_bwd; the same bits forward)."""
     lib = L.load()
     m = _f32(c2w[:, :3, :4])
     if not pix_inds.is_cuda or pix_inds.dtype != torch.int64:
@@ -65,6 +119,9 @@ def sample_rays(pix_inds, H, W, focal, c2w, images=None, check=True):
         img = _f32(images)
         if tuple(img.shape) != (T, H, W, 3):
             raise ValueError(f"sample_rays: images must be ({T}, {H}, {W}, 3), got {tuple(img.shape)}")
+    if _pose_grad(c2w):
+        out = _RaysFromPoses.apply(m, pix, H, W, focal, img, check)
+        return out if img is not None else (*out, None)
     o = torch.empty(n, 3, device=m.device); vd = torch.empty_like(o); rd = torch.empty_like(o)
     rad = torch.empty(n, 1, device=m.device)
     tgt = torch.empty(n, 3, device=m.device) if img is not None else None

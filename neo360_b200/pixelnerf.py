@@ -3,7 +3,8 @@
 `PixelNeRF.forward(rays, randomized, white_bkgd, near, far)` takes the NeO-360 batch dict (rays_o / rays_d / viewdirs and src_imgs /
 src_poses / src_focal / src_c, datasets/nerds360_ae.py with model_type="pixelnerf") and returns the reference's `list[2]` of
 `(comp_rgb, acc, depth)`.  Parameter names equal the reference's (`coarse_mlp.pts_linears.0.weight`, ..., `encoder.model.*`), so its
-checkpoints load.  CUDA only, no CPU fallback.
+checkpoints load.  CUDA only, no CPU fallback.  The rays get no gradient (unlike the reference's plain-PyTorch module): that needs the
+spatial gradient of the pixel-aligned lookup; vanilla NeRF has ray and pose gradients (DESIGN.md section 12).
 
 Inference: sampling, the per-level field (csrc/pixelnerf.cu, fp32 CUDA cores in the reference formulation) and compositing run in the
 library.  The encoder is hoisted: it runs once per `src_imgs` tensor and in-place version (the same deliberate difference as NeO-360's

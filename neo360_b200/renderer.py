@@ -1,4 +1,6 @@
-"""Drop-in for the reference's NeO-360 renderer behind its own call surface.
+"""Drop-in for the reference's NeO-360 renderer behind its own call surface.  The rays get no gradient (unlike the reference's plain
+PyTorch): that needs the spatial gradient of the tri-plane and projected-map lookups; vanilla NeRF has ray and pose gradients
+(DESIGN.md section 12).
 
     reference                                         here
     ---------------------------------------------     ------------------------------------------------

@@ -179,7 +179,11 @@ class _Composite(torch.autograd.Function):
                 gs = [f(g_comp), f(g_acc), f(g_w), f(g_lam) if mode else None, f(g_depth)]
                 L.check(lib.neo_volumetric_rendering_bwd(L.ptr(rgb_c), L.ptr(sig_c), L.ptr(t_c), L.ptr(d_c), L.ptr(far_c), n, N, white, mode,
                                                          *[L.ptr(g) for g in gs], L.ptr(d_rgb), L.ptr(d_sig), _stream()))
-        return d_rgb, d_sig.reshape(n, N, 1), None, None, None, None, None
+        g_d = None
+        if mode == 2 and ctx.needs_input_grad[3]:
+            # alpha_i depends on sigma_i and |rays_d| only through sigma_i delta_i |rays_d|: dL/d|d| = sum_i g_sigma_i sigma_i / |d|
+            g_d = (d_sig * sig_c).sum(-1, keepdim=True) / (d_c * d_c).sum(-1, keepdim=True) * d_c
+        return d_rgb, d_sig.reshape(n, N, 1), None, g_d, None, None, None
 
 
 def _pos_enc(x: Tensor, min_deg: int, max_deg: int) -> Tensor:
@@ -358,6 +362,13 @@ def _mlp_projected_tc(mlp, cam: Tensor, dir_tile: Tensor, local_p: Tensor, world
 
 
 TRAIN_PRECISIONS = ("fp32", "tc")
+RAY_KEYS = ("rays_o", "rays_d", "viewdirs", "radii")
+
+
+def rays_need_grad(rays: Dict[str, Tensor]) -> bool:
+    """True when a ray tensor of the batch requires grad: vanilla NeRF and Mip-NeRF 360 then take their autograd path even with frozen parameters or in eval
+    mode, so the rays (and, through ops.sample_rays, the camera poses) get gradients."""
+    return any(k in rays and torch.is_tensor(rays[k]) and rays[k].requires_grad for k in RAY_KEYS)
 
 
 def check_train_precision(p: str) -> str:
@@ -434,7 +445,16 @@ class _MLPTrainTC(torch.autograd.Function):
                 L.check(lib.neo_tc_gemm_bf16(hl.data_ptr(), W, wbp.data_ptr(), W, L.ptr(bb), beta.data_ptr(), nb, M, nb, W, 1, s))
                 L.check(lib.neo_tc_gemm_bf16(beta.data_ptr(), nb, wvp.data_ptr(), nb, None, yb.data_ptr(), nv, M, nv, nb, 2, s))
                 out, saved = (sig, yb), [beta, wbt, wvt]
+            # the input rows' gradient (pose refinement) reads W0^T and the skip layer's feature columns transposed, zero padded to Kf
+            wft = []
+            if feats.requires_grad:
+                for i, c0 in ((0, 0),) + (((5, W),) if skip else ()):
+                    w = ws[i][0]
+                    wt = torch.zeros(Kf, W, dtype=torch.bfloat16, device=dev)
+                    L.check(lib.neo_tc_pack_bf16(w.data_ptr() + 4 * c0, W, F, w.shape[1], wt.data_ptr(), F, W, 1, s))
+                    wft.append((i, wt))
         ctx.save_for_backward(XS, *H, *WT, wsig, *saved)
+        ctx.wft = wft
         ctx.meta = (depth, M, F, W, Kf, fo, X, [w.shape[1] for w, _ in ws], rgb)
         return out if rgb else sig
 
@@ -460,6 +480,8 @@ class _MLPTrainTC(torch.autograd.Function):
                                                                                      L.ptr(ws), need, s))
         G = [_bf16(M, W, dev=dev), _bf16(M, W, dev=dev)]
         grads = [None] * (2 * depth + 2)
+        wft = dict(ctx.wft)
+        g_in = {i: torch.empty(M, Kf, device=dev) for i in wft}
         extra = []
         with torch.cuda.device(dev):
             if rgb:
@@ -485,10 +507,15 @@ class _MLPTrainTC(torch.autograd.Function):
                 gw, gb = torch.empty(W, kvalid[i], device=dev), torch.empty(W, device=dev)
                 wg(G[0].data_ptr(), W, xp, ldx, W, kin, gw, kvalid[i], gb)
                 grads[2 * i], grads[2 * i + 1] = gw, gb
+                if i in wft:        # dL/dz_i . W_i[:, feature columns] in fp32 (fp32 epilogue of the bf16 GEMM)
+                    L.check(lib.neo_tc_gemm_bf16(G[0].data_ptr(), W, wft[i].data_ptr(), W, None, g_in[i].data_ptr(), Kf, M, Kf, W, 2, s))
                 if i > 0:
                     L.check(lib.neo_tc_dgrad_bf16(G[0].data_ptr(), W, WT[i - 1].data_ptr(), W, xp, ldx, None, None, G[1].data_ptr(), W, M, W, W, s))
                     G.reverse()
-        return (None, None, *grads, *extra)
+        g_feats = None
+        if g_in:
+            g_feats = (g_in[0] + g_in[5] if 5 in g_in else g_in[0])[:, :F]
+        return (None, g_feats, *grads, *extra)
 
 
 def mlp_train_tc(m, feats: Tensor, denc: Tensor, n: int, N: int):

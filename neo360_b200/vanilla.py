@@ -9,7 +9,13 @@ Training: with autograd on, the module in train mode and parameters that require
 differentiable w.r.t. every MLP parameter (LitNeRF.training_step, model.py:273-299).  Sampling, encodings and compositing forward and
 backward are hand-written CUDA; the dense layers are framework fp32 GEMMs under autograd, or with `train_precision="tc"` bf16 tensor-core
 GEMMs forward and backward (training._MLPTrainTC, csrc/dense_train.cu).  `precision` applies to inference only.  After an optimiser step the next inference call re-packs the weights (`_ensure` keys on each
-parameter's storage and version)."""
+parameter's storage and version).
+
+Ray and pose gradients: when grad is enabled and `rays_o`, `rays_d` or `viewdirs` requires grad, `forward` takes the same autograd path,
+also with the MLPs frozen or the module in eval mode, and the outputs are differentiable w.r.t. those rays as the reference's plain-PyTorch
+module is: the points o + t viewdirs and the direction encoding through `neo_vanilla_encode_bwd`, |rays_d| through the compositing (the
+sample positions t carry no gradient, as in the reference).  With `ops.sample_rays` / `ops.get_rays` on a `c2w` that requires grad and
+`cameras.PoseCorrection`, this refines camera poses by photometric gradient.  With no ray requiring grad, nothing of this runs."""
 from __future__ import annotations
 
 import ctypes as C
@@ -20,7 +26,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib as L
-from .training import _Composite, check_train_precision, mlp_train_tc
+from .training import _Composite, check_train_precision, mlp_train_tc, rays_need_grad
 
 
 class NeRFMLP(nn.Module):
@@ -79,6 +85,36 @@ def _mlp_train(m: NeRFMLP, enc: torch.Tensor, denc: torch.Tensor, n: int, N: int
     return raw_rgb, raw_sigma.reshape(n, N, 1)
 
 
+class _VanillaEncode(torch.autograd.Function):
+    """neo_vanilla_encode under autograd: rays_o, viewdirs (n,3), t (n,N) -> enc (n*N, 63), dir_enc (n, 27).  The backward
+    (neo_vanilla_encode_bwd) gives rays_o and viewdirs their gradients; t carries none (the reference's sample positions are detached)."""
+
+    @staticmethod
+    def forward(ctx, o, vd, t):
+        lib = L.load()
+        o_c, vd_c, t_c = (x.detach().contiguous().float() for x in (o, vd, t))
+        n, N = t_c.shape
+        enc, denc = torch.empty(n * N, 63, device=o_c.device), torch.empty(n, 27, device=o_c.device)
+        with torch.cuda.device(o_c.device):
+            L.check(lib.neo_vanilla_encode(L.ptr(o_c), L.ptr(vd_c), L.ptr(t_c), n, N, L.ptr(enc), L.ptr(denc), torch.cuda.current_stream().cuda_stream))
+        ctx.save_for_backward(o_c, vd_c, t_c)
+        return enc, denc
+
+    @staticmethod
+    def backward(ctx, g_enc, g_denc):
+        lib = L.load()
+        o_c, vd_c, t_c = ctx.saved_tensors
+        n, N = t_c.shape
+        dev = o_c.device
+        g_enc = torch.zeros(n * N, 63, device=dev) if g_enc is None else g_enc.contiguous().float()
+        g_denc = torch.zeros(n, 27, device=dev) if g_denc is None else g_denc.contiguous().float()
+        g_o, g_vd = torch.empty(n, 3, device=dev), torch.empty(n, 3, device=dev)
+        with torch.cuda.device(dev):
+            L.check(lib.neo_vanilla_encode_bwd(L.ptr(o_c), L.ptr(vd_c), L.ptr(t_c), n, N, L.ptr(g_enc), L.ptr(g_denc), L.ptr(g_o), L.ptr(g_vd),
+                                               torch.cuda.current_stream().cuda_stream))
+        return g_o, g_vd, None
+
+
 class NeRF(nn.Module):
     def __init__(self, num_levels: int = 2, min_deg_point: int = 0, max_deg_point: int = 10, deg_view: int = 4, num_coarse_samples: int = 64,
                  num_fine_samples: int = 128, use_viewdirs: bool = True, noise_std: float = 0.0, lindisp: bool = False,
@@ -119,7 +155,7 @@ class NeRF(nn.Module):
             pass
 
     def forward(self, rays: Dict[str, torch.Tensor], randomized: bool, white_bkgd: bool, near, far, debug: bool = False) -> List[tuple]:
-        if torch.is_grad_enabled() and self.training and any(p.requires_grad for p in self.parameters()):
+        if torch.is_grad_enabled() and ((self.training and any(p.requires_grad for p in self.parameters())) or rays_need_grad(rays)):
             return self._forward_train(rays, randomized, white_bkgd, near, far, debug)
         o = rays["rays_o"].contiguous().float()
         d = rays["rays_d"].contiguous().float()
@@ -219,21 +255,25 @@ class NeRF(nn.Module):
             u = [x.contiguous().float() for x in u]
         stream = torch.cuda.current_stream(dev).cuda_stream
         tc = check_train_precision(self.train_precision) == "tc"
+        ray_grad = o.requires_grad or vd.requires_grad
         ret, t, w = [], None, None
         dbg = {"t": [], "weights": []}
         for lvl, mlp in enumerate((self.coarse_mlp, self.fine_mlp)):
             with torch.cuda.device(dev):
                 if lvl == 0:
                     t = torch.empty(n, nc + 1, device=dev)
-                    L.check(lib.neo_vanilla_sample_along_rays(L.ptr(o), L.ptr(vd), n, nc, float(near), float(far), L.ptr(u[0]), L.ptr(t), stream))
+                    L.check(lib.neo_vanilla_sample_along_rays(L.ptr(o.detach()), L.ptr(vd.detach()), n, nc, float(near), float(far), L.ptr(u[0]), L.ptr(t), stream))
                 else:       # bins = mids(t), weights[1:-1] of the DETACHED level-0 weights (helper.py:613)
                     t1 = torch.empty(n, t.shape[1] + nf, device=dev)
-                    L.check(lib.neo_sample_pdf(L.ptr(o), L.ptr(vd), None, L.ptr(t), L.ptr(w.detach().contiguous()), n, t.shape[1], nf, 1, 0.0,
+                    L.check(lib.neo_sample_pdf(L.ptr(o.detach()), L.ptr(vd.detach()), None, L.ptr(t), L.ptr(w.detach().contiguous()), n, t.shape[1], nf, 1, 0.0,
                                                L.ptr(u[1]), L.ptr(t1), None, None, stream))
                     t = t1
                 N = t.shape[1]
-                enc, denc = torch.empty(n * N, 63, device=dev), torch.empty(n, 27, device=dev)
-                L.check(lib.neo_vanilla_encode(L.ptr(o), L.ptr(vd), L.ptr(t), n, N, L.ptr(enc), L.ptr(denc), stream))
+                if ray_grad:
+                    enc, denc = _VanillaEncode.apply(o, vd, t)
+                else:
+                    enc, denc = torch.empty(n * N, 63, device=dev), torch.empty(n, 27, device=dev)
+                    L.check(lib.neo_vanilla_encode(L.ptr(o), L.ptr(vd), L.ptr(t), n, N, L.ptr(enc), L.ptr(denc), stream))
             if tc:
                 raw_sigma, raw_rgb = mlp_train_tc(mlp, enc, denc, n, N)
                 raw_sigma = raw_sigma.reshape(n, N, 1)
