@@ -116,8 +116,9 @@ struct Params {
 };
 
 // Phase clocks (diagnostic build only, -DNEO_FIELD_PHASES; read by tools/field_phases.py): the first thread of every consumer
-// warpgroup and of every producer half adds the clock64() cycles between consecutive marks to its phase, and at the end of the
-// kernel the sums (and the consumers' tile counts) go into the launch's row of g_phase_cycles.  The marks bound the phases as the
+// warpgroup and of every producer half adds the clock() cycles between consecutive marks to its phase (32-bit: one register less
+// than clock64() in the background consumers, and a phase lasts far less than 2^32 cycles), and at the end of the kernel the sums
+// (and the consumers' tile counts) go into the launch's row of g_phase_cycles.  The marks bound the phases as the
 // compiler scheduled them, which is close to, but not exactly, the source order.  Without the macro the kernel has no marks at all.
 #ifdef NEO_FIELD_PHASES
 enum Phase {
@@ -125,20 +126,22 @@ enum Phase {
     kPhSetup, kPhEnc, kPhTaps, kPhSlot,                                                      // producer
     kPhases
 };
-constexpr int kPhaseCols = kPhases + 2;                                  // the phases, then tiles, then taps of non-zero weight
+// the phases, then tiles, taps of non-zero weight, and those of them that row n shares with row n + 8 (TapTable::share)
+constexpr int kPhaseCols = kPhases + 3;
 constexpr int kPhaseUnits = 2 * kConsumers;                              // the consumers, then the producer halves
 constexpr uint32_t kPhaseBytes = kPhaseUnits * (kPhases + 1) * 8;        // per-unit sums (phases, tiles) in shared memory
 constexpr int kPhaseSlots = 64;
 __device__ unsigned long long g_phase_cycles[kPhaseSlots][kPhaseCols];    // [launch][column]
 static int g_phase_launches = 0;
 #define FIELD_PHASE_INIT(unit, lead) \
-    long long ph_t = clock64();      \
+    unsigned ph_t = clock();         \
     unsigned long long ph_taps = 0;  \
+    unsigned long long ph_shared = 0; \
     const int ph_unit = (unit);      \
     const bool ph_lead = (lead)
 #define FIELD_PHASE(p)                                        \
     do {                                                      \
-        const long long now_ = clock64();                     \
+        const unsigned now_ = clock();                        \
         if (ph_lead) ph_acc[ph_unit][p] += now_ - ph_t;       \
         ph_t = now_;                                          \
     } while (0)
@@ -456,18 +459,25 @@ __device__ __forceinline__ uint64_t wdesc(uint32_t base, int ks, uint32_t slab) 
 
 // Tap table of one (tile, view), per consumer in shared memory: for every point n of the tile and map m (latent, xz, xy, yz), the
 // texel indices (view included) of the four taps {nw, ne, sw, se} and their bilinear weights.  Split in two arrays of 16-byte
-// entries [m][n], so that the 8 points a warp reads at once fall on distinct banks.
+// entries [m][n], so that the 8 points a warp reads at once fall on distinct banks.  A consumer thread blends rows r0 and r0 + 8
+// (r0 % 16 < 8): the same sample of two vertically adjacent pixels, which mostly read the same texels.  Foreground only:
+// share[share_pair(r0)] has bit 4 m + k set when tap k of map m is the same texel for both rows and both weights are non-zero, so
+// the blend fetches it once.
 struct TapTable {
     int4 tex[4][kTilePts];
     float4 w[4][kTilePts];
+    uint16_t share[kTilePts / 2];
 };
+__host__ __device__ constexpr int share_pair(int r0) { return (r0 >> 4) * 8 + (r0 & 7); }
 __device__ __forceinline__ int comp4(const int4& x, int k) { return k == 0 ? x.x : k == 1 ? x.y : k == 2 ? x.z : x.w; }
 __device__ __forceinline__ float comp4(const float4& x, int k) { return k == 0 ? x.x : k == 1 ? x.y : k == 2 ? x.z : x.w; }
 
 // entry (point n, map m) of the tap table from the camera-frame lookup point cl: grid_sample(bilinear, align_corners=True, zeros)
 // taps of the map in source view v.  A tap out of range has weight 0, which the blend skips, and index 0, so that every index in the
-// table is a texel of the map.
-__device__ __forceinline__ void tap_entry(TapTable& tab, const SceneDev& sc, const float (&cl)[3], int v, int n, int m) {
+// table is a texel of the map.  With SHARE, returns in the threads with n % 16 < 8 bit k set when tap k is a texel of non-zero weight that is
+// also tap k of point n + 8 with non-zero weight (lane n + 8 of the same warp; every lane of the warp must call this together).
+template <bool SHARE>
+__device__ __forceinline__ uint32_t tap_entry(TapTable& tab, const SceneDev& sc, const float (&cl)[3], int v, int n, int m) {
     float gx, gy;
     int mw, mh;
     if (m == 0) {
@@ -485,41 +495,73 @@ __device__ __forceinline__ void tap_entry(TapTable& tab, const SceneDev& sc, con
     for (int k = 0; k < 4; ++k) tx[k] = tq.w[k] == 0.f ? 0 : (v * mh + tq.y0 + (k >> 1)) * mw + tq.x0 + (k & 1);
     tab.tex[m][n] = make_int4(tx[0], tx[1], tx[2], tx[3]);
     tab.w[m][n] = make_float4(tq.w[0], tq.w[1], tq.w[2], tq.w[3]);
+    if (!SHARE) return 0;
+    uint32_t shared = 0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const int key = tq.w[k] == 0.f ? -1 : tx[k];              // a zero-weight tap (index 0) matches nothing
+        const int other = __shfl_down_sync(0xffffffffu, key, 8);
+        shared |= (uint32_t)(key >= 0 && key == other) << k;
+    }
+    return shared;
+}
+
+// acc[4 j + 2 I + e] += w * (channel 8 j + 2 t + e of the texel chunks q): one tap of the point in row r0 + 8 I
+template <int I>
+__device__ __forceinline__ void blend_tap(float (&acc)[64], float w, const uint4 (&q)[4]) {
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+        const uint32_t wd[4] = {q[u].x, q[u].y, q[u].z, q[u].w};
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&wd[jj]));
+            const int j = 4 * u + jj;
+            acc[4 * j + 2 * I] = fmaf(w, f.x, acc[4 * j + 2 * I]);
+            acc[4 * j + 2 * I + 1] = fmaf(w, f.y, acc[4 * j + 2 * I + 1]);
+        }
+    }
 }
 
 // acc[4 j + 2 i + e] += bilinear blend (grid_sample, align_corners=True, zeros) of channel 8 j + 2 t + e of half HALF of [P0 | P3]
 // over the four maps, at this thread's two points (rows r0, r0 + 8 of the tile); fp32 blend of fp16 texels.
-// The taps' geometry comes from the tap table; the taps are still fetched one at a time: each tap's four 16-byte loads sit behind
-// its zero-weight skip, and the FMAs that use them follow.  (Issuing a map's four taps ahead of their FMAs needs the skip replaced
-// by masking, 64 more live registers and the FMAs of out-of-range taps; measured on H100 that made the field launches 10 % slower
-// than this form, see DESIGN.md §5.)
-template <int HALF>
+// The taps' geometry comes from the tap table.  For each map and tap k the thread blends tap k of row r0, then tap k of row r0 + 8;
+// a tap of zero weight is skipped (zeros padding: no contribution).  Each accumulator belongs to one row and gets its taps in
+// (m, k) order with the same fmaf operands whatever the path, so the sums are bit for bit those of blending each row on its own.
+// All lanes step through (m, k) together, so lanes of a quarter-warp that read the same line in one load still share it.
+// PAIR (foreground): both rows' loads of tap k are issued before either row's FMAs, two texels in flight instead of one (the
+// blends wait on each texel's first fetch, DESIGN.md §5); and a tap the table marks as the same texel for both rows
+// (TapTable::share) is loaded once, row r0 + 8 blending row r0's chunks.  The background kernel has no registers for the second
+// set of chunks (it spills), so it loads and blends one row's tap at a time, without the mask.  (Issuing a map's four taps ahead of
+// their FMAs needs the skip replaced by masking, 64 more live registers and the FMAs of out-of-range taps; measured on H100 that
+// made the field launches 10 % slower than one tap at a time, see DESIGN.md §5.)
+template <int HALF, bool PAIR>
 __device__ __forceinline__ void blend_maps(float (&acc)[64], const Params& P, const TapTable& tab, int r0, int t) {
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
+    uint32_t share = PAIR ? tab.share[share_pair(r0)] : 0u;
 #pragma unroll 1
-        for (int m = 0; m < 4; ++m) {
-            const int4 tx = tab.tex[m][r0 + 8 * i];
-            const float4 wv = tab.w[m][r0 + 8 * i];
-            const uint4* base = reinterpret_cast<const uint4*>(P.mlp.pmap[m] + HALF * 128 + t * 8);
+    for (int m = 0; m < 4; ++m, share >>= 4) {
+        const float4 wv0 = tab.w[m][r0], wv1 = tab.w[m][r0 + 8];
+        const int* tx0 = reinterpret_cast<const int*>(&tab.tex[m][r0]);    // read per tap, behind its skip: fewer live registers
+        const int* tx1 = reinterpret_cast<const int*>(&tab.tex[m][r0 + 8]);
+        const uint4* base = reinterpret_cast<const uint4*>(P.mlp.pmap[m] + HALF * 128 + t * 8);
 #pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const float w = comp4(wv, k);
-                if (w == 0.f) continue;                                // out-of-range tap (zeros padding): no contribution
-                uint4 q[4];
+        for (int k = 0; k < 4; ++k) {
+            const float w0 = comp4(wv0, k), w1 = comp4(wv1, k);
+            const bool both = (share >> k) & 1u;                       // shared: w0, w1 != 0 and q0 holds row r0 + 8's texel
+            uint4 q0[4], q1[4];
+            if (w0 != 0.f) {
 #pragma unroll
-                for (int u = 0; u < 4; ++u) q[u] = __ldg(base + (size_t)comp4(tx, k) * 32 + 4 * u);   // 32 uint4 per texel
+                for (int u = 0; u < 4; ++u) q0[u] = __ldg(base + (size_t)tx0[k] * 32 + 4 * u);   // 32 uint4 per texel
+                if (!PAIR) blend_tap<0>(acc, w0, q0);
+            }
+            if (w1 != 0.f && !both)
 #pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const uint32_t wd[4] = {q[u].x, q[u].y, q[u].z, q[u].w};
+                for (int u = 0; u < 4; ++u) q1[u] = __ldg(base + (size_t)tx1[k] * 32 + 4 * u);
+            if (PAIR && w0 != 0.f) blend_tap<0>(acc, w0, q0);
+            if (w1 != 0.f) {
+                if (both)
 #pragma unroll
-                    for (int jj = 0; jj < 4; ++jj) {
-                        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&wd[jj]));
-                        const int j = 4 * u + jj;
-                        acc[4 * j + 2 * i] = fmaf(w, f.x, acc[4 * j + 2 * i]);
-                        acc[4 * j + 2 * i + 1] = fmaf(w, f.y, acc[4 * j + 2 * i + 1]);
-                    }
-                }
+                    for (int u = 0; u < 4; ++u) q1[u] = q0[u];
+                blend_tap<1>(acc, w1, q1);
             }
         }
     }
@@ -638,11 +680,18 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
                 if constexpr (IS_BG) to_camera(vxs[v], pts[n].xl, cl);
                 bar_wait(P.trap, bar, cb + kTapsEmpty, (k_taps & 1) ^ 1);    // the consumer's blends have read the previous table
                 FIELD_PHASE(kPhSlot);
+                uint32_t shared = 0;
 #pragma unroll 1
                 for (int m = 0; m < 4; ++m) {
-                    tap_entry(*tab, P.sc, cl, v, n, m);
+                    shared |= tap_entry<!IS_BG>(*tab, P.sc, cl, v, n, m) << (4 * m);
 #ifdef NEO_FIELD_PHASES
                     for (int k = 0; k < 4; ++k) ph_taps += comp4(tab->w[m][n], k) != 0.f;
+#endif
+                }
+                if (!IS_BG && (n & 15) < 8) {
+                    tab->share[share_pair(n)] = (uint16_t)shared;
+#ifdef NEO_FIELD_PHASES
+                    ph_shared += __popc(shared);
 #endif
                 }
                 mbar_arrive(bar + 8u * (cb + kTapsFull));
@@ -654,6 +703,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
         if (ph_lead)
             for (int p = kPhSetup; p < kPhases; ++p) atomicAdd(&g_phase_cycles[P.phase_slot][p], ph_acc[ph_unit][p]);
         atomicAdd(&g_phase_cycles[P.phase_slot][kPhases + 1], ph_taps);
+        atomicAdd(&g_phase_cycles[P.phase_slot][kPhases + 2], ph_shared);
 #endif
         return;
     }
@@ -731,7 +781,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
             // layer 0: blend of P0 + W0enc . enc (b0 on the constant-one column)
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-            blend_maps<0>(acc, P, *tab, r0, t);
+            blend_maps<0, !IS_BG>(acc, P, *tab, r0, t);
             FIELD_PHASE(kPhBlend0);
             wgmma_fence();
 #pragma unroll
@@ -754,7 +804,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;
             FIELD_PHASE(kPhLayers);
-            blend_maps<1>(acc, P, *tab, r0, t);
+            blend_maps<1, !IS_BG>(acc, P, *tab, r0, t);
             mbar_arrive(bar + 8u * (cb + kTapsEmpty));                              // the producer may build the next table
             ++k_taps;
             FIELD_PHASE(kPhBlend3);
@@ -1041,8 +1091,8 @@ extern "C" const char* neo_tc_trap_info(void) { return neo::tc_trap_info(); }
 
 #ifdef NEO_FIELD_PHASES
 // diagnostic build only (not part of include/neo360_b200.h): zero the phase clocks, and read them back after a synchronise as
-// [launch][kPhases + 2] (cycles per phase, then tiles, then taps of non-zero weight), one row per field launch since the reset;
-// returns the number of launches
+// [launch][kPhases + 3] (cycles per phase, then tiles, taps of non-zero weight and shared taps), one row per field launch since the
+// reset; returns the number of launches
 extern "C" int neo_field_phases_reset(void) {
     neo::tc::g_phase_launches = 0;
     void* p = nullptr;

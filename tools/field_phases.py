@@ -6,7 +6,9 @@ once to warm up and once measured, and prints for each field launch the cycles p
 consumer warpgroups' phases (blends and MMAs, and their waits for geometry) summed over the two consumers, and the producer's
 phases (points, encodings, tap tables, and its waits for a free slot) summed over its two halves.  Whichever side waits less bounds
 the tile.  It also prints the texel traffic the blends request: taps of non-zero weight per tile (each one 2 x 256 bytes, the P0
-and P3 halves of a texel) over the cycles of the two blend phases.  Usage on a GPU box:
+and P3 halves of a texel) over the cycles of the two blend phases, and how many of those taps a thread's two points share (the same
+texel as the same tap of the other point, both weights non-zero: TapTable::share), which the blends fetch once for both points.
+Usage on a GPU box:
 
   python tools/field_phases.py [--lib PATH] [--clock-mhz F]
       --lib: an instrumented library built beforehand, e.g. from another source tree
@@ -78,7 +80,7 @@ def main():
         net.render_rays_test(rays, chunk=Bm.CHUNK, img_wh=wh)
         torch.cuda.synchronize()
     net.check()
-    cols = len(PHASES) + 2                                               # phases, tiles, non-zero-weight taps
+    cols = len(PHASES) + 3                                               # phases, tiles, non-zero-weight taps, shared taps
     buf = (C.c_ulonglong * (MAX_LAUNCHES * cols))()
     n = lib.neo_field_phases_read(buf, MAX_LAUNCHES)
     if n < 0:
@@ -92,22 +94,24 @@ def main():
         print(f"{'launch':<12}{'tiles':>9}" + "".join(f"{p:>24}" for p in names) + f"{'total':>12}")
         for li in range(n):
             row = buf[li * cols:(li + 1) * cols]
-            tiles = max(row[-2], 1)
+            tiles = max(row[-3], 1)
             per = [c / tiles for c in row[lo:lo + len(names)]]
             if lo == 0:
-                rows.append((tiles, [c / tiles for c in row[:-2]], row[-1] / tiles))
-            print(f"{LAUNCHES[li % 4]:<12}{row[-2]:>9}" + "".join(f"{x:>16.0f} ({x / max(sum(per), 1):4.0%})" for x in per)
+                rows.append((tiles, [c / tiles for c in row[:-3]], row[-2] / tiles, row[-1] / tiles))
+            print(f"{LAUNCHES[li % 4]:<12}{row[-3]:>9}" + "".join(f"{x:>16.0f} ({x / max(sum(per), 1):4.0%})" for x in per)
                   + f"{sum(per):>12.0f}")
     # request rate of the blends: a warpgroup's texel bytes per tile over its blend cycles per tile; the GPU figure assumes both
     # warpgroups of every SM blend at once (an upper bound), the launch figure spreads the bytes over the whole tile
     print(f"texel requests ({n_sm} SMs, 2 consumer warpgroups each, SM clock {args.clock_mhz:.0f} MHz):")
-    print(f"{'launch':<12}{'taps/tile':>10}{'KB/tile':>9}{'B/cycle in blends':>19}{'GPU TB/s in blends':>20}{'GPU TB/s over tile':>20}")
-    for li, (tiles, per, taps) in enumerate(rows):
-        by = taps * 512
+    # a shared tap is fetched once for the thread's two points: the fetches saved are shared / taps, and the bytes below are fetched
+    print(f"{'launch':<12}{'taps/tile':>10}{'shared/tile':>12}{'fetches saved':>14}{'KB/tile':>9}{'B/cycle in blends':>19}"
+          f"{'GPU TB/s in blends':>20}{'GPU TB/s over tile':>20}")
+    for li, (tiles, per, taps, shared) in enumerate(rows):
+        by = (taps - shared) * 512
         blend = per[PHASES.index("blend P0")] + per[PHASES.index("blend P3")]
         scale = 2 * n_sm * args.clock_mhz * 1e6 / 1e12
         tile = sum(per[:len(CONSUMER)])
-        print(f"{LAUNCHES[li % 4]:<12}{taps:>10.0f}{by / 1024:>9.0f}{by / blend:>19.1f}{by / blend * scale:>20.2f}{by / tile * scale:>20.2f}")
+        print(f"{LAUNCHES[li % 4]:<12}{taps:>10.0f}{shared:>12.0f}{shared / max(taps, 1):>14.1%}{by / 1024:>9.0f}{by / blend:>19.1f}{by / blend * scale:>20.2f}{by / tile * scale:>20.2f}")
 
 
 if __name__ == "__main__":
