@@ -12,7 +12,9 @@
 //
 // Layout: one persistent CTA per SM, three warpgroups.  Two consumer warpgroups each work on their own tiles of 64 points (32 rays x 2
 // consecutive samples); the producer warpgroup builds their geometry (points, camera-frame encodings, tap tables: 64 threads per
-// consumer, one point each) and hands it over through full / empty mbarrier pairs, so the consumers only blend and multiply.
+// consumer, one point each) and hands it over through full / empty mbarrier pairs, so the consumers only blend and multiply.  A tile's
+// rows (and, in the background, its view-independent s encoding columns) go over once per tile, then the encodings and tap table of
+// one view at a time: the producer builds the next tile's rows and first view while the consumer is still on its current tile.
 // setmaxnreg moves registers from the producer (56) to the consumers (224).
 // The rays of a tile are 32 consecutive slots of the ray order (one 8x4 pixel block of a frame, renderer._blocked_order): rays that
 // close together read the same texels at a sample, while consecutive samples move on to the next texel, so a tile that spans more
@@ -345,38 +347,42 @@ __device__ __forceinline__ void bar_wait(int* trapinfo, uint32_t bar0, int id, u
 
 __device__ __forceinline__ float sel4(const float* x, int i) { return i == 0 ? x[0] : i == 1 ? x[1] : i == 2 ? x[2] : x[3]; }
 
-// Encoding staging: per (tile, view) the producer computes a consumer's 64 points' encodings once, as a flat set of items, into one
-// row of 64 fp16 per point; then every thread of the consumer loads its A-fragment columns from the rows.  Row slot 21 j + k holds column k of staged coordinate j: k = 0 the coordinate, 1 + l sin(2^l x), 11 + l cos(2^l x), the
-// order of enc_col<3> (slot == column for the foreground).  The 32-bit words of a row are XOR-swizzled by the point (bits 2-4), so
+// Encoding staging: per (tile, view) the producer computes a consumer's 64 points' camera-frame encodings once, as a flat set of
+// items, into one row of 64 fp16 per point; then every thread of the consumer loads its A-fragment columns from the rows.  (The
+// background's s columns do not depend on the view and go with the tile's rows instead: kSRow.)  Row slot 21 j + k holds column k
+// of coordinate j: k = 0 the coordinate, 1 + l sin(2^l x), 11 + l cos(2^l x), the order of enc_col<3> (slot == column for the
+// foreground).  The 32-bit words of a row are XOR-swizzled by the point (bits 2-4), so
 // that the 8 points x 4 words a warp loads per fragment register fall on 32 distinct banks.
 constexpr int kStageRow = 64;
 __device__ __forceinline__ int stage_slot(int n, int k) { return n * kStageRow + ((((k >> 1) ^ ((n & 7) << 2))) << 1 | (k & 1)); }
 
 // items first .. first + count - 1 of one point (item i: staged coordinate i / 10, level i % 10): sin and cos of 2^l x, rounded to
-// fp16 as pack_h2 does.  Rolled, so the kernel has one sincosf call site per use instead of one sinf / cosf per fragment column.
-__device__ __forceinline__ void stage_items(__half* stage, int n, const float (&x)[3], int first, int count) {
+// fp16 as pack_h2 does, into rows[slot(k)] for row slot k.  Rolled, so the kernel has one sincosf call site per use instead of one
+// sinf / cosf per fragment column.
+template <typename Slot>
+__device__ __forceinline__ void stage_items(__half* rows, Slot slot, const float (&x)[3], int first, int count) {
 #pragma unroll 1
     for (int i = first; i < first + count; ++i) {
         const int j = i / 10, l = i - 10 * j;
         const float xc = j == 0 ? x[0] : j == 1 ? x[1] : x[2];
         float s, c;
         sincosf(xc * (float)(1 << l), &s, &c);           // exact: power-of-two scaling
-        stage[stage_slot(n, 21 * j + 1 + l)] = __float2half_rn(s);
-        stage[stage_slot(n, 21 * j + 11 + l)] = __float2half_rn(c);
+        rows[slot(21 * j + 1 + l)] = __float2half_rn(s);
+        rows[slot(21 * j + 11 + l)] = __float2half_rn(c);
     }
 }
 
-// fp16 bits of encoding column c = c0 + u (enc_col<ICH> order; c0 a multiple of 8, u < 8) of point n, from rows that stage
-// coordinates j0, j0 + 1, ...  Beyond a coordinate's 21 columns: the constant one (column 21 of the background) or zero.
+// fp16 bits of encoding column c = c0 + u (enc_col<ICH> order; c0 a multiple of 8, u < 8, c < 72 in the background) of point n,
+// from the staging rows.  Beyond a coordinate's 21 columns: the constant one (column 21 of the background) or zero.
 template <int ICH>
-__device__ __forceinline__ uint32_t enc_staged(const __half* stage, int n, int c0, int u, int j0) {
+__device__ __forceinline__ uint32_t enc_staged(const __half* stage, int n, int c0, int u) {
     if (ICH == 3) {                                      // stride 21: the slot is the column
         const int c = c0 + u;
         return c == 63 ? 0x3c00u : __half_as_ushort(stage[stage_slot(n, c)]);
     }
     const int j = c0 / 24, k = c0 % 24 + u;              // c0 % 24 <= 16: the 8 columns from c0 share one coordinate block
     if (k >= 21) return (j == 0 && k == 21) ? 0x3c00u : 0u;
-    return __half_as_ushort(stage[stage_slot(n, 21 * (j - j0) + k)]);
+    return __half_as_ushort(stage[stage_slot(n, 21 * j + k)]);
 }
 // the slot arithmetic above, checked against enc_col<> for every column
 template <int ICH>
@@ -397,6 +403,35 @@ constexpr bool stage_layout_ok() {
     return true;
 }
 static_assert(stage_layout_ok<3>() && stage_layout_ok<4>(), "enc_staged does not match enc_col");
+
+// The background's s columns 72-95 (coordinate 3 of enc_col<4>: the inverse radius tv, its sin / cos levels and three zero columns)
+// do not depend on the view.  The producer writes them once per tile, with the tile's PtsRows and before the same rows-full arrive,
+// into one row of kSRow fp16 per point, slot k = column 72 + k; the consumer loads its A-fragment words of them when it copies the
+// rows.  So the staging rows hold one view's encodings and nothing else, and the producer can build the next tile's first view while
+// the consumer still works on the current tile.  A fragment word (columns 72 + 8 h' + 2 t, + 1) is one 32-bit load at slot
+// 8 h' + 2 t: the 8 rows x 4 threads t of a warp's load fall on 32 distinct banks with the plain 48-byte row stride.
+constexpr int kSRow = 24;
+constexpr int kSCol0 = 72;
+__device__ __forceinline__ uint32_t s_word(const __half* srows, int n, int k) {
+    return *reinterpret_cast<const uint32_t*>(srows + n * kSRow + k);
+}
+constexpr bool s_layout_ok() {
+    for (int k = 0; k < kSRow; ++k) {
+        const EncCol e = enc_col<4>(kSCol0 + k);
+        const int slot = e.kind == 2 ? 0 : e.kind == 3 ? 1 + e.lvl : 11 + e.lvl;
+        if (k < 21 && (e.kind < 2 || e.cc != 3 || slot != k)) return false;
+        if (k >= 21 && e.kind != 0) return false;
+    }
+    if (kSCol0 + kSRow != 96 || kSRow % 2) return false;
+    for (int h = 0; h < 3; ++h) {                        // fragment words at slots 8 h + 2 t of rows r .. r + 7
+        unsigned banks = 0;
+        for (int r = 0; r < 8; ++r)
+            for (int t = 0; t < 4; ++t) banks |= 1u << ((r * kSRow + 8 * h + 2 * t) / 2 % 32);
+        if (banks != 0xffffffffu) return false;
+    }
+    return true;
+}
+static_assert(s_layout_ok(), "s rows do not match enc_col<4> or their fragment loads conflict on banks");
 
 // column e of the direction encoding of the conditioning ray in one source camera's frame (model.py:357-360): [d, sin(2^k d),
 // sin(2^k d + pi/2)], 27 columns, zero beyond
@@ -458,24 +493,27 @@ __device__ __forceinline__ void seed_bias(float (&d)[NC / 2], const float* b, in
 __device__ __forceinline__ uint64_t wdesc(uint32_t base, int ks, uint32_t slab) { return desc_sw128(base + (uint32_t)(ks >> 2) * slab + (uint32_t)(ks & 3) * 32u); }
 
 // Tap table of one (tile, view), per consumer in shared memory: for every point n of the tile and map m (latent, xz, xy, yz), the
-// texel indices (view included) of the four taps {nw, ne, sw, se} and their bilinear weights.  Split in two arrays of 16-byte
-// entries [m][n], so that the 8 points a warp reads at once fall on distinct banks.  A consumer thread blends rows r0 and r0 + 8
-// (r0 % 16 < 8): the same sample of two vertically adjacent pixels, which mostly read the same texels.  Foreground only:
-// share[share_pair(r0)] has bit 4 m + k set when tap k of map m is the same texel for both rows and both weights are non-zero, so
-// the blend fetches it once.
+// texel index (view included) of the quad's nw tap and the bilinear weights of its four taps {nw, ne, sw, se}; tap k is texel
+// base + (k >> 1) mw + (k & 1) (tap_index), mw the map's width.  Arrays [m][n], so that the 8 points a warp reads at once fall on
+// distinct banks.  A consumer thread blends rows r0 and r0 + 8 (r0 % 16 < 8): the same sample of two vertically adjacent pixels,
+// which mostly read the same texels.  Foreground only: share[share_pair(r0)] has bit 4 m + k set when tap k of map m is the same
+// texel for both rows and both weights are non-zero, so the blend fetches it once.
 struct TapTable {
-    int4 tex[4][kTilePts];
+    int base[4][kTilePts];
     float4 w[4][kTilePts];
     uint16_t share[kTilePts / 2];
 };
 __host__ __device__ constexpr int share_pair(int r0) { return (r0 >> 4) * 8 + (r0 & 7); }
-__device__ __forceinline__ int comp4(const int4& x, int k) { return k == 0 ? x.x : k == 1 ? x.y : k == 2 ? x.z : x.w; }
 __device__ __forceinline__ float comp4(const float4& x, int k) { return k == 0 ? x.x : k == 1 ? x.y : k == 2 ? x.z : x.w; }
+// texel index of tap k of the quad whose nw tap is texel `base` of a map mw texels wide
+__device__ __forceinline__ int tap_index(int base, int mw, int k) { return base + (k >> 1) * mw + (k & 1); }
 
 // entry (point n, map m) of the tap table from the camera-frame lookup point cl: grid_sample(bilinear, align_corners=True, zeros)
-// taps of the map in source view v.  A tap out of range has weight 0, which the blend skips, and index 0, so that every index in the
-// table is a texel of the map.  With SHARE, returns in the threads with n % 16 < 8 bit k set when tap k is a texel of non-zero weight that is
-// also tap k of point n + 8 with non-zero weight (lane n + 8 of the same warp; every lane of the warp must call this together).
+// taps of the map in source view v.  A tap out of range has weight 0, and a tap of weight 0 is never loaded (blend_maps), so only
+// the taps of non-zero weight need tap_index to be a texel of the map: at a map's edge (x0 or y0 = -1) the base and the other taps
+// may lie outside it.  A quad whose four weights are all zero (e.g. x0, y0 = -2: off the map) stores base 0.  With SHARE, returns in the
+// threads with n % 16 < 8 bit k set when tap k is a texel of non-zero weight that is also tap k of point n + 8 with non-zero weight
+// (lane n + 8 of the same warp; every lane of the warp must call this together).
 template <bool SHARE>
 __device__ __forceinline__ uint32_t tap_entry(TapTable& tab, const SceneDev& sc, const float (&cl)[3], int v, int n, int m) {
     float gx, gy;
@@ -493,7 +531,8 @@ __device__ __forceinline__ uint32_t tap_entry(TapTable& tab, const SceneDev& sc,
     int tx[4];
 #pragma unroll
     for (int k = 0; k < 4; ++k) tx[k] = tq.w[k] == 0.f ? 0 : (v * mh + tq.y0 + (k >> 1)) * mw + tq.x0 + (k & 1);
-    tab.tex[m][n] = make_int4(tx[0], tx[1], tx[2], tx[3]);
+    const bool any = (tq.w[0] != 0.f) | (tq.w[1] != 0.f) | (tq.w[2] != 0.f) | (tq.w[3] != 0.f);
+    tab.base[m][n] = any ? (v * mh + tq.y0) * mw + tq.x0 : 0;
     tab.w[m][n] = make_float4(tq.w[0], tq.w[1], tq.w[2], tq.w[3]);
     if (!SHARE) return 0;
     uint32_t shared = 0;
@@ -525,23 +564,26 @@ __device__ __forceinline__ void blend_tap(float (&acc)[64], float w, const uint4
 // acc[4 j + 2 i + e] += bilinear blend (grid_sample, align_corners=True, zeros) of channel 8 j + 2 t + e of half HALF of [P0 | P3]
 // over the four maps, at this thread's two points (rows r0, r0 + 8 of the tile); fp32 blend of fp16 texels.
 // The taps' geometry comes from the tap table.  For each map and tap k the thread blends tap k of row r0, then tap k of row r0 + 8;
-// a tap of zero weight is skipped (zeros padding: no contribution).  Each accumulator belongs to one row and gets its taps in
-// (m, k) order with the same fmaf operands whatever the path, so the sums are bit for bit those of blending each row on its own.
-// All lanes step through (m, k) together, so lanes of a quarter-warp that read the same line in one load still share it.
-// PAIR (foreground): both rows' loads of tap k are issued before either row's FMAs, two texels in flight instead of one (the
-// blends wait on each texel's first fetch, DESIGN.md §5); and a tap the table marks as the same texel for both rows
-// (TapTable::share) is loaded once, row r0 + 8 blending row r0's chunks.  The background kernel has no registers for the second
-// set of chunks (it spills), so it loads and blends one row's tap at a time, without the mask.  (Issuing a map's four taps ahead of
-// their FMAs needs the skip replaced by masking, 64 more live registers and the FMAs of out-of-range taps; measured on H100 that
-// made the field launches 10 % slower than one tap at a time, see DESIGN.md §5.)
-template <int HALF, bool PAIR>
+// a tap of zero weight is skipped (zeros padding: no contribution), and its texel index, which may lie outside the map, is never
+// formed into a load.  Each accumulator belongs to one row and gets its taps in (m, k) order with the same fmaf operands whatever
+// the path, so the sums are bit for bit those of blending each row on its own.  All lanes step through (m, k) together, so lanes of
+// a quarter-warp that read the same line in one load still share it.
+// PAIR: both rows' loads of tap k are issued before either row's FMAs, two texels in flight instead of one (the blends wait on each
+// texel's first fetch, DESIGN.md §5).  SHARE (foreground, with PAIR): a tap the table marks as the same texel for both rows
+// (TapTable::share) is loaded once, row r0 + 8 blending row r0's chunks; the background producer builds no mask.  The background
+// kernel has no registers for the second set of chunks in its P3 blend (it spills), so there it loads and blends one row's tap at a
+// time.  (Issuing a map's four taps ahead of their FMAs needs the skip replaced by masking, 64 more live registers and the FMAs of
+// out-of-range taps; measured on H100 that made the field launches 10 % slower than one tap at a time, see DESIGN.md §5.)
+template <int HALF, bool PAIR, bool SHARE>
 __device__ __forceinline__ void blend_maps(float (&acc)[64], const Params& P, const TapTable& tab, int r0, int t) {
-    uint32_t share = PAIR ? tab.share[share_pair(r0)] : 0u;
+    static_assert(PAIR || !SHARE, "a shared tap is blended into both rows from one load: the paired form");
+    uint32_t share = SHARE ? tab.share[share_pair(r0)] : 0u;
 #pragma unroll 1
     for (int m = 0; m < 4; ++m, share >>= 4) {
         const float4 wv0 = tab.w[m][r0], wv1 = tab.w[m][r0 + 8];
-        const int* tx0 = reinterpret_cast<const int*>(&tab.tex[m][r0]);    // read per tap, behind its skip: fewer live registers
-        const int* tx1 = reinterpret_cast<const int*>(&tab.tex[m][r0 + 8]);
+        const int* bx0 = &tab.base[m][r0];                             // read per tap, behind its skip: fewer live registers
+        const int* bx1 = &tab.base[m][r0 + 8];
+        const int mw = m == 0 ? P.sc.lat_w : P.sc.plane_w;
         const uint4* base = reinterpret_cast<const uint4*>(P.mlp.pmap[m] + HALF * 128 + t * 8);
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
@@ -549,13 +591,16 @@ __device__ __forceinline__ void blend_maps(float (&acc)[64], const Params& P, co
             const bool both = (share >> k) & 1u;                       // shared: w0, w1 != 0 and q0 holds row r0 + 8's texel
             uint4 q0[4], q1[4];
             if (w0 != 0.f) {
+                const int tx = tap_index(*bx0, mw, k);
 #pragma unroll
-                for (int u = 0; u < 4; ++u) q0[u] = __ldg(base + (size_t)tx0[k] * 32 + 4 * u);   // 32 uint4 per texel
+                for (int u = 0; u < 4; ++u) q0[u] = __ldg(base + (size_t)tx * 32 + 4 * u);   // 32 uint4 per texel
                 if (!PAIR) blend_tap<0>(acc, w0, q0);
             }
-            if (w1 != 0.f && !both)
+            if (w1 != 0.f && !both) {
+                const int tx = tap_index(*bx1, mw, k);
 #pragma unroll
-                for (int u = 0; u < 4; ++u) q1[u] = __ldg(base + (size_t)tx1[k] * 32 + 4 * u);
+                for (int u = 0; u < 4; ++u) q1[u] = __ldg(base + (size_t)tx * 32 + 4 * u);
+            }
             if (PAIR && w0 != 0.f) blend_tap<0>(acc, w0, q0);
             if (w1 != 0.f) {
                 if (both)
@@ -572,7 +617,8 @@ struct SmemMap {
     static constexpr uint32_t HEAD = trunk_bytes(KE), BIAS = HEAD + WH_BYTES, VIEWS = BIAS + BIAS_BYTES,
                               PTS = VIEWS + kMaxViews * 64, TAPS = PTS + kConsumers * kTilePts * (uint32_t)sizeof(PtsRow),
                               STAGE = TAPS + kConsumers * (uint32_t)sizeof(TapTable),
-                              BAR = STAGE + kConsumers * kTilePts * kStageRow * (uint32_t)sizeof(__half),
+                              SROWS = STAGE + kConsumers * kTilePts * kStageRow * (uint32_t)sizeof(__half),
+                              BAR = SROWS + (KE == 96 ? kConsumers * kTilePts * kSRow * (uint32_t)sizeof(__half) : 0u),
                               PHASES = BAR + (kBars * 8 + 15) / 16 * 16, TOTAL = PHASES + kPhaseBytes;
     static_assert(KE % 64 == 0 || KE % 64 == 32, "an encoding segment ends on a whole or a half slab (w3enc_tail)");
     static_assert(TOTAL + 1024 <= 227u * 1024u, "field kernel shared memory exceeds the 227 KB an sm_90 CTA can have");
@@ -622,6 +668,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
         PtsRow* pts = reinterpret_cast<PtsRow*>(sgen + SM::PTS) + c * kTilePts;
         TapTable* tab = reinterpret_cast<TapTable*>(sgen + SM::TAPS) + c;
         __half* stage = reinterpret_cast<__half*>(sgen + SM::STAGE) + c * kTilePts * kStageRow;
+        __half* srows = reinterpret_cast<__half*>(sgen + SM::SROWS) + c * kTilePts * kSRow;   // background only
         const int cb = 1 + kChans * c;                   // id of this consumer's first channel barrier
         uint32_t k_rows = 0, k_stage = 0, k_taps = 0;   // fills so far: the producer's wait for fill k is on parity (k & 1) ^ 1
         FIELD_PHASE_INIT(kConsumers + c, n == 0);
@@ -649,21 +696,19 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
                 pr.src = c0 + (int)(jl % Bc);
                 pr.pad = 0;
                 pts[n] = pr;
+                if constexpr (IS_BG) {
+                    // the s columns 72-95, once per tile: they travel with the rows
+                    const float sx[3] = {pr.tv, 0.f, 0.f};
+                    __half* srow = srows + n * kSRow;
+                    srow[0] = __float2half_rn(sx[0]);
+                    stage_items(srow, [](int k) { return k; }, sx, 0, 10);
+#pragma unroll
+                    for (int k = 21; k < kSRow; ++k) srow[k] = __float2half_rn(0.f);
+                }
             }
             mbar_arrive(bar + 8u * (cb + kRowsFull));
             ++k_rows;
             FIELD_PHASE(kPhSetup);
-            if constexpr (IS_BG) {
-                // the s columns 72-92 do not depend on the view: staged as coordinate 0 once per tile
-                const float sx[3] = {pts[n].tv, 0.f, 0.f};
-                bar_wait(P.trap, bar, cb + kStageEmpty, (k_stage & 1) ^ 1);
-                FIELD_PHASE(kPhSlot);
-                stage[stage_slot(n, 0)] = __float2half_rn(sx[0]);
-                stage_items(stage, n, sx, 0, 10);
-                mbar_arrive(bar + 8u * (cb + kStageFull));
-                ++k_stage;
-                FIELD_PHASE(kPhEnc);
-            }
 #pragma unroll 1
             for (int v = 0; v < nv; ++v) {
                 float ce[3];
@@ -672,7 +717,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
                 FIELD_PHASE(kPhSlot);
 #pragma unroll
                 for (int j = 0; j < 3; ++j) stage[stage_slot(n, 21 * j)] = __float2half_rn(ce[j]);
-                stage_items(stage, n, ce, 0, 30);
+                stage_items(stage, [n](int k) { return stage_slot(n, k); }, ce, 0, 30);
                 mbar_arrive(bar + 8u * (cb + kStageFull));
                 ++k_stage;
                 FIELD_PHASE(kPhEnc);
@@ -715,6 +760,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
     const PtsRow* pts = reinterpret_cast<const PtsRow*>(sgen + SM::PTS) + wg * kTilePts;
     const TapTable* tab = reinterpret_cast<const TapTable*>(sgen + SM::TAPS) + wg;
     const __half* stage = reinterpret_cast<const __half*>(sgen + SM::STAGE) + wg * kTilePts * kStageRow;
+    const __half* srows = reinterpret_cast<const __half*>(sgen + SM::SROWS) + wg * kTilePts * kSRow;   // background only
     const int cb = 1 + kChans * wg;
     uint32_t k_rows = 0, k_stage = 0, k_taps = 0;       // fills consumed so far: the wait for fill k is on parity k & 1
     const float* sb = reinterpret_cast<const float*>(sgen + SM::BIAS);
@@ -728,35 +774,30 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
         FIELD_PHASE(kPhWait);
         long long gp[2];                                 // output index rid * N + sidx of rows r0, r0 + 8, -1: padding row
         int src[2];
+        // A-fragment columns 16 ks + 8 h + 2 t + e of rows r0, r0 + 8 (e: the low / high half of a word)
+        uint32_t enc[KS][4];
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
             const PtsRow& pr = pts[r0 + 8 * i];
             gp[i] = pr.valid ? (long long)pr.rid * N + pr.sidx : -1;
             src[i] = pr.src;
+            if constexpr (IS_BG) {                       // the s columns 72-95: enc[4][2..3], enc[5][*]
+                enc[KS - 2][2 + i] = s_word(srows, r0 + 8 * i, 2 * t);
+                enc[KS - 1][i] = s_word(srows, r0 + 8 * i, 8 + 2 * t);
+                enc[KS - 1][2 + i] = s_word(srows, r0 + 8 * i, 16 + 2 * t);
+            }
         }
         mbar_arrive(bar + 8u * (cb + kRowsEmpty));
         ++k_rows;
 #ifdef NEO_FIELD_PHASES
         if (wt == 0) ph_acc[wg][kPhases] += 1ull;
 #endif
-        // A-fragment columns 16 ks + 8 h + 2 t + e of rows r0, r0 + 8, as enc_staged reads them (c0 = 16 ks + 8 h, u = 2 t + e)
-        uint32_t enc[KS][4];
-        auto load_enc = [&](int ks, int h, int j0) {
+        auto load_enc = [&](int ks, int h) {             // the columns as enc_staged reads them (c0 = 16 ks + 8 h, u = 2 t + e)
 #pragma unroll
             for (int i = 0; i < 2; ++i)
-                enc[ks][2 * h + i] = enc_staged<ICH>(stage, r0 + 8 * i, 16 * ks + 8 * h, 2 * t, j0) |
-                                     enc_staged<ICH>(stage, r0 + 8 * i, 16 * ks + 8 * h, 2 * t + 1, j0) << 16;
+                enc[ks][2 * h + i] = enc_staged<ICH>(stage, r0 + 8 * i, 16 * ks + 8 * h, 2 * t) |
+                                     enc_staged<ICH>(stage, r0 + 8 * i, 16 * ks + 8 * h, 2 * t + 1) << 16;
         };
-        if constexpr (IS_BG) {
-            // the s columns 72-92 (enc[4][2..3], enc[5][*]), staged as coordinate 0 once per tile
-            bar_wait(P.trap, bar, cb + kStageFull, k_stage & 1);
-            FIELD_PHASE(kPhWait);
-            load_enc(KS - 2, 1, 3);
-            load_enc(KS - 1, 0, 3);
-            load_enc(KS - 1, 1, 3);
-            mbar_arrive(bar + 8u * (cb + kStageEmpty));
-            ++k_stage;
-        }
         FIELD_PHASE(kPhRows);
 
         float hacc[40];                                 // folded head: [q (64) | sigma | pad], summed over the views
@@ -769,8 +810,8 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
 #pragma unroll
             for (int ks = 0; ks < 4; ++ks)
 #pragma unroll
-                for (int h = 0; h < 2; ++h) load_enc(ks, h, 0);
-            if constexpr (IS_BG) load_enc(4, 0, 0);                                  // columns 64-71: the last levels of coordinate 2
+                for (int h = 0; h < 2; ++h) load_enc(ks, h);
+            if constexpr (IS_BG) load_enc(4, 0);                               // columns 64-71: the last levels of coordinate 2
             mbar_arrive(bar + 8u * (cb + kStageEmpty));
             ++k_stage;
             FIELD_PHASE(kPhRows);
@@ -781,7 +822,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
             // layer 0: blend of P0 + W0enc . enc (b0 on the constant-one column)
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-            blend_maps<0, !IS_BG>(acc, P, *tab, r0, t);
+            blend_maps<0, !IS_BG, !IS_BG>(acc, P, *tab, r0, t);
             FIELD_PHASE(kPhBlend0);
             wgmma_fence();
 #pragma unroll
@@ -804,7 +845,7 @@ __global__ void __launch_bounds__(kThreads, 1) field_tc_kernel(const __grid_cons
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;
             FIELD_PHASE(kPhLayers);
-            blend_maps<1, !IS_BG>(acc, P, *tab, r0, t);
+            blend_maps<1, !IS_BG, !IS_BG>(acc, P, *tab, r0, t);
             mbar_arrive(bar + 8u * (cb + kTapsEmpty));                              // the producer may build the next table
             ++k_taps;
             FIELD_PHASE(kPhBlend3);
