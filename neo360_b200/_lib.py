@@ -2,6 +2,7 @@
 
 The product path has no CPU fallback: importing the renderer without the shared library, or calling it
 without a CUDA device, raises."""
+import contextlib
 import ctypes as C
 import os
 
@@ -254,11 +255,42 @@ def check(rc: int):
         raise RuntimeError(f"neo360_b200 error {rc}: {load().neo_last_error().decode()}{load().neo_tc_trap_info().decode()}")
 
 
+@contextlib.contextmanager
+def on(x):
+    """Device guard of a library call: enters the CUDA device of tensor or device `x` and yields that device's current stream handle,
+    so the kernels and the stream handed to the library belong to the device of the call's tensors, not to the current device."""
+    import torch
+    with torch.cuda.device(x.device if torch.is_tensor(x) else x):
+        yield torch.cuda.current_stream().cuda_stream
+
+
+def workspace(need: int, device):
+    """The byte buffer of a `*_workspace_bytes` query; a query that returned 0 refused its sizes and raises with neo_last_error."""
+    import torch
+    if need == 0:
+        check(-1)
+    return torch.empty(need, dtype=torch.uint8, device=device)
+
+
+def grow(cached, need: int, device):
+    """`cached` when it is a workspace on `device` of at least `need` bytes, else a new one of `need` bytes."""
+    if cached is None or cached.numel() < need or cached.device != device:
+        return workspace(need, device)
+    return cached
+
+
+def require_cuda(t):
+    if not t.is_cuda:
+        raise ValueError("neo360_b200 takes CUDA tensors")
+
+
 def ptr(t):
-    """device pointer of a contiguous fp32 CUDA tensor (None -> NULL)."""
+    """device pointer of a contiguous CUDA tensor of a dtype the library reads (None -> NULL); bool masks go in as view(torch.uint8)."""
     if t is None:
         return None
     import torch
-    if not (t.is_cuda and t.is_contiguous() and t.dtype in (torch.float32, torch.int32, torch.uint8)):
-        raise ValueError("neo360_b200 takes contiguous fp32 CUDA tensors")
+    if not (t.is_contiguous() and t.dtype in (torch.float32, torch.int32, torch.int64, torch.uint8, torch.bfloat16, torch.float16,
+                                              torch.float64)):
+        raise ValueError(f"neo360_b200 takes contiguous CUDA tensors of fp32, fp16, bf16, float64, int32, int64 or uint8, got {t.dtype}")
+    require_cuda(t)
     return t.data_ptr()

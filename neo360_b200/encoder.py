@@ -31,6 +31,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import _lib as L
+from . import bf16
 from .training import check_train_precision
 
 
@@ -69,8 +70,8 @@ class _UpsampleBilinear(torch.autograd.Function):
         n, c, hi, wi = ctx.in_shape
         gc = g.contiguous().float()
         g_in = torch.empty(ctx.in_shape, device=gc.device)
-        with torch.cuda.device(gc.device):
-            L.check(lib.neo_upsample_bilinear_bwd(L.ptr(gc), n * c, hi, wi, gc.shape[-2], gc.shape[-1], L.ptr(g_in), _stream()))
+        with L.on(gc) as s:
+            L.check(lib.neo_upsample_bilinear_bwd(L.ptr(gc), n * c, hi, wi, gc.shape[-2], gc.shape[-1], L.ptr(g_in), s))
         return g_in, None
 
 
@@ -148,10 +149,6 @@ def _floorplan_convnet():
         nn.Conv2d(128, 128, 3, padding=1))
 
 
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
 class _Features(torch.autograd.Function):
     """Grid lookup rows: latent_cl (NV,Hl,Wl,512) channel-last -> X (NV*G^3, 518) = [latent lookup | cam xyz | masked unit direction], the
     input of depth_fc.  Returned as a view of a 520-wide buffer (16-byte rows); the gradient flows to the latent only (poses do not train)."""
@@ -164,8 +161,8 @@ class _Features(torch.autograd.Function):
         pose_c = poses.detach().contiguous().float()
         X = torch.empty(nv * GridEncoder.GRID ** 3, 520, device=lat.device)
         geo = (nv, lh, lw, int(W), int(H))
-        with torch.cuda.device(lat.device):
-            L.check(lib.neo_grid_encoder_features(L.ptr(lat), *geo, L.ptr(pose_c), focal, cx, cy, L.ptr(X), X.shape[1], _stream()))
+        with L.on(lat) as s:
+            L.check(lib.neo_grid_encoder_features(L.ptr(lat), *geo, L.ptr(pose_c), focal, cx, cy, L.ptr(X), X.shape[1], s))
         ctx.save_for_backward(pose_c)
         ctx.geo, ctx.cam = geo, (focal, cx, cy)
         ctx.det = torch.are_deterministic_algorithms_enabled()
@@ -174,7 +171,7 @@ class _Features(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_X):
         (pose_c,) = ctx.saved_tensors
-        return _lookup_bwd(L.load(), ctx, pose_c, g_X.contiguous().float()), None, None, None, None, None, None
+        return _lookup_bwd(ctx, pose_c, g_X.contiguous().float()), None, None, None, None, None, None
 
 
 class _Pool(torch.autograd.Function):
@@ -187,8 +184,8 @@ class _Pool(torch.autograd.Function):
         G = GridEncoder.GRID
         nv = lat_c.shape[0] // G ** 3
         out = [torch.empty(nv, 512, G, G, device=lat_c.device) for _ in range(3)]
-        with torch.cuda.device(lat_c.device):
-            L.check(lib.neo_grid_encoder_pool(L.ptr(lat_c), L.ptr(lg), nv, *[L.ptr(t) for t in out], _stream()))
+        with L.on(lat_c) as s:
+            L.check(lib.neo_grid_encoder_pool(L.ptr(lat_c), L.ptr(lg), nv, *[L.ptr(t) for t in out], s))
         ctx.save_for_backward(lat_c, lg)
         return tuple(out)
 
@@ -199,8 +196,8 @@ class _Pool(torch.autograd.Function):
         nv = lat_c.shape[0] // GridEncoder.GRID ** 3
         d_lat, d_logits = torch.empty_like(lat_c), torch.empty_like(lg)
         gs = [None if g is None else g.contiguous().float() for g in (g_xz, g_xy, g_yz)]
-        with torch.cuda.device(lat_c.device):
-            L.check(lib.neo_grid_encoder_pool_bwd(L.ptr(lat_c), L.ptr(lg), nv, *[L.ptr(g) for g in gs], L.ptr(d_lat), L.ptr(d_logits), _stream()))
+        with L.on(lat_c) as s:
+            L.check(lib.neo_grid_encoder_pool_bwd(L.ptr(lat_c), L.ptr(lg), nv, *[L.ptr(g) for g in gs], L.ptr(d_lat), L.ptr(d_logits), s))
         return d_lat, d_logits
 
 
@@ -218,7 +215,7 @@ class _DenseTC(torch.autograd.Function):
         lib = L.load()
         lat = latent_cl.detach().contiguous().float()
         nv, lh, lw, _ = lat.shape
-        dev, s = lat.device, _stream()
+        dev = lat.device
         pose_c = poses.detach().contiguous().float()
         R = nv * GridEncoder.GRID ** 3
         P = [t.detach().contiguous().float() for t in params]
@@ -238,23 +235,22 @@ class _DenseTC(torch.autograd.Function):
         logits = torch.empty(3, R, device=dev)
         out = [torch.empty(nv, 512, GridEncoder.GRID, GridEncoder.GRID, device=dev) for _ in range(3)]
         geo, cam = (nv, lh, lw, int(W), int(H)), (focal, cx, cy)
-        gemm = lambda a_, lda, w_, ldw, bias, c_, ldc, N, K, epi: L.check(lib.neo_tc_gemm_bf16(a_, lda, w_, ldw, L.ptr(bias), c_, ldc, R, N, K,
-                                                                                               epi, s))
-        with torch.cuda.device(dev):
+        lb, ldl = bf16.rows(Lb)
+        with L.on(dev) as s:
             for i, wi in enumerate(w):
-                L.check(lib.neo_tc_pack_bf16(L.ptr(wi), 512, wi.shape[1], wi.shape[1], Wp[i].data_ptr(), Wp[i].shape[1], Wp[i].shape[1], 0, s))
-                L.check(lib.neo_tc_pack_bf16(L.ptr(wi), 512, wi.shape[1], wi.shape[1], WT[i].data_ptr(), 512, 512, 1, s))
-            L.check(lib.neo_tc_pack_bf16(L.ptr(U), 1536, 576, 576, Up.data_ptr(), 576, 576, 0, s))
-            L.check(lib.neo_tc_pack_bf16(L.ptr(U), 1536, 576, 576, UT.data_ptr(), 512, 1536, 1, s))
-            L.check(lib.neo_grid_encoder_features_bf16(L.ptr(lat), *geo, L.ptr(pose_c), *cam, X.data_ptr(), 576, s))
-            gemm(X.data_ptr(), 576, Wp[0].data_ptr(), 576, b[0], H0.data_ptr(), 512, 512, 576, 0)
-            gemm(H0.data_ptr(), 512, Wp[1].data_ptr(), 512, b[1], H1.data_ptr(), 512, 512, 512, 0)
-            gemm(H1.data_ptr(), 512, Wp[2].data_ptr(), 512, b[2], Lb.data_ptr(), 576, 512, 512, 1)
-            L.check(lib.neo_grid_encoder_coords_bf16(Lb.data_ptr(), nv, 576, s))
-            gemm(Lb.data_ptr(), 576, Up.data_ptr(), 576, cs, A.data_ptr(), 1536, 1536, 576, 0)
+                bf16.pack(wi, Wp[i], False, s)
+                bf16.pack(wi, WT[i], True, s)
+            bf16.pack(U, Up, False, s)
+            bf16.pack(U, UT, True, s)
+            L.check(lib.neo_grid_encoder_features_bf16(L.ptr(lat), *geo, L.ptr(pose_c), *cam, *bf16.rows(X), s))
+            bf16.gemm(X, Wp[0], b[0], H0, 0, s)
+            bf16.gemm(H0, Wp[1], b[1], H1, 0, s)
+            bf16.gemm(H1, Wp[2], b[2], Lb[:, :512], 1, s)
+            L.check(lib.neo_grid_encoder_coords_bf16(lb, nv, ldl, s))
+            bf16.gemm(Lb, Up, cs, A, 0, s)
             for a in range(3):
-                L.check(lib.neo_tc_rowdot_bf16(A.data_ptr() + 1024 * a, 1536, 512, L.ptr(q[a]), L.ptr(e[a]), 1, R, logits[a].data_ptr(), s))
-            L.check(lib.neo_grid_encoder_pool_bf16(Lb.data_ptr(), 576, L.ptr(logits), nv, *[t.data_ptr() for t in out], s))
+                bf16.rowdot(A[:, 512 * a:512 * (a + 1)], q[a], e[a], logits[a], s)
+            L.check(lib.neo_grid_encoder_pool_bf16(lb, ldl, L.ptr(logits), nv, *[L.ptr(t) for t in out], s))
         ctx.save_for_backward(X, H0, H1, Lb, A, logits, *WT, UT, pose_c, *q)
         ctx.geo, ctx.cam = geo, cam
         ctx.det = torch.are_deterministic_algorithms_enabled()
@@ -265,72 +261,64 @@ class _DenseTC(torch.autograd.Function):
         lib = L.load()
         X, H0, H1, Lb, A, logits, *rest = ctx.saved_tensors
         WT, UT, pose_c, q = rest[0:3], rest[3], rest[4], rest[5:8]
-        nv, lh, lw, _, _ = ctx.geo
-        R, dev, s = X.shape[0], X.device, _stream()
+        nv = ctx.geo[0]
+        R, dev = X.shape[0], X.device
         bf = lambda *shape: torch.empty(*shape, dtype=torch.bfloat16, device=dev)
         gs = [None if g is None else g.contiguous().float() for g in (g_xz, g_xy, g_yz)]
-        need = max(lib.neo_tc_wgrad_bf16_workspace_bytes(*c) for c in ((R, 64, 512), (R, 1536, 576), (R, 512, 512), (R, 512, 576)))
-        if need == 0:
-            L.check(-1)
-        ws = torch.empty(need, dtype=torch.uint8, device=dev)
-        wg = lambda dy, ldy, x, ldx, N, K, dw, kv, db: L.check(lib.neo_tc_wgrad_bf16(dy, ldy, x, ldx, R, N, K, L.ptr(dw), kv, L.ptr(db),
-                                                                                     ws.data_ptr(), need, s))
+        ws = L.workspace(max(lib.neo_tc_wgrad_bf16_workspace_bytes(R, *c) for c in ((64, 512), (1536, 576), (512, 512), (512, 576))), dev)
         d_pool, d_lg = torch.empty(R, 512, device=dev), torch.empty(3, R, device=dev)
         dA, g1 = bf(R, 1536), bf(R, 64)
         agg = []
-        with torch.cuda.device(dev):
-            L.check(lib.neo_grid_encoder_pool_bwd_bf16(Lb.data_ptr(), 576, L.ptr(logits), nv, *[L.ptr(g) for g in gs], L.ptr(d_pool),
-                                                       L.ptr(d_lg), s))
+        with L.on(dev) as s:
+            L.check(lib.neo_grid_encoder_pool_bwd_bf16(*bf16.rows(Lb), L.ptr(logits), nv, *[L.ptr(g) for g in gs], L.ptr(d_pool), L.ptr(d_lg),
+                                                       s))
             for a in range(3):
-                L.check(lib.neo_tc_relu_rank1_bf16(L.ptr(d_lg[a]), L.ptr(q[a]), A.data_ptr() + 1024 * a, 1536, R, 512, dA.data_ptr() + 1024 * a,
-                                                   1536, s))
-                L.check(lib.neo_tc_pack_bf16(L.ptr(d_lg[a]), R, 1, 1, g1.data_ptr(), 64, 64, 0, s))
+                cols = slice(512 * a, 512 * (a + 1))
+                bf16.relu_rank1(d_lg[a], q[a], A[:, cols], dA[:, cols], s)
+                bf16.pack(d_lg[a][:, None], g1, False, s)
                 gq = torch.empty(64, 512, device=dev)
-                wg(g1.data_ptr(), 64, A.data_ptr() + 1024 * a, 1536, 64, 512, gq, 512, None)
+                bf16.wgrad(g1, A[:, cols], gq, None, ws, s)
                 agg.append((gq[:1].clone(), d_lg[a].sum().reshape(1)))
             gU, gc = torch.empty(1536, 515, device=dev), torch.empty(1536, device=dev)
-            wg(dA.data_ptr(), 1536, Lb.data_ptr(), 576, 1536, 576, gU, 515, gc)
+            bf16.wgrad(dA, Lb, gU, gc, ws, s)
             d_agg = torch.empty(R, 512, device=dev)
-            L.check(lib.neo_tc_gemm_bf16(dA.data_ptr(), 1536, UT.data_ptr(), 1536, None, d_agg.data_ptr(), 512, R, 512, 1536, 2, s))
+            bf16.gemm(dA, UT, None, d_agg, 2, s)
             del dA
             G = [bf(R, 512), bf(R, 512)]
-            L.check(lib.neo_grid_encoder_lat_grad_bf16(L.ptr(d_pool), L.ptr(d_agg), nv, G[0].data_ptr(), s))
+            L.check(lib.neo_grid_encoder_lat_grad_bf16(L.ptr(d_pool), L.ptr(d_agg), nv, L.ptr(G[0]), s))
             del d_pool, d_agg
             grads = [None] * 6
-            for i, x, ldx in ((2, H1, 512), (1, H0, 512), (0, X, 576)):
+            for i, x in ((2, H1), (1, H0), (0, X)):
                 gw, gb = torch.empty(512, 518 if i == 0 else 512, device=dev), torch.empty(512, device=dev)
-                wg(G[0].data_ptr(), 512, x.data_ptr(), ldx, 512, ldx, gw, gw.shape[1], gb)
+                bf16.wgrad(G[0], x, gw, gb, ws, s)
                 grads[2 * i], grads[2 * i + 1] = gw, gb
                 if i > 0:
-                    L.check(lib.neo_tc_dgrad_bf16(G[0].data_ptr(), 512, WT[i].data_ptr(), 512, x.data_ptr(), 512, None, None, G[1].data_ptr(), 512,
-                                                  R, 512, 512, s))
+                    bf16.dgrad(G[0], WT[i], x, None, None, G[1], s)
                     G.reverse()
             g_lat = None
             if ctx.needs_input_grad[0]:
                 g_X = torch.empty(R, 512, device=dev)
-                L.check(lib.neo_tc_gemm_bf16(G[0].data_ptr(), 512, WT[0].data_ptr(), 512, None, g_X.data_ptr(), 512, R, 512, 512, 2, s))
-                g_lat = _lookup_bwd(lib, ctx, pose_c, g_X)
+                bf16.gemm(G[0], WT[0], None, g_X, 2, s)
+                g_lat = _lookup_bwd(ctx, pose_c, g_X)
         for a in range(3):
             rows = slice(512 * a, 512 * (a + 1))
             grads += [torch.cat([gU[rows, :512], gU[rows, 512 + a:513 + a]], 1), gc[rows].clone(), *agg[a]]
         return (g_lat, None, None, None, None, None, None, *grads)
 
 
-def _lookup_bwd(lib, ctx, pose_c, g):
+def _lookup_bwd(ctx, pose_c, g):
     """Latent gradient (NV,Hl,Wl,512) of the lookup rows' 512 lookup columns g (R, ld) fp32: the order-fixed scatter under
     torch.use_deterministic_algorithms (ctx.det, recorded in the forward), the atomic one otherwise."""
+    lib = L.load()
     nv, lh, lw, _, _ = ctx.geo
     g_lat = torch.zeros(nv, lh, lw, 512, device=g.device)
-    with torch.cuda.device(g.device):
+    with L.on(g) as s:
         if ctx.det:                 # order-fixed scatter: bit-reproducible
-            need = lib.neo_grid_encoder_features_bwd_det_workspace_bytes(nv, lh, lw)
-            if need == 0:
-                L.check(-1)
-            ws = torch.empty(need, dtype=torch.uint8, device=g.device)
+            ws = L.workspace(lib.neo_grid_encoder_features_bwd_det_workspace_bytes(nv, lh, lw), g.device)
             L.check(lib.neo_grid_encoder_features_bwd_det(*ctx.geo, L.ptr(pose_c), *ctx.cam, L.ptr(g), g.stride(0), L.ptr(g_lat), L.ptr(ws),
-                                                          need, _stream()))
+                                                          ws.numel(), s))
         else:
-            L.check(lib.neo_grid_encoder_features_bwd(*ctx.geo, L.ptr(pose_c), *ctx.cam, L.ptr(g), g.stride(0), L.ptr(g_lat), _stream()))
+            L.check(lib.neo_grid_encoder_features_bwd(*ctx.geo, L.ptr(pose_c), *ctx.cam, L.ptr(g), g.stride(0), L.ptr(g_lat), s))
     return g_lat
 
 
@@ -439,7 +427,7 @@ class GridEncoder(nn.Module):
         lat = latent.detach().contiguous().float()
         NV, _, lh, lw = lat.shape
         keep = []
-        f = lambda t: (keep.append(t.detach().contiguous().float()) or keep[-1].data_ptr())
+        f = lambda t: (keep.append(t.detach().contiguous().float()) or L.ptr(keep[-1]))
         p = L.NeoGridEncoderParams()
         fc = [self.depth_fc.common_branch[0], self.depth_fc.common_branch[2], self.depth_fc.depth_encoder]
         for i, m in enumerate(fc):
@@ -448,15 +436,13 @@ class GridEncoder(nn.Module):
             agg = getattr(self, f"pillar_aggregator_{pl}")
             setattr(p, f"agg_{pl}_w0", f(agg[0].weight)); setattr(p, f"agg_{pl}_b0", f(agg[0].bias))
             setattr(p, f"agg_{pl}_w1", f(agg[2].weight)); setattr(p, f"agg_{pl}_b1", f(agg[2].bias))
-        need = lib.neo_grid_encoder_workspace_bytes(NV, lh, lw)
-        if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        self._ws = L.grow(self._ws, lib.neo_grid_encoder_workspace_bytes(NV, lh, lw), dev)
         out = [torch.empty(NV, 512, self.GRID, self.GRID, device=dev) for _ in range(3)]
         pose_c = poses.detach().contiguous().float()
-        with torch.cuda.device(dev):
-            L.check(lib.neo_grid_encoder_dense(C.byref(p), lat.data_ptr(), NV, lh, lw, int(W), int(H), pose_c.data_ptr(), float(focal[0]),
-                                               float(c[0, 0]), float(c[0, 1]), out[0].data_ptr(), out[1].data_ptr(), out[2].data_ptr(),
-                                               self._ws.data_ptr(), self._ws.numel(), torch.cuda.current_stream().cuda_stream))
+        with L.on(dev) as s:
+            L.check(lib.neo_grid_encoder_dense(C.byref(p), L.ptr(lat), NV, lh, lw, int(W), int(H), L.ptr(pose_c), float(focal[0]),
+                                               float(c[0, 0]), float(c[0, 1]), L.ptr(out[0]), L.ptr(out[1]), L.ptr(out[2]),
+                                               L.ptr(self._ws), self._ws.numel(), s))
         return out[0], out[1], out[2]
 
     def _spatial_latent(self, images):

@@ -41,12 +41,8 @@ def _vgg16_features() -> nn.Sequential:
     return nn.Sequential(*layers)
 
 
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
 def _ptrs(ts: Sequence[Tensor]):
-    return (C.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
+    return (C.c_void_p * len(ts))(*[L.ptr(t) for t in ts])
 
 
 def _check_features(fx: Sequence[Tensor], fy: Sequence[Tensor], w: Sequence[Tensor]):
@@ -73,12 +69,11 @@ def head(fx: Sequence[Tensor], fy: Sequence[Tensor], w: Sequence[Tensor], per_la
     if nbytes == 0:
         raise ValueError(f"LPIPS needs n >= 1 frames of at least {MIN_SIZE}x{MIN_SIZE} pixels, got n {n}, {H}x{W}")
     dev = fx[0].device
-    ws = torch.empty(nbytes // 8, dtype=torch.float64, device=dev)
+    ws = L.workspace(nbytes, dev)
     out = torch.empty(n, dtype=torch.float64, device=dev)
     lay = torch.empty(n, 5, dtype=torch.float64, device=dev) if per_layer else None
-    with torch.cuda.device(dev):
-        L.check(lib.neo_lpips_head(_ptrs(fx), _ptrs(fy), _ptrs(w), n, H, W, out.data_ptr(), None if lay is None else lay.data_ptr(),
-                                   ws.data_ptr(), nbytes, _stream()))
+    with L.on(dev) as s:
+        L.check(lib.neo_lpips_head(_ptrs(fx), _ptrs(fy), _ptrs(w), n, H, W, L.ptr(out), L.ptr(lay), L.ptr(ws), nbytes, s))
     return (out, lay) if per_layer else out
 
 
@@ -90,9 +85,9 @@ def head_bwd(fx: Sequence[Tensor], fy: Sequence[Tensor], w: Sequence[Tensor], g:
     gc = g.detach().to(device=fx[0].device, dtype=torch.float32).contiguous()
     gx = [torch.empty_like(t) for t in fx]
     gy = [torch.empty_like(t) for t in fy] if with_y else None
-    with torch.cuda.device(gc.device):
-        L.check(L.load().neo_lpips_head_bwd(_ptrs(fx), _ptrs(fy), _ptrs(w), n, H, W, gc.data_ptr(), _ptrs(gx), None if gy is None else _ptrs(gy),
-                                            _stream()))
+    with L.on(gc) as s:
+        L.check(L.load().neo_lpips_head_bwd(_ptrs(fx), _ptrs(fy), _ptrs(w), n, H, W, L.ptr(gc), _ptrs(gx), None if gy is None else _ptrs(gy),
+                                            s))
     return gx, gy
 
 
@@ -125,8 +120,8 @@ class _Prepare(torch.autograd.Function):
             raise ValueError(f"LPIPS takes (n, H, W, 3) frames, got {tuple(img.shape)}")
         n, H, W, _ = x.shape
         out = torch.empty(n, 3, H, W, device=x.device)
-        with torch.cuda.device(x.device):
-            L.check(L.load().neo_lpips_prepare(x.data_ptr(), n, H, W, int(form), out.data_ptr(), _stream()))
+        with L.on(x) as s:
+            L.check(L.load().neo_lpips_prepare(L.ptr(x), n, H, W, int(form), L.ptr(out), s))
         ctx.save_for_backward(x)
         ctx.form = int(form)
         return out
@@ -136,8 +131,8 @@ class _Prepare(torch.autograd.Function):
         (x,) = ctx.saved_tensors
         n, H, W, _ = x.shape
         gi = torch.empty_like(x)
-        with torch.cuda.device(x.device):
-            L.check(L.load().neo_lpips_prepare_bwd(x.data_ptr(), g.contiguous().float().data_ptr(), n, H, W, ctx.form, gi.data_ptr(), _stream()))
+        with L.on(x) as s:
+            L.check(L.load().neo_lpips_prepare_bwd(L.ptr(x), L.ptr(g.contiguous().float()), n, H, W, ctx.form, L.ptr(gi), s))
         return gi, None
 
 

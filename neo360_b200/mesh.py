@@ -191,8 +191,7 @@ def density_grid(net, resolution, bbox=UNIT_BOX, level: Optional[int] = None, pr
     d = torch.empty(slab, 3, device=dev)
     t = torch.empty(slab, nx, device=dev)
     lib = L.load()
-    with torch.cuda.device(dev):
-        s = torch.cuda.current_stream().cuda_stream
+    with L.on(dev) as s:
         for r0 in range(0, rows, slab):
             n = min(slab, rows - r0)
             L.check(lib.neo_grid_rays(C.byref(g), r0, n, L.ptr(o), L.ptr(d), L.ptr(t), s))
@@ -210,18 +209,14 @@ def marching_tetrahedra(sigma: torch.Tensor, iso: float, bbox=UNIT_BOX):
     g = _grid_of(sigma, bbox)
     sig = sigma.contiguous()
     lib = L.load()
-    need = lib.neo_mt_workspace_bytes(C.byref(g))
-    if need == 0:
-        raise RuntimeError("neo360_b200: " + lib.neo_last_error().decode())
     dev = sig.device
-    ws = torch.empty(need, dtype=torch.uint8, device=dev)
+    ws = L.workspace(lib.neo_mt_workspace_bytes(C.byref(g)), dev)
     nv, nf = C.c_int(), C.c_int()
-    with torch.cuda.device(dev):
-        s = torch.cuda.current_stream().cuda_stream
-        L.check(lib.neo_mt_count(L.ptr(sig), C.byref(g), float(iso), L.ptr(ws), need, C.byref(nv), C.byref(nf), s))
+    with L.on(dev) as s:
+        L.check(lib.neo_mt_count(L.ptr(sig), C.byref(g), float(iso), L.ptr(ws), ws.numel(), C.byref(nv), C.byref(nf), s))
         verts = torch.empty(nv.value, 3, device=dev)
         faces = torch.empty(nf.value, 3, dtype=torch.int32, device=dev)
-        L.check(lib.neo_mt_emit(L.ptr(sig), C.byref(g), float(iso), L.ptr(ws), need, L.ptr(verts) if nv.value else None, nv.value,
+        L.check(lib.neo_mt_emit(L.ptr(sig), C.byref(g), float(iso), L.ptr(ws), ws.numel(), L.ptr(verts) if nv.value else None, nv.value,
                                 L.ptr(faces) if nf.value else None, nf.value, s))
     return verts, faces
 
@@ -232,9 +227,8 @@ def grid_normals(sigma: torch.Tensor, verts: torch.Tensor, bbox=UNIT_BOX) -> tor
     v = verts.contiguous().float()
     out = torch.empty_like(v)
     if v.shape[0]:
-        with torch.cuda.device(v.device):
-            L.check(L.load().neo_grid_normals(L.ptr(sigma.contiguous()), C.byref(g), L.ptr(v), v.shape[0], L.ptr(out),
-                                              torch.cuda.current_stream().cuda_stream))
+        with L.on(v) as s:
+            L.check(L.load().neo_grid_normals(L.ptr(sigma.contiguous()), C.byref(g), L.ptr(v), v.shape[0], L.ptr(out), s))
     return out
 
 

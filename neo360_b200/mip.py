@@ -110,12 +110,8 @@ class MipNeRF360(nn.Module):
             for i in range(3):
                 j = jit[i].reshape(-1).contiguous()
                 keep.append(j)
-                cfg.jitter[i] = j.data_ptr()
-        need = lib.neo_mip_workspace_bytes(n, C.byref(cfg), self.mlps[2].netwidth)
-        if need == 0:
-            raise RuntimeError("neo360_b200: " + lib.neo_last_error().decode())
-        if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+                cfg.jitter[i] = L.ptr(j)
+        self._ws = L.grow(self._ws, lib.neo_mip_workspace_bytes(n, C.byref(cfg), self.mlps[2].netwidth), dev)
         ns = (cfg.n_prop, cfg.n_prop, cfg.n_nerf)
         out = L.NeoMipOut()
         ren, hist = [], []
@@ -123,12 +119,12 @@ class MipNeRF360(nn.Module):
             T = {"rgb": torch.empty(n, 3, device=dev), "density": torch.empty(n, ns[l], device=dev), "rgb_s": torch.empty(n, ns[l], 3, device=dev),
                  "sdist": torch.empty(n, ns[l] + 1, device=dev), "weights": torch.empty(n, ns[l], device=dev)}
             for k, t in T.items():
-                getattr(out, k)[l] = t.data_ptr()
+                getattr(out, k)[l] = L.ptr(t)
             ren.append({"rgb": T["rgb"]})
             hist.append({"density": T["density"], "rgb": T["rgb_s"], "sdist": T["sdist"], "weights": T["weights"]})
-        with torch.cuda.device(dev):
-            L.check(lib.neo_mip_render_fwd(arr, L.ptr(o), L.ptr(d), L.ptr(vd), L.ptr(radii), n, C.byref(cfg), C.byref(out), self._ws.data_ptr(),
-                                           self._ws.numel(), torch.cuda.current_stream().cuda_stream))
+        with L.on(dev) as s:
+            L.check(lib.neo_mip_render_fwd(arr, L.ptr(o), L.ptr(d), L.ptr(vd), L.ptr(radii), n, C.byref(cfg), C.byref(out), L.ptr(self._ws),
+                                           self._ws.numel(), s))
         return ren, hist
 
     @torch.no_grad()
@@ -153,16 +149,16 @@ class MipNeRF360(nn.Module):
         need = lib.neo_mip_field_workspace_bytes(n * N, self.mlps[level].netwidth if 0 <= level < 3 else 0, P)
         if need == 0:
             raise ValueError(f"Mip-NeRF 360 field: bad level {level} or size {n} x {N}")
-        ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        ws = L.workspace(need, dev)
         r = L.NeoRays()
         r.n_rays, r.chunk = n, 0
         r.rays_o, r.rays_d, r.viewdirs = L.ptr(o), L.ptr(vd), L.ptr(vd)
         v = (C.c_float * 3)(*[float(x) for x in var])
         out_rgb = torch.empty(n, N, 3, device=dev) if rgb and level == 2 else None
         density = torch.empty(n, N, device=dev)
-        with torch.cuda.device(dev):
+        with L.on(dev) as s:
             L.check(lib.neo_mip_field_eval(arr, int(level), C.byref(r), L.ptr(t), N, v, P, L.ptr(out_rgb), L.ptr(density), L.ptr(ws), need,
-                                           torch.cuda.current_stream().cuda_stream))
+                                           s))
         return out_rgb, density
 
     def density_grid(self, resolution, bbox=((-1.0, -1.0, -1.0), (1.0, 1.0, 1.0)), level: int = 2, precision: Optional[str] = None,
@@ -186,18 +182,17 @@ class MipNeRF360(nn.Module):
         if randomized:
             jit = batch.get("_uniforms") or [torch.rand((n, 1), device=dev) for _ in range(3)]     # helper.py:361 (single_jitter)
             jit = [j.reshape(-1).contiguous().float() for j in jit]
-        stream = torch.cuda.current_stream(dev).cuda_stream
         ns = (self.num_prop_samples, self.num_prop_samples, self.num_nerf_samples)
         tc = check_train_precision(self.train_precision) == "tc"
         ren, hist = [], []
         sdist = w = None
         for lvl, mlp in enumerate(self.mlps):
             N = ns[lvl]
-            with torch.cuda.device(dev):
+            with L.on(dev) as s:
                 s1, t1 = torch.empty(n, N + 1, device=dev), torch.empty(n, N + 1, device=dev)
                 wp = w.detach().contiguous() if lvl else None
                 L.check(lib.neo_mip_resample(L.ptr(sdist), L.ptr(wp), n, ns[lvl - 1] if lvl else 1, lvl, N, float(near), float(far),
-                                             float(train_frac), L.ptr(jit[lvl]), L.ptr(s1), L.ptr(t1), stream))
+                                             float(train_frac), L.ptr(jit[lvl]), L.ptr(s1), L.ptr(t1), s))
                 sdist = s1
                 basis = mlp.pos_basis_t.to(dev).contiguous().float()
                 if vd.requires_grad:
@@ -205,7 +200,7 @@ class MipNeRF360(nn.Module):
                 else:
                     feats, denc = torch.empty(n * N, 504, device=dev), torch.empty(n, 27, device=dev)
                     L.check(lib.neo_mip_encode(L.ptr(o), L.ptr(d), L.ptr(vd), L.ptr(radii), L.ptr(t1), L.ptr(basis), n, N, L.ptr(feats),
-                                               L.ptr(denc), stream))
+                                               L.ptr(denc), s))
             if tc:
                 raw_density, raw_rgb = mlp_train_tc(mlp, feats, denc, n, N)
                 raw_density = raw_density.reshape(n, N)
@@ -249,9 +244,9 @@ class _MipEncode(torch.autograd.Function):
         o, d, vd, radii, tdist = (x.detach().contiguous().float() for x in (o, d, vd, radii, tdist))
         n, N = tdist.shape[0], tdist.shape[1] - 1
         feats, denc = torch.empty(n * N, 504, device=o.device), torch.empty(n, 27, device=o.device)
-        with torch.cuda.device(o.device):
+        with L.on(o) as s:
             L.check(lib.neo_mip_encode(L.ptr(o), L.ptr(d), L.ptr(vd), L.ptr(radii), L.ptr(tdist), L.ptr(basis), n, N, L.ptr(feats), L.ptr(denc),
-                                       torch.cuda.current_stream(o.device).cuda_stream))
+                                       s))
         ctx.save_for_backward(vd)
         return feats, denc
 
@@ -262,9 +257,9 @@ class _MipEncode(torch.autograd.Function):
         n = vd.shape[0]
         g_vd = torch.zeros(n, 3, device=vd.device)
         if g_denc is not None:
-            with torch.cuda.device(vd.device):
+            with L.on(vd) as s:
                 L.check(lib.neo_mip_encode_bwd(L.ptr(vd), n, L.ptr(g_denc.contiguous().float()), L.ptr(g_vd),
-                                               torch.cuda.current_stream(vd.device).cuda_stream))
+                                               s))
         return None, None, g_vd, None, None, None
 
 
@@ -282,9 +277,9 @@ class _MipComposite(torch.autograd.Function):
         n, N = rd.shape
         dev = rd.device
         rgb, w, dens, rgb_s = torch.empty(n, 3, device=dev), torch.empty(n, N, device=dev), torch.empty(n, N, device=dev), torch.empty(n, N, 3, device=dev)
-        with torch.cuda.device(dev):
+        with L.on(dev) as s:
             L.check(lib.neo_mip_composite(L.ptr(rd), L.ptr(rc), L.ptr(t), L.ptr(d), n, N, L.ptr(rgb), L.ptr(w), L.ptr(dens), L.ptr(rgb_s),
-                                          torch.cuda.current_stream(dev).cuda_stream))
+                                          s))
         ctx.save_for_backward(rd, rc, t, d)
         ctx.want_d = rays_d.requires_grad
         if rc is None:
@@ -302,14 +297,14 @@ class _MipComposite(torch.autograd.Function):
         f = lambda g: None if g is None else g.contiguous().float()
         gs = [L.ptr(f(g_rgb)), L.ptr(f(g_w)), L.ptr(f(g_dens)), L.ptr(f(g_rgb_s) if rc is not None else None)]
         g_d = None
-        with torch.cuda.device(dev):
+        with L.on(dev) as s:
             if ctx.needs_input_grad[3]:
                 g_d = torch.empty(n, 3, device=dev)
                 L.check(lib.neo_mip_composite_bwd_rays_d(L.ptr(rd), L.ptr(rc), L.ptr(t), L.ptr(d), n, N, *gs, L.ptr(d_rd), L.ptr(d_rc), L.ptr(g_d),
-                                                         torch.cuda.current_stream(dev).cuda_stream))
+                                                         s))
             else:
                 L.check(lib.neo_mip_composite_bwd(L.ptr(rd), L.ptr(rc), L.ptr(t), L.ptr(d), n, N, *gs, L.ptr(d_rd), L.ptr(d_rc),
-                                                  torch.cuda.current_stream(dev).cuda_stream))
+                                                  s))
         return d_rd, d_rc, None, g_d
 
 
@@ -334,8 +329,8 @@ class _Interlevel(torch.autograd.Function):
         n, Nc = ts[1].shape
         Np = ts[3].shape[1]
         out = torch.empty(n, device=ts[0].device)
-        with torch.cuda.device(out.device):
-            L.check(lib.neo_interlevel_loss(*[L.ptr(x) for x in ts], n, Nc, Np, L.ptr(out), torch.cuda.current_stream(out.device).cuda_stream))
+        with L.on(out) as s:
+            L.check(lib.neo_interlevel_loss(*[L.ptr(x) for x in ts], n, Nc, Np, L.ptr(out), s))
         ctx.save_for_backward(*ts)
         return out
 
@@ -346,9 +341,9 @@ class _Interlevel(torch.autograd.Function):
         n, Nc = ts[1].shape
         Np = ts[3].shape[1]
         d_we = torch.empty_like(ts[3])
-        with torch.cuda.device(d_we.device):
+        with L.on(d_we) as s:
             L.check(lib.neo_interlevel_loss_bwd(*[L.ptr(x) for x in ts], n, Nc, Np, L.ptr(g.contiguous().float()), L.ptr(d_we),
-                                                torch.cuda.current_stream(d_we.device).cuda_stream))
+                                                s))
         return None, None, None, d_we
 
 

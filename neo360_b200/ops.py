@@ -15,28 +15,25 @@ import torch
 from . import _lib as L
 
 
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
-class _on:
-    """Device guard: kernels and the stream handed to the library belong to the device of the call's tensors, not to whatever device
-    happens to be current in the process (ADVICE round 1)."""
-
-    def __init__(self, t):
-        self.g = torch.cuda.device(t.device)
-
-    def __enter__(self):
-        self.g.__enter__()
-
-    def __exit__(self, *e):
-        return self.g.__exit__(*e)
-
-
 def _f32(t):
     if not t.is_cuda:
         raise RuntimeError("neo360_b200 ops run on CUDA tensors only (no CPU fallback)")
     return t.contiguous().float()
+
+
+def _sample_rays(pix, H, W, focal, m, img, check):
+    """neo_sample_rays: pix (n) int64, m (T,3,4), img (T,H,W,3) or None -> rays_o, viewdirs, rays_d, radii (n,1), target or None."""
+    n = pix.numel()
+    o = torch.empty(n, 3, device=m.device); vd = torch.empty_like(o); rd = torch.empty_like(o)
+    rad = torch.empty(n, 1, device=m.device)
+    tgt = torch.empty(n, 3, device=m.device) if img is not None else None
+    err = torch.zeros(1, dtype=torch.int32, device=m.device)
+    with L.on(m) as s:
+        L.check(L.load().neo_sample_rays(n, L.ptr(pix), m.shape[0], H, W, float(focal), L.ptr(m), L.ptr(img), L.ptr(o), L.ptr(vd), L.ptr(rd),
+                                         L.ptr(rad), L.ptr(tgt), L.ptr(err), s))
+    if check and int(err.item()):   # the reference's fancy indexing raises IndexError synchronously
+        raise IndexError("sample_rays: pix_inds out of range")
+    return o, vd, rd, rad, tgt
 
 
 class _RaysFromPoses(torch.autograd.Function):
@@ -46,18 +43,8 @@ class _RaysFromPoses(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, c2w, pix, H, W, focal, img, check):
-        lib = L.load()
         m = c2w.detach().contiguous().float()
-        n, T = pix.numel(), m.shape[0]
-        o = torch.empty(n, 3, device=m.device); vd = torch.empty_like(o); rd = torch.empty_like(o)
-        rad = torch.empty(n, 1, device=m.device)
-        tgt = torch.empty(n, 3, device=m.device) if img is not None else None
-        err = torch.zeros(1, dtype=torch.int32, device=m.device)
-        with _on(m):
-            L.check(lib.neo_sample_rays(n, pix.data_ptr(), T, H, W, float(focal), L.ptr(m), L.ptr(img), L.ptr(o), L.ptr(vd), L.ptr(rd),
-                                        L.ptr(rad), L.ptr(tgt), L.ptr(err), _stream()))
-        if check and int(err.item()):   # the reference's fancy indexing raises IndexError synchronously
-            raise IndexError("sample_rays: pix_inds out of range")
+        o, vd, rd, rad, tgt = _sample_rays(pix, H, W, focal, m, img, check)
         ctx.save_for_backward(m, pix)
         ctx.dims = (H, W, float(focal))
         ctx.mark_non_differentiable(rad)
@@ -74,11 +61,11 @@ class _RaysFromPoses(torch.autograd.Function):
         n, T = pix.numel(), m.shape[0]
         f = lambda g: None if g is None else g.contiguous().float()
         need = lib.neo_sample_rays_bwd_workspace_bytes(n, T)
-        ws = torch.empty(max(need, 1), dtype=torch.uint8, device=m.device)
+        ws = L.workspace(need, m.device) if n else None          # no rays: no workspace, the call only zeroes g_c2w
         g_c2w = torch.empty(T, 3, 4, device=m.device)
-        with _on(m):
-            L.check(lib.neo_sample_rays_bwd(n, pix.data_ptr(), T, H, W, focal, L.ptr(m), L.ptr(f(g_o)), L.ptr(f(g_vd)), L.ptr(f(g_rd)),
-                                            L.ptr(g_c2w), L.ptr(ws), need, _stream()))
+        with L.on(m) as s:
+            L.check(lib.neo_sample_rays_bwd(n, L.ptr(pix), T, H, W, focal, L.ptr(m), L.ptr(f(g_o)), L.ptr(f(g_vd)), L.ptr(f(g_rd)),
+                                            L.ptr(g_c2w), L.ptr(ws), need, s))
         return g_c2w, None, None, None, None, None, None
 
 
@@ -99,8 +86,8 @@ def get_rays(H, W, focal, c2w, output_radii=True):
     n = H * W
     o = torch.empty(n, 3, device=m.device); vd = torch.empty_like(o); rd = torch.empty_like(o)
     rad = torch.empty(n, device=m.device) if output_radii else None
-    with _on(m):
-        L.check(lib.neo_get_rays(H, W, float(focal), L.ptr(m), L.ptr(o), L.ptr(vd), L.ptr(rd), L.ptr(rad), _stream()))
+    with L.on(m) as s:
+        L.check(lib.neo_get_rays(H, W, float(focal), L.ptr(m), L.ptr(o), L.ptr(vd), L.ptr(rd), L.ptr(rad), s))
     return (o, vd, rd, rad) if output_radii else (o, vd, rd)
 
 
@@ -108,12 +95,11 @@ def sample_rays(pix_inds, H, W, focal, c2w, images=None, check=True):
     """The `pix_inds`-selected rays of the (T, H, W) stack of target views (nerds360_ae.py:730-748) without building the stack.
     pix_inds (n) int64 CUDA, c2w (T,3,4) CUDA, images (T,H,W,3) fp32 CUDA or None -> rays_o, viewdirs, rays_d, radii (n,1), target.
     When c2w requires grad, rays_o, viewdirs and rays_d are differentiable w.r.t. it (neo_sample_rays_bwd; the same bits forward)."""
-    lib = L.load()
     m = _f32(c2w[:, :3, :4])
     if not pix_inds.is_cuda or pix_inds.dtype != torch.int64:
         raise RuntimeError("sample_rays: pix_inds must be an int64 CUDA tensor")
     pix = pix_inds.contiguous()
-    n, T = pix.numel(), m.shape[0]
+    T = m.shape[0]
     img = None
     if images is not None:
         img = _f32(images)
@@ -122,16 +108,7 @@ def sample_rays(pix_inds, H, W, focal, c2w, images=None, check=True):
     if _pose_grad(c2w):
         out = _RaysFromPoses.apply(m, pix, H, W, focal, img, check)
         return out if img is not None else (*out, None)
-    o = torch.empty(n, 3, device=m.device); vd = torch.empty_like(o); rd = torch.empty_like(o)
-    rad = torch.empty(n, 1, device=m.device)
-    tgt = torch.empty(n, 3, device=m.device) if img is not None else None
-    err = torch.zeros(1, dtype=torch.int32, device=m.device)
-    with _on(m):
-        L.check(lib.neo_sample_rays(n, pix.data_ptr(), T, H, W, float(focal), L.ptr(m), L.ptr(img), L.ptr(o), L.ptr(vd), L.ptr(rd), L.ptr(rad),
-                                    L.ptr(tgt), L.ptr(err), _stream()))
-    if check and int(err.item()):   # the reference's fancy indexing raises IndexError synchronously
-        raise IndexError("sample_rays: pix_inds out of range")
-    return o, vd, rd, rad, tgt
+    return _sample_rays(pix, H, W, focal, m, img, check)
 
 
 def intersect_sphere(rays_o, rays_d):
@@ -140,8 +117,8 @@ def intersect_sphere(rays_o, rays_d):
     n = o.shape[0]
     far = torch.empty(n, 1, device=o.device)
     err = torch.zeros(1, dtype=torch.int32, device=o.device)
-    with _on(o):
-        L.check(lib.neo_intersect_sphere(L.ptr(o), L.ptr(d), n, L.ptr(far), L.ptr(err), _stream()))
+    with L.on(o) as s:
+        L.check(lib.neo_intersect_sphere(L.ptr(o), L.ptr(d), n, L.ptr(far), L.ptr(err), s))
     if int(err.item()):   # the reference asserts synchronously here (helper.py:271)
         raise AssertionError("1.0 - p_norm_sq should be greater than 0")
     return far
@@ -159,18 +136,12 @@ def sample_along_rays(rays_o, rays_d, num_samples, near, far, randomized, lindis
         u_rand = torch.rand((n, N), device=o.device)
     u = _f32(u_rand) if u_rand is not None else None
     t = torch.empty(n, N, device=o.device)
-    if in_sphere:
-        pts = torch.empty(n, N, 3, device=o.device)
-        with _on(o):
-            L.check(lib.neo_sample_along_rays(L.ptr(o), L.ptr(d), L.ptr(fr), n, num_samples, 1, float(far_uncontracted),
-                                              L.ptr(u), L.ptr(t), L.ptr(pts), None, _stream()))
-        return t, pts
-    pts = torch.empty(n, N, 4, device=o.device)
-    lin = torch.empty(n, N, 3, device=o.device)
-    with _on(o):
-        L.check(lib.neo_sample_along_rays(L.ptr(o), L.ptr(d), L.ptr(fr), n, num_samples, 0, float(far_uncontracted),
-                                          L.ptr(u), L.ptr(t), L.ptr(pts), L.ptr(lin), _stream()))
-    return t, pts, lin
+    pts = torch.empty(n, N, 3 if in_sphere else 4, device=o.device)
+    lin = None if in_sphere else torch.empty(n, N, 3, device=o.device)
+    with L.on(o) as s:
+        L.check(lib.neo_sample_along_rays(L.ptr(o), L.ptr(d), L.ptr(fr), n, num_samples, int(bool(in_sphere)), float(far_uncontracted),
+                                          L.ptr(u), L.ptr(t), L.ptr(pts), L.ptr(lin), s))
+    return (t, pts) if in_sphere else (t, pts, lin)
 
 
 def sample_pdf(t_vals, weights, origins, directions, num_samples, randomized, in_sphere, far, far_uncontracted=3.0,
@@ -186,18 +157,12 @@ def sample_pdf(t_vals, weights, origins, directions, num_samples, randomized, in
         u_rand = torch.rand((n, num_samples), device=o.device)
     u = _f32(u_rand) if u_rand is not None else None
     t = torch.empty(n, N1, device=o.device)
-    if in_sphere:
-        pts = torch.empty(n, N1, 3, device=o.device)
-        with _on(o):
-            L.check(lib.neo_sample_pdf(L.ptr(o), L.ptr(d), L.ptr(fr), L.ptr(t_old), L.ptr(w), n, n_old, num_samples, 1,
-                                       float(far_uncontracted), L.ptr(u), L.ptr(t), L.ptr(pts), None, _stream()))
-        return t, pts
-    pts = torch.empty(n, N1, 4, device=o.device)
-    lin = torch.empty(n, N1, 3, device=o.device)
-    with _on(o):
-        L.check(lib.neo_sample_pdf(L.ptr(o), L.ptr(d), L.ptr(fr), L.ptr(t_old), L.ptr(w), n, n_old, num_samples, 0,
-                                   float(far_uncontracted), L.ptr(u), L.ptr(t), L.ptr(pts), L.ptr(lin), _stream()))
-    return t, pts, lin
+    pts = torch.empty(n, N1, 3 if in_sphere else 4, device=o.device)
+    lin = None if in_sphere else torch.empty(n, N1, 3, device=o.device)
+    with L.on(o) as s:
+        L.check(lib.neo_sample_pdf(L.ptr(o), L.ptr(d), L.ptr(fr), L.ptr(t_old), L.ptr(w), n, n_old, num_samples, int(bool(in_sphere)),
+                                   float(far_uncontracted), L.ptr(u), L.ptr(t), L.ptr(pts), L.ptr(lin), s))
+    return (t, pts) if in_sphere else (t, pts, lin)
 
 
 def volumetric_rendering(rgb, density, t_vals, dirs, white_bkgd, in_sphere, t_far=None, out_depth=None):
@@ -208,10 +173,10 @@ def volumetric_rendering(rgb, density, t_vals, dirs, white_bkgd, in_sphere, t_fa
     comp = torch.empty(n, 3, device=t.device); acc = torch.empty(n, device=t.device)
     w = torch.empty(n, N, device=t.device); depth = torch.empty(n, device=t.device)
     lam = torch.empty(n, 1, device=t.device) if in_sphere else None
-    with _on(t):
+    with L.on(t) as s:
         L.check(lib.neo_volumetric_rendering(L.ptr(rgb), L.ptr(sig), L.ptr(t), L.ptr(d), L.ptr(far), n, N, int(bool(white_bkgd)),
                                              int(bool(in_sphere)), L.ptr(comp), L.ptr(acc), L.ptr(w), L.ptr(lam), L.ptr(depth),
-                                             _stream()))
+                                             s))
     if out_depth is not None:
         return comp, acc, w, lam, depth
     return comp, acc, w, lam

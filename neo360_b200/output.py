@@ -40,8 +40,8 @@ def psnr(pred: torch.Tensor, gt: torch.Tensor) -> float:
     if a.shape != b.shape:
         raise ValueError(f"shape mismatch {tuple(a.shape)} vs {tuple(b.shape)}")
     out = torch.zeros(1, dtype=torch.float64, device=a.device)
-    with torch.cuda.device(a.device):
-        L.check(L.load().neo_clipped_sq_err(a.data_ptr(), b.data_ptr(), a.numel(), out.data_ptr(), torch.cuda.current_stream().cuda_stream))
+    with L.on(a) as s:
+        L.check(L.load().neo_clipped_sq_err(L.ptr(a), L.ptr(b), a.numel(), L.ptr(out), s))
     mse = float(out.item()) / a.numel()
     return float("inf") if mse == 0 else -10.0 * math.log10(mse)
 
@@ -73,9 +73,8 @@ def psnr_obj_each(preds: Sequence[torch.Tensor], gts: Sequence[torch.Tensor], ma
             raise ValueError(f"frame {i}: the mask must be bool or uint8, not {m.dtype}")
         a, b, mk = p.contiguous().float(), g.contiguous().float(), m.contiguous().view(torch.uint8)
         keep.append((a, b, mk))
-        with torch.cuda.device(dev):
-            L.check(L.load().neo_clipped_sq_err_masked(a.data_ptr(), b.data_ptr(), mk.data_ptr(), mk.numel(), sums[i:].data_ptr(),
-                                                       counts[i:].data_ptr(), torch.cuda.current_stream().cuda_stream))
+        with L.on(dev) as s:
+            L.check(L.load().neo_clipped_sq_err_masked(L.ptr(a), L.ptr(b), L.ptr(mk), mk.numel(), L.ptr(sums[i:]), L.ptr(counts[i:]), s))
     out = []
     for s, c in zip(sums.tolist(), counts.tolist()):
         mse = s / c if c else float("nan")
@@ -96,12 +95,11 @@ def ssim_batch(pred: torch.Tensor, gt: torch.Tensor, return_map: bool = False):
     nbytes = lib.neo_ssim_workspace_bytes(n, H, W)
     if nbytes == 0:
         raise ValueError(f"SSIM needs n >= 1 frames of at least 11x11 pixels, got {tuple(pred.shape)}")
-    ws = torch.empty(nbytes // 8, dtype=torch.float64, device=a.device)
+    ws = L.workspace(nbytes, a.device)
     out = torch.empty(n, dtype=torch.float64, device=a.device)
     ss_map = torch.empty(n, H - 10, W - 10, 3, dtype=torch.float32, device=a.device) if return_map else None
-    with torch.cuda.device(a.device):
-        L.check(lib.neo_ssim(a.data_ptr(), b.data_ptr(), n, H, W, out.data_ptr(), None if ss_map is None else ss_map.data_ptr(),
-                             ws.data_ptr(), nbytes, torch.cuda.current_stream().cuda_stream))
+    with L.on(a) as s:
+        L.check(lib.neo_ssim(L.ptr(a), L.ptr(b), n, H, W, L.ptr(out), L.ptr(ss_map), L.ptr(ws), nbytes, s))
     return (out, ss_map) if return_map else out
 
 

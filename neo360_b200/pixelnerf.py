@@ -34,10 +34,6 @@ from .renderer import Scene
 from .training import _Composite, _PixelTrunkTC, _index_maps_bwd_det, check_train_precision, view_mean_head
 
 
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
-
-
 class NeRFMLP(nn.Module):
     """model_pixel.py:35-93 at the defaults PixelNeRF uses: trunk [enc 63 | latent 512] -> 128 x4, views 155 -> 128 -> 128, rgb 128 -> 3."""
 
@@ -81,7 +77,7 @@ class NeRFMLP(nn.Module):
             w = lin.weight.detach().float()
             k = -(-w.shape[1] // 64) * 64
             keep.append(F.pad(w, (0, k - w.shape[1])).half().contiguous())
-            return keep[-1].data_ptr()
+            return L.ptr(keep[-1])
 
         f = lambda x: (keep.append(x.detach().float().contiguous()) or L.ptr(keep[-1]))
         for i in range(4):
@@ -130,7 +126,8 @@ class _LatentLookup(torch.autograd.Function):
         M, Cc = pts.shape[0], latent_cl.shape[-1]
         lat = latent_cl.detach().contiguous()
         out = torch.empty(sc.nv * M, Cc, device=pts.device)
-        L.check(lib.neo_index_maps(sc.handle, L.ptr(pts), M, Cc, L.ptr(lat), None, None, None, L.ptr(out), None, _stream()))
+        with L.on(pts) as s:
+            L.check(lib.neo_index_maps(sc.handle, L.ptr(pts), M, Cc, L.ptr(lat), None, None, None, L.ptr(out), None, s))
         ctx.save_for_backward(pts)
         ctx.sc, ctx.shape = sc, latent_cl.shape
         ctx.det = torch.are_deterministic_algorithms_enabled()
@@ -146,7 +143,8 @@ class _LatentLookup(torch.autograd.Function):
         if ctx.det:
             _index_maps_bwd_det(sc, pts, M, ctx.shape[-1], g, None, g_lat, [None] * 3)
         else:
-            L.check(lib.neo_index_maps_bwd(sc.handle, L.ptr(pts), M, ctx.shape[-1], L.ptr(g), None, L.ptr(g_lat), None, None, None, _stream()))
+            with L.on(pts) as s:
+                L.check(lib.neo_index_maps_bwd(sc.handle, L.ptr(pts), M, ctx.shape[-1], L.ptr(g), None, L.ptr(g_lat), None, None, None, s))
         return None, g_lat, None
 
 
@@ -202,7 +200,8 @@ class PixelNeRF(nn.Module):
         d.planes_xz = d.planes_xy = d.planes_yz = d.latent = L.ptr(dummy)     # not read by a cameras-only scene
         d.src_poses, d.src_focal, d.src_c = L.ptr(poses), L.ptr(focal), L.ptr(c)
         h = C.c_void_p()
-        L.check(L.load().neo_scene_create(C.byref(d), (L.NeoMLPParams * 4)(), 0, C.byref(h), _stream()))
+        with L.on(poses) as s:
+            L.check(L.load().neo_scene_create(C.byref(d), (L.NeoMLPParams * 4)(), 0, C.byref(h), s))
         sc = Scene(h, 0)
         sc.nv = nv
         self._scene = (key, sc, src)
@@ -236,14 +235,15 @@ class PixelNeRF(nn.Module):
 
     def _sample(self, lvl, o, d, t, w, n, near, far, u):
         lib, dev = L.load(), o.device
-        if lvl == 0:
-            t1 = torch.empty(n, self.num_coarse_samples + 1, device=dev)
-            L.check(lib.neo_vanilla_sample_along_rays(L.ptr(o), L.ptr(d), n, self.num_coarse_samples, float(near), float(far), L.ptr(u), L.ptr(t1),
-                                                      _stream()))
-        else:       # bins = mids(t), weights[1:-1] of the detached level-0 weights (model_pixel.py:195-204)
-            t1 = torch.empty(n, t.shape[1] + self.num_fine_samples, device=dev)
-            L.check(lib.neo_sample_pdf(L.ptr(o), L.ptr(d), None, L.ptr(t), L.ptr(w.detach().contiguous()), n, t.shape[1], self.num_fine_samples,
-                                       1, 0.0, L.ptr(u), L.ptr(t1), None, None, _stream()))
+        with L.on(o) as s:
+            if lvl == 0:
+                t1 = torch.empty(n, self.num_coarse_samples + 1, device=dev)
+                L.check(lib.neo_vanilla_sample_along_rays(L.ptr(o), L.ptr(d), n, self.num_coarse_samples, float(near), float(far), L.ptr(u),
+                                                          L.ptr(t1), s))
+            else:       # bins = mids(t), weights[1:-1] of the detached level-0 weights (model_pixel.py:195-204)
+                t1 = torch.empty(n, t.shape[1] + self.num_fine_samples, device=dev)
+                L.check(lib.neo_sample_pdf(L.ptr(o), L.ptr(d), None, L.ptr(t), L.ptr(w.detach().contiguous()), n, t.shape[1],
+                                           self.num_fine_samples, 1, 0.0, L.ptr(u), L.ptr(t1), None, None, s))
         return t1
 
     def _field(self, r, sc, lat, t, lvl, precision: str):
@@ -251,14 +251,13 @@ class PixelNeRF(nn.Module):
         n, N = t.shape
         mlp = self._ensure_weights(precision)[lvl]
         rgb, sigma = torch.empty(n, N, 3, device=dev), torch.empty(n, N, device=dev)
-        if precision == "fp32":
-            L.check(lib.neo_pixelnerf_field(sc.handle, L.ptr(lat), C.byref(mlp), C.byref(r), L.ptr(t), N, L.ptr(rgb), L.ptr(sigma), _stream()))
-        else:
-            need = lib.neo_pixelnerf_tc_workspace_bytes(sc.nv, n * N)
-            if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-                self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
-            L.check(lib.neo_pixelnerf_field_tc(sc.handle, L.ptr(lat), C.byref(mlp), C.byref(r), L.ptr(t), N, L.ptr(rgb), L.ptr(sigma),
-                                               L.ptr(self._ws), self._ws.numel(), _stream()))
+        with L.on(t) as s:
+            if precision == "fp32":
+                L.check(lib.neo_pixelnerf_field(sc.handle, L.ptr(lat), C.byref(mlp), C.byref(r), L.ptr(t), N, L.ptr(rgb), L.ptr(sigma), s))
+            else:
+                self._ws = L.grow(self._ws, lib.neo_pixelnerf_tc_workspace_bytes(sc.nv, n * N), dev)
+                L.check(lib.neo_pixelnerf_field_tc(sc.handle, L.ptr(lat), C.byref(mlp), C.byref(r), L.ptr(t), N, L.ptr(rgb), L.ptr(sigma),
+                                                   L.ptr(self._ws), self._ws.numel(), s))
         return rgb, sigma
 
     @torch.no_grad()
@@ -269,11 +268,10 @@ class PixelNeRF(nn.Module):
         prec = precision or self.precision
         if prec not in ("fp32", "tc"):
             raise ValueError(f"PixelNeRF precision must be 'fp32' or 'tc', got {prec!r}")
-        r, (o, _, _) = self._rays(rays, chunk)
-        with torch.cuda.device(o.device):
-            lat = self._hoisted_latent(rays["src_imgs"])
-            sc = self._ensure_scene(rays, lat.shape[1:3])
-            return self._field(r, sc, lat, t.contiguous().float(), level, prec)
+        r, _ = self._rays(rays, chunk)
+        lat = self._hoisted_latent(rays["src_imgs"])
+        sc = self._ensure_scene(rays, lat.shape[1:3])
+        return self._field(r, sc, lat, t.contiguous().float(), level, prec)
 
     def density_grid(self, resolution, bbox=((-1.0, -1.0, -1.0), (1.0, 1.0, 1.0)), level: int = 1, precision: Optional[str] = None,
                      slab_rays: Optional[int] = None, batch: Optional[Dict[str, torch.Tensor]] = None) -> torch.Tensor:
@@ -292,7 +290,7 @@ class PixelNeRF(nn.Module):
         lib = L.load()
         r, (o, d, vd) = self._rays(rays, chunk)
         n, dev = o.shape[0], o.device
-        with torch.cuda.device(dev):
+        with L.on(dev) as s:
             lat = self._hoisted_latent(rays["src_imgs"])
             sc = self._ensure_scene(rays, lat.shape[1:3])
             u = self._uniforms(rays, randomized, n, dev)
@@ -303,7 +301,7 @@ class PixelNeRF(nn.Module):
                 rgb, sigma = self._field(r, sc, lat, t, lvl, self.precision)
                 comp, acc, w, depth = torch.empty(n, 3, device=dev), torch.empty(n, device=dev), torch.empty(n, N, device=dev), torch.empty(n, device=dev)
                 L.check(lib.neo_volumetric_rendering(L.ptr(rgb), L.ptr(sigma), L.ptr(t), L.ptr(d), None, n, N, int(bool(white_bkgd)), 2,
-                                                     L.ptr(comp), L.ptr(acc), L.ptr(w), None, L.ptr(depth), _stream()))
+                                                     L.ptr(comp), L.ptr(acc), L.ptr(w), None, L.ptr(depth), s))
                 ret.append((comp, acc, depth))
         return ret
 
@@ -315,7 +313,7 @@ class PixelNeRF(nn.Module):
         r, (o, d, vd) = self._rays(rays, chunk)
         n, dev = o.shape[0], o.device
         nv = self.num_src_views
-        with torch.cuda.device(dev):
+        with L.on(dev) as s:
             latent = self.encoder(rays["src_imgs"])
             lat_cl = latent.permute(0, 2, 3, 1)                         # channel-last: the lookup's layout, the projection contracts it
             if not tc:
@@ -328,7 +326,7 @@ class PixelNeRF(nn.Module):
                 N = t.shape[1]
                 M = n * N
                 enc, dtile, pts = torch.empty(nv * M, 63, device=dev), torch.empty(nv * M, 27, device=dev), torch.empty(M, 3, device=dev)
-                L.check(lib.neo_pixelnerf_encode(sc.handle, C.byref(r), L.ptr(t), N, L.ptr(enc), L.ptr(dtile), L.ptr(pts), _stream()))
+                L.check(lib.neo_pixelnerf_encode(sc.handle, C.byref(r), L.ptr(t), N, L.ptr(enc), L.ptr(dtile), L.ptr(pts), s))
                 if tc:
                     p0 = _LatentLookup.apply(pts, lat_cl @ mlp.pts_linears[0].weight[:, 63:].t(), sc)
                     raw_rgb, raw_sigma = _mlp_train_tc(mlp, enc[:, :3].reshape(nv, M, 3), dtile, p0, nv)

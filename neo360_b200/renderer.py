@@ -160,8 +160,8 @@ class NeRF_TP(nn.Module):
         for p in precisions:
             mask |= 1 << PRECISIONS[p]
         h = C.c_void_p()
-        with torch.cuda.device(dev):
-            L.check(lib.neo_scene_create(C.byref(d), arr, mask, C.byref(h), torch.cuda.current_stream().cuda_stream))
+        with L.on(dev) as s:
+            L.check(lib.neo_scene_create(C.byref(d), arr, mask, C.byref(h), s))
         self._scene = Scene(h, lib.neo_scene_bytes(h))
         self._scene.nv = nv
         self._scene.mask = mask
@@ -246,12 +246,8 @@ class NeRF_TP(nn.Module):
         order = rays.get("_ray_order")
         if order is not None:
             keep.append(order)
-            r.ray_order = order.data_ptr()
-        need = lib.neo_render_workspace_bytes(n, C.byref(cfg))
-        if need == 0:
-            raise RuntimeError("neo360_b200: " + lib.neo_last_error().decode())
-        if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+            r.ray_order = L.ptr(order)
+        self._ws = L.grow(self._ws, lib.neo_render_workspace_bytes(n, C.byref(cfg)), dev)
         out = L.NeoOut()
         T: Dict[str, list] = {}
 
@@ -260,7 +256,7 @@ class NeRF_TP(nn.Module):
             for lvl in range(2):
                 t = torch.empty(*[s(lvl) if callable(s) else s for s in shape_fn], device=dev)
                 T[name].append(t)
-                getattr(out, name)[lvl] = t.data_ptr()
+                getattr(out, name)[lvl] = L.ptr(t)
 
         NL = lambda lvl: N[lvl]
         want("comp_rgb", n, 3)
@@ -274,9 +270,8 @@ class NeRF_TP(nn.Module):
             want("fg_rgb_s", n, NL, 3); want("bg_rgb_s", n, NL, 3)
             if out_depth:
                 want("fg_w", n, NL); want("bg_w", n, NL)
-        with torch.cuda.device(dev):
-            L.check(lib.neo_render_fwd(sc.handle, C.byref(r), C.byref(cfg), C.byref(out), self._ws.data_ptr(), self._ws.numel(),
-                                       torch.cuda.current_stream().cuda_stream))
+        with L.on(dev) as s:
+            L.check(lib.neo_render_fwd(sc.handle, C.byref(r), C.byref(cfg), C.byref(out), L.ptr(self._ws), self._ws.numel(), s))
         ret = []
         for lvl in range(2):
             if out_depth:
@@ -318,18 +313,16 @@ class NeRF_TP(nn.Module):
         """encoder_tp_fusion_conv.py:122-209: samples (...,3) world -> (NV*M,128), rows ordered (view, point)."""
         pts = samples.reshape(-1, 3).contiguous().float()
         out = torch.empty(self._scene.nv * pts.shape[0], 128, device=pts.device)
-        with torch.cuda.device(pts.device):
-            L.check(L.load().neo_index_grid(self._scene.handle, L.ptr(pts), pts.shape[0], L.ptr(out),
-                                            torch.cuda.current_stream().cuda_stream))
+        with L.on(pts) as s:
+            L.check(L.load().neo_index_grid(self._scene.handle, L.ptr(pts), pts.shape[0], L.ptr(out), s))
         return out
 
     def get_local_feats(self, samples: torch.Tensor) -> torch.Tensor:
         """model.py:239-264: samples (...,3) world -> (NV*M,512)."""
         pts = samples.reshape(-1, 3).contiguous().float()
         out = torch.empty(self._scene.nv * pts.shape[0], 512, device=pts.device)
-        with torch.cuda.device(pts.device):
-            L.check(L.load().neo_index_local(self._scene.handle, L.ptr(pts), pts.shape[0], L.ptr(out),
-                                             torch.cuda.current_stream().cuda_stream))
+        with L.on(pts) as s:
+            L.check(L.load().neo_index_local(self._scene.handle, L.ptr(pts), pts.shape[0], L.ptr(out), s))
         return out
 
     def field_eval(self, rays, far, t_vals, mlp_index: int, chunk: int = 0, precision: Optional[str] = None,
@@ -347,13 +340,12 @@ class NeRF_TP(nn.Module):
             if ray_order.dtype != torch.int32 or ray_order.numel() != n or ray_order.device != t.device:
                 raise ValueError("ray_order must be an int32 permutation of the rays on their device")
             ray_order = ray_order.contiguous()
-            r.ray_order = ray_order.data_ptr()
+            r.ray_order = L.ptr(ray_order)
         rgb = torch.empty(n, N, 3, device=t.device)
         sig = torch.empty(n, N, 1, device=t.device)
-        with torch.cuda.device(t.device):
+        with L.on(t) as s:
             L.check(L.load().neo_field_eval(self._scene.handle, C.byref(r), L.ptr(fr), L.ptr(t), N, mlp_index,
-                                            PRECISIONS[precision or self.precision], L.ptr(rgb), L.ptr(sig),
-                                            torch.cuda.current_stream().cuda_stream))
+                                            PRECISIONS[precision or self.precision], L.ptr(rgb), L.ptr(sig), s))
         return rgb, sig
 
     def density_grid(self, resolution, bbox=((-1.0, -1.0, -1.0), (1.0, 1.0, 1.0)), level: int = 1, precision: Optional[str] = None,
@@ -364,7 +356,8 @@ class NeRF_TP(nn.Module):
 
     def check(self):
         """Synchronise and surface deferred device-side errors (the reference's asserts, helper.py:271,426)."""
-        L.check(L.load().neo_check_async(self._scene.handle, torch.cuda.current_stream().cuda_stream))
+        with L.on(self._scene_inputs[0]) as s:
+            L.check(L.load().neo_check_async(self._scene.handle, s))
 
     def _blocked_order(self, n: int, img_wh, dev) -> torch.Tensor:
         """Permutation visiting a row-major W x H frame in 8x4 pixel blocks: the 32 rays of a TC tile then hit neighbouring

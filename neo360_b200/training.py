@@ -33,26 +33,20 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib as L
-from . import ops
+from . import bf16, ops
 
 Tensor = torch.Tensor
-
-
-def _stream():
-    return torch.cuda.current_stream().cuda_stream
 
 
 def _index_maps_bwd_det(sc, p, M, Cc, g_local, g_world, g_lat, g_pl):
     """neo_index_maps_bwd_det (no floating-point atomics, bit-reproducible) with a workspace of the queried size; a None row gradient skips
     its maps."""
     lib = L.load()
-    need = lib.neo_index_maps_bwd_det_workspace_bytes(sc.handle, M, Cc)
-    if need == 0:
-        L.check(-1)
-    ws = torch.empty(need, dtype=torch.uint8, device=p.device)
+    ws = L.workspace(lib.neo_index_maps_bwd_det_workspace_bytes(sc.handle, M, Cc), p.device)
     f = lambda g: None if g is None else g.contiguous().float()
-    L.check(lib.neo_index_maps_bwd_det(sc.handle, L.ptr(p), M, Cc, L.ptr(f(g_local)), L.ptr(f(g_world)), L.ptr(g_lat), *[L.ptr(t) for t in g_pl],
-                                       L.ptr(ws), need, _stream()))
+    with L.on(p) as s:
+        L.check(lib.neo_index_maps_bwd_det(sc.handle, L.ptr(p), M, Cc, L.ptr(f(g_local)), L.ptr(f(g_world)), L.ptr(g_lat),
+                                           *[L.ptr(t) for t in g_pl], L.ptr(ws), ws.numel(), s))
 
 
 class _Lookup(torch.autograd.Function):
@@ -67,9 +61,9 @@ class _Lookup(torch.autograd.Function):
         M, nv = p.shape[0], sc.nv
         world = torch.empty(nv * M, 128, device=p.device)
         local = torch.empty(nv * M, 512, device=p.device)
-        with torch.cuda.device(p.device):
-            L.check(lib.neo_index_grid(sc.handle, L.ptr(p), M, L.ptr(world), _stream()))
-            L.check(lib.neo_index_local(sc.handle, L.ptr(p), M, L.ptr(local), _stream()))
+        with L.on(p) as s:
+            L.check(lib.neo_index_grid(sc.handle, L.ptr(p), M, L.ptr(world), s))
+            L.check(lib.neo_index_local(sc.handle, L.ptr(p), M, L.ptr(local), s))
         ctx.save_for_backward(p)
         ctx.net, ctx.scene = net, sc
         ctx.shapes = (planes_xz.shape, latent.shape)
@@ -85,14 +79,14 @@ class _Lookup(torch.autograd.Function):
         M = p.shape[0]
         g_planes = [torch.zeros(nv, hp, wp, cw, device=p.device) for _ in range(3)]
         g_lat = torch.zeros(nv, hl, wl, cl, device=p.device)
-        with torch.cuda.device(p.device):
-            if ctx.det:
-                _index_maps_bwd_det(sc, p, M, cw, None, g_world, None, g_planes)
-                _index_maps_bwd_det(sc, p, M, cl, g_local, None, g_lat, [None] * 3)
-            else:
+        if ctx.det:
+            _index_maps_bwd_det(sc, p, M, cw, None, g_world, None, g_planes)
+            _index_maps_bwd_det(sc, p, M, cl, g_local, None, g_lat, [None] * 3)
+        else:
+            with L.on(p) as s:
                 L.check(lib.neo_index_grid_bwd(sc.handle, L.ptr(p), M, L.ptr(g_world.contiguous().float()), L.ptr(g_planes[0]),
-                                               L.ptr(g_planes[1]), L.ptr(g_planes[2]), _stream()))
-                L.check(lib.neo_index_local_bwd(sc.handle, L.ptr(p), M, L.ptr(g_local.contiguous().float()), L.ptr(g_lat), _stream()))
+                                               L.ptr(g_planes[1]), L.ptr(g_planes[2]), s))
+                L.check(lib.neo_index_local_bwd(sc.handle, L.ptr(p), M, L.ptr(g_local.contiguous().float()), L.ptr(g_lat), s))
         nchw = lambda t: t.permute(0, 3, 1, 2)
         return None, nchw(g_planes[0]), nchw(g_planes[1]), nchw(g_planes[2]), nchw(g_lat), None
 
@@ -110,8 +104,8 @@ class _LookupMaps(torch.autograd.Function):
         maps = [t.detach().contiguous().float() for t in (lat_cl, xz_cl, xy_cl, yz_cl)]
         local = torch.empty(nv * M, Cc, device=p.device)
         world = torch.empty(nv * M, Cc, device=p.device)
-        with torch.cuda.device(p.device):
-            L.check(lib.neo_index_maps(sc.handle, L.ptr(p), M, Cc, *[L.ptr(t) for t in maps], L.ptr(local), L.ptr(world), _stream()))
+        with L.on(p) as s:
+            L.check(lib.neo_index_maps(sc.handle, L.ptr(p), M, Cc, *[L.ptr(t) for t in maps], L.ptr(local), L.ptr(world), s))
         ctx.save_for_backward(p)
         ctx.scene, ctx.C = sc, Cc
         ctx.shapes = (lat_cl.shape, xz_cl.shape)
@@ -126,13 +120,12 @@ class _LookupMaps(torch.autograd.Function):
         M = p.shape[0]
         g_lat = torch.zeros(ctx.shapes[0], device=p.device)
         g_pl = [torch.zeros(ctx.shapes[1], device=p.device) for _ in range(3)]
-        with torch.cuda.device(p.device):
-            if ctx.det:
-                _index_maps_bwd_det(sc, p, M, Cc, g_local, g_world, g_lat, g_pl)
-            else:
+        if ctx.det:
+            _index_maps_bwd_det(sc, p, M, Cc, g_local, g_world, g_lat, g_pl)
+        else:
+            with L.on(p) as s:
                 L.check(lib.neo_index_maps_bwd(sc.handle, L.ptr(p), M, Cc, L.ptr(g_local.contiguous().float()),
-                                               L.ptr(g_world.contiguous().float()), L.ptr(g_lat), L.ptr(g_pl[0]), L.ptr(g_pl[1]), L.ptr(g_pl[2]),
-                                               _stream()))
+                                               L.ptr(g_world.contiguous().float()), L.ptr(g_lat), L.ptr(g_pl[0]), L.ptr(g_pl[1]), L.ptr(g_pl[2]), s))
         return None, g_lat, g_pl[0], g_pl[1], g_pl[2], None
 
 
@@ -153,10 +146,10 @@ class _Composite(torch.autograd.Function):
         comp, acc = torch.empty(n, 3, device=dev), torch.empty(n, device=dev)
         w, depth = torch.empty(n, N, device=dev), torch.empty(n, device=dev)
         lam = torch.empty(n, 1, device=dev) if mode == 1 else torch.zeros(n, 1, device=dev)
-        with torch.cuda.device(dev):
+        with L.on(dev) as s:
             L.check(lib.neo_volumetric_rendering(L.ptr(rgb_c), L.ptr(sig_c), L.ptr(t_c), L.ptr(d_c), L.ptr(far_c), n, N, int(bool(white)),
                                                  mode, L.ptr(comp), L.ptr(acc), L.ptr(w), L.ptr(lam) if mode == 1 else None,
-                                                 L.ptr(depth), _stream()))
+                                                 L.ptr(depth), s))
         ctx.save_for_backward(rgb_c, sig_c, t_c, d_c, far_c)
         ctx.flags = (int(bool(white)), mode)
         return comp, acc, w, lam, depth
@@ -170,15 +163,15 @@ class _Composite(torch.autograd.Function):
         dev = t_c.device
         d_rgb, d_sig = torch.empty(n, N, 3, device=dev), torch.empty(n, N, device=dev)
         f = lambda g: None if g is None else g.contiguous().float()
-        with torch.cuda.device(dev):
+        with L.on(dev) as s:
             if mode == 2:
                 gs = [f(g_comp), f(g_acc), f(g_w), f(g_depth)]
                 L.check(lib.neo_vanilla_composite_bwd(L.ptr(rgb_c), L.ptr(sig_c), L.ptr(t_c), L.ptr(d_c), n, N, white,
-                                                      *[L.ptr(g) for g in gs], L.ptr(d_rgb), L.ptr(d_sig), _stream()))
+                                                      *[L.ptr(g) for g in gs], L.ptr(d_rgb), L.ptr(d_sig), s))
             else:
                 gs = [f(g_comp), f(g_acc), f(g_w), f(g_lam) if mode else None, f(g_depth)]
                 L.check(lib.neo_volumetric_rendering_bwd(L.ptr(rgb_c), L.ptr(sig_c), L.ptr(t_c), L.ptr(d_c), L.ptr(far_c), n, N, white, mode,
-                                                         *[L.ptr(g) for g in gs], L.ptr(d_rgb), L.ptr(d_sig), _stream()))
+                                                         *[L.ptr(g) for g in gs], L.ptr(d_rgb), L.ptr(d_sig), s))
         g_d = None
         if mode == 2 and ctx.needs_input_grad[3]:
             # alpha_i depends on sigma_i and |rays_d| only through sigma_i delta_i |rays_d|: dL/d|d| = sum_i g_sigma_i sigma_i / |d|
@@ -248,13 +241,6 @@ def _mlp_projected(mlp, enc: Tensor, dir_tile: Tensor, local_p: Tensor, world_p:
     return lin(mlp.rgb_layer, q), raw_sigma
 
 
-def _trunk_workspace(need: int, dev) -> Tensor:
-    """A byte buffer of the size a `*_train_workspace_bytes` query returned (0: the query refused the sizes)."""
-    if need == 0:
-        L.check(-1)
-    return torch.empty(need, dtype=torch.uint8, device=dev)
-
-
 def _trunk_grads(E: int, k3: int, dev) -> List[Tensor]:
     """Outputs of a trunk backward: gw0 (128, E), gb0, gw1 (128, 128), gb1, gw2 (128, 128), gb2, gw3 (128, k3), gb3."""
     return [torch.empty(128, E, device=dev), torch.empty(128, device=dev), torch.empty(128, 128, device=dev), torch.empty(128, device=dev),
@@ -274,12 +260,11 @@ class _TrunkTC(torch.autograd.Function):
         f = lambda t: t.detach().contiguous().float()
         cam_c, lp, wp = f(cam), f(local_p), f(world_p)
         ws = [f(t) for t in (w0e, b0, w1, b1, w2, b2, w3e, b3)]
-        need = lib.neo_field_train_workspace_bytes(nv, M, ich, 0)
-        saved = _trunk_workspace(need, cam.device)
+        saved = L.workspace(lib.neo_field_train_workspace_bytes(nv, M, ich, 0), cam.device)
         hbar = torch.empty(M, 128, device=cam.device)
-        with torch.cuda.device(cam.device):
+        with L.on(cam) as s:
             L.check(lib.neo_field_train_fwd(L.ptr(cam_c), L.ptr(lp), L.ptr(wp), nv, M, ich, *[L.ptr(t) for t in ws], L.ptr(hbar),
-                                            L.ptr(saved), need, _stream()))
+                                            L.ptr(saved), saved.numel(), s))
         ctx.save_for_backward(saved, ws[2], ws[4], ws[6])
         ctx.dims = (nv, M, ich)
         return hbar
@@ -290,13 +275,12 @@ class _TrunkTC(torch.autograd.Function):
         saved, w1, w2, w3e = ctx.saved_tensors
         nv, M, ich = ctx.dims
         E, dev = 21 * ich, saved.device
-        need = lib.neo_field_train_workspace_bytes(nv, M, ich, 1)
-        scratch = _trunk_workspace(need, dev)
+        scratch = L.workspace(lib.neo_field_train_workspace_bytes(nv, M, ich, 1), dev)
         d_pm = torch.empty(nv * M, 256, device=dev)
         g = _trunk_grads(E, 128 + E, dev)
-        with torch.cuda.device(dev):
+        with L.on(dev) as s:
             L.check(lib.neo_field_train_bwd(L.ptr(g_hbar.contiguous().float()), nv, M, ich, L.ptr(w1), L.ptr(w2), L.ptr(w3e), L.ptr(saved),
-                                            saved.numel(), L.ptr(d_pm), *[L.ptr(t) for t in g], L.ptr(scratch), need, _stream()))
+                                            saved.numel(), L.ptr(d_pm), *[L.ptr(t) for t in g], L.ptr(scratch), scratch.numel(), s))
         return (None, d_pm, d_pm, *g)
 
 
@@ -313,11 +297,11 @@ class _PixelTrunkTC(torch.autograd.Function):
         f = lambda t: t.detach().contiguous().float()
         cam_c, p0c = f(cam), f(p0)
         ws = [f(t) for t in (w0e, b0, w1, b1, w2, b2, w3, b3)]
-        saved = _trunk_workspace(lib.neo_pixelnerf_train_workspace_bytes(nv, M, 0), cam.device)
+        saved = L.workspace(lib.neo_pixelnerf_train_workspace_bytes(nv, M, 0), cam.device)
         hbar = torch.empty(M, 128, device=cam.device)
-        with torch.cuda.device(cam.device):
+        with L.on(cam) as s:
             L.check(lib.neo_pixelnerf_train_fwd(L.ptr(cam_c), L.ptr(p0c), nv, M, *[L.ptr(t) for t in ws], L.ptr(hbar), L.ptr(saved),
-                                                saved.numel(), _stream()))
+                                                saved.numel(), s))
         ctx.save_for_backward(saved, ws[2], ws[4], ws[6])
         ctx.dims = (nv, M)
         return hbar
@@ -328,13 +312,12 @@ class _PixelTrunkTC(torch.autograd.Function):
         saved, w1, w2, w3 = ctx.saved_tensors
         nv, M = ctx.dims
         dev = saved.device
-        need = lib.neo_pixelnerf_train_workspace_bytes(nv, M, 1)
-        scratch = _trunk_workspace(need, dev)
+        scratch = L.workspace(lib.neo_pixelnerf_train_workspace_bytes(nv, M, 1), dev)
         d_p0 = torch.empty(nv * M, 128, device=dev)
         g = _trunk_grads(63, 128, dev)
-        with torch.cuda.device(dev):
+        with L.on(dev) as s:
             L.check(lib.neo_pixelnerf_train_bwd(L.ptr(g_hbar.contiguous().float()), nv, M, L.ptr(w1), L.ptr(w2), L.ptr(w3), L.ptr(saved),
-                                                saved.numel(), L.ptr(d_p0), *[L.ptr(t) for t in g], L.ptr(scratch), need, _stream()))
+                                                saved.numel(), L.ptr(d_p0), *[L.ptr(t) for t in g], L.ptr(scratch), scratch.numel(), s))
         return (None, d_p0, *g)
 
 
@@ -377,14 +360,6 @@ def check_train_precision(p: str) -> str:
     return p
 
 
-def _bf16(*shape, dev):
-    return torch.empty(*shape, dtype=torch.bfloat16, device=dev)
-
-
-def _ceil64(x: int) -> int:
-    return (x + 63) // 64 * 64
-
-
 class _MLPTrainTC(torch.autograd.Function):
     """The dense layers of vanilla NeRF's NeRFMLP and Mip-NeRF 360's PropMLP / NeRFMLP on the tensor cores (csrc/dense_train.cu and
     gemm_tc.cu: bf16 operands, fp32 accumulation, no floating-point atomics).  `depth` ReLU layers of width W on feats (M, F), the
@@ -397,120 +372,104 @@ class _MLPTrainTC(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, depth, feats, *params):
-        lib = L.load()
-        dev, s = feats.device, _stream()
         M, F = feats.shape
         f = lambda t: t.detach().contiguous().float()
         P = [f(t) for t in params]
         ws = [(P[2 * i], P[2 * i + 1]) for i in range(depth)]
         wsig, bsig = P[2 * depth], P[2 * depth + 1]
         rgb = len(P) > 2 * depth + 2
-        W, Kf = ws[0][0].shape[0], _ceil64(F)
+        W, Kf = ws[0][0].shape[0], -(-F // 64) * 64
         skip = depth > 5
         fo = W if skip else 0
-        XS = _bf16(M, fo + Kf, dev=dev)                                          # [h4 | feats] (feats alone without a skip)
-        e = XS.data_ptr() + 2 * fo
-        fc = f(feats)
-        with torch.cuda.device(dev):
-            L.check(lib.neo_tc_pack_bf16(L.ptr(fc), M, F, F, e, Kf, fo + Kf, 0, s))
-            H, Wp, WT, X = [], [], [], []
+        bf = lambda *shape: torch.empty(*shape, dtype=torch.bfloat16, device=feats.device)
+        XS = bf(M, fo + Kf)                                                      # [h4 | feats] (feats alone without a skip)
+        with L.on(feats) as s:
+            bf16.pack(f(feats), XS[:, fo:], False, s)
+            H, WT, xs = [], [], []                                              # xs: each layer's input view
             for i, (w, b) in enumerate(ws):
-                kin = Kf if i == 0 else (W + Kf if skip and i == 5 else W)
-                wp = _bf16(W, kin, dev=dev)
-                L.check(lib.neo_tc_pack_bf16(L.ptr(w), W, w.shape[1], w.shape[1], wp.data_ptr(), kin, kin, 0, s))
-                Wp.append(wp)
+                xs.append(XS[:, fo:] if i == 0 else (XS if skip and i == 5 else H[-1]))
+                x = xs[-1]
+                wp = bf(W, x.shape[1])
+                bf16.pack(w, wp, False, s)
                 if i > 0:
-                    wt = _bf16(W, W, dev=dev)
-                    L.check(lib.neo_tc_pack_bf16(L.ptr(w), W, w.shape[1], w.shape[1], wt.data_ptr(), W, W, 1, s))
-                    WT.append(wt)
-                x = (e, fo + Kf) if i == 0 else ((XS.data_ptr(), W + Kf) if skip and i == 5 else (H[-1].data_ptr(), W))
-                X.append(x + (kin,))
-                h = XS if skip and i == 4 else _bf16(M, W, dev=dev)
-                L.check(lib.neo_tc_gemm_bf16(x[0], x[1], wp.data_ptr(), kin, L.ptr(b), h.data_ptr(), W + Kf if h is XS else W, M, W, kin, 0, s))
-                H.append(h)
+                    WT.append(bf(W, W))
+                    bf16.pack(w, WT[-1], True, s)
+                H.append(XS[:, :W] if skip and i == 4 else bf(M, W))
+                bf16.gemm(x, wp, b, H[-1], 0, s)
             hl = H[-1]
-            sig = torch.empty(M, 1, device=dev)
-            L.check(lib.neo_tc_rowdot_bf16(hl.data_ptr(), W, W, L.ptr(wsig), L.ptr(bsig), 1, M, L.ptr(sig), s))
+            sig = torch.empty(M, 1, device=feats.device)
+            bf16.rowdot(hl, wsig, bsig, sig, s)
             out, saved = (sig,), []
             if rgb:
-                wb, bb, wv = P[2 * depth + 2], P[2 * depth + 3], P[2 * depth + 4]
+                wb, bb, wv = P[2 * depth + 2:]
                 nb, nv = wb.shape[0], wv.shape[0]
-                wbp, wvp, wbt, wvt = _bf16(nb, W, dev=dev), _bf16(nv, nb, dev=dev), _bf16(W, nb, dev=dev), _bf16(nb, nv, dev=dev)
-                L.check(lib.neo_tc_pack_bf16(L.ptr(wb), nb, W, W, wbp.data_ptr(), W, W, 0, s))
-                L.check(lib.neo_tc_pack_bf16(L.ptr(wv), nv, nb, nb, wvp.data_ptr(), nb, nb, 0, s))
-                L.check(lib.neo_tc_pack_bf16(L.ptr(wb), nb, W, W, wbt.data_ptr(), W, nb, 1, s))
-                L.check(lib.neo_tc_pack_bf16(L.ptr(wv), nv, nb, nb, wvt.data_ptr(), nb, nv, 1, s))
-                beta = _bf16(M, nb, dev=dev)
-                yb = torch.empty(M, nv, device=dev)
-                L.check(lib.neo_tc_gemm_bf16(hl.data_ptr(), W, wbp.data_ptr(), W, L.ptr(bb), beta.data_ptr(), nb, M, nb, W, 1, s))
-                L.check(lib.neo_tc_gemm_bf16(beta.data_ptr(), nb, wvp.data_ptr(), nb, None, yb.data_ptr(), nv, M, nv, nb, 2, s))
+                wbp, wvp, wbt, wvt = bf(nb, W), bf(nv, nb), bf(W, nb), bf(nb, nv)
+                bf16.pack(wb, wbp, False, s)
+                bf16.pack(wv, wvp, False, s)
+                bf16.pack(wb, wbt, True, s)
+                bf16.pack(wv, wvt, True, s)
+                beta = bf(M, nb)
+                yb = torch.empty(M, nv, device=feats.device)
+                bf16.gemm(hl, wbp, bb, beta, 1, s)
+                bf16.gemm(beta, wvp, None, yb, 2, s)
                 out, saved = (sig, yb), [beta, wbt, wvt]
             # the input rows' gradient (pose refinement) reads W0^T and the skip layer's feature columns transposed, zero padded to Kf
             wft = []
             if feats.requires_grad:
                 for i, c0 in ((0, 0),) + (((5, W),) if skip else ()):
-                    w = ws[i][0]
-                    wt = torch.zeros(Kf, W, dtype=torch.bfloat16, device=dev)
-                    L.check(lib.neo_tc_pack_bf16(w.data_ptr() + 4 * c0, W, F, w.shape[1], wt.data_ptr(), F, W, 1, s))
+                    wt = torch.zeros(Kf, W, dtype=torch.bfloat16, device=feats.device)
+                    bf16.pack(ws[i][0][:, c0:c0 + F], wt[:F], True, s)
                     wft.append((i, wt))
-        ctx.save_for_backward(XS, *H, *WT, wsig, *saved)
+        ctx.save_for_backward(*xs, hl, *WT, wsig, *saved)
         ctx.wft = wft
-        ctx.meta = (depth, M, F, W, Kf, fo, X, [w.shape[1] for w, _ in ws], rgb)
+        ctx.meta = (depth, F, Kf, [w.shape for w, _ in ws], rgb)
         return out if rgb else sig
 
     @staticmethod
     def backward(ctx, g_sig, g_yb=None):
-        lib = L.load()
-        depth, M, F, W, Kf, fo, X, kvalid, rgb = ctx.meta
+        depth, F, Kf, wshapes, rgb = ctx.meta
         T = ctx.saved_tensors
-        XS, H, WT, wsig = T[0], T[1:1 + depth], T[1 + depth:2 * depth], T[2 * depth]
-        hl = H[-1]
-        dev, s = XS.device, _stream()
+        xs, hl, WT, wsig = T[:depth], T[depth], T[1 + depth:2 * depth], T[2 * depth]
+        (M, W), dev = hl.shape, hl.device
+        bf = lambda *shape: torch.empty(*shape, dtype=torch.bfloat16, device=dev)
         g_sig = torch.zeros(M, 1, device=dev) if g_sig is None else g_sig.contiguous().float()
-        calls = [(M, 64, W)] + [(M, W, x[2]) for x in X]
+        calls = [(64, W)] + [(W, x.shape[1]) for x in xs]
         if rgb:
             beta, wbt, wvt = T[2 * depth + 1:]
             nb, nv = beta.shape[1], wvt.shape[1]
-            calls += [(M, nv, nb), (M, nb, W)]
-        need = max(lib.neo_tc_wgrad_bf16_workspace_bytes(*c) for c in calls)
-        if need == 0:
-            L.check(-1)
-        ws = torch.empty(need, dtype=torch.uint8, device=dev)
-        wg = lambda dy, ldy, x, ldx, N, K, dw, kv, db: L.check(lib.neo_tc_wgrad_bf16(dy, ldy, x, ldx, M, N, K, L.ptr(dw), kv, L.ptr(db),
-                                                                                     L.ptr(ws), need, s))
-        G = [_bf16(M, W, dev=dev), _bf16(M, W, dev=dev)]
+            calls += [(nv, nb), (nb, W)]
+        ws = L.workspace(max(L.load().neo_tc_wgrad_bf16_workspace_bytes(M, N, K) for N, K in calls), dev)
+        G = [bf(M, W), bf(M, W)]
         grads = [None] * (2 * depth + 2)
         wft = dict(ctx.wft)
         g_in = {i: torch.empty(M, Kf, device=dev) for i in wft}
         extra = []
-        with torch.cuda.device(dev):
+        with L.on(dev) as s:
             if rgb:
                 g_yb = torch.zeros(M, nv, device=dev) if g_yb is None else g_yb.contiguous().float()
-                dyb, dbeta = _bf16(M, nv, dev=dev), _bf16(M, nb, dev=dev)
+                dyb, dbeta = bf(M, nv), bf(M, nb)
                 gwv, gwb, gbb = torch.empty(nv, nb, device=dev), torch.empty(nb, W, device=dev), torch.empty(nb, device=dev)
-                L.check(lib.neo_tc_pack_bf16(L.ptr(g_yb), M, nv, nv, dyb.data_ptr(), nv, nv, 0, s))
-                wg(dyb.data_ptr(), nv, beta.data_ptr(), nb, nv, nb, gwv, nb, None)
-                L.check(lib.neo_tc_dgrad_bf16(dyb.data_ptr(), nv, wvt.data_ptr(), nv, None, 0, None, None, dbeta.data_ptr(), nb, M, nb, nv, s))
-                wg(dbeta.data_ptr(), nb, hl.data_ptr(), W, nb, W, gwb, W, gbb)
-                L.check(lib.neo_tc_dgrad_bf16(dbeta.data_ptr(), nb, wbt.data_ptr(), nb, hl.data_ptr(), W, L.ptr(g_sig), L.ptr(wsig),
-                                              G[0].data_ptr(), W, M, W, nb, s))
+                bf16.pack(g_yb, dyb, False, s)
+                bf16.wgrad(dyb, beta, gwv, None, ws, s)
+                bf16.dgrad(dyb, wvt, None, None, None, dbeta, s)
+                bf16.wgrad(dbeta, hl, gwb, gbb, ws, s)
+                bf16.dgrad(dbeta, wbt, hl, g_sig, wsig, G[0], s)
                 extra = [gwb, gbb, gwv]
             else:
-                L.check(lib.neo_tc_relu_rank1_bf16(L.ptr(g_sig), L.ptr(wsig), hl.data_ptr(), W, M, W, G[0].data_ptr(), W, s))
-            gs = _bf16(M, 64, dev=dev)
+                bf16.relu_rank1(g_sig, wsig, hl, G[0], s)
+            gs = bf(M, 64)
             gwsig = torch.empty(64, W, device=dev)
-            L.check(lib.neo_tc_pack_bf16(L.ptr(g_sig), M, 1, 1, gs.data_ptr(), 64, 64, 0, s))
-            wg(gs.data_ptr(), 64, hl.data_ptr(), W, 64, W, gwsig, W, None)
+            bf16.pack(g_sig, gs, False, s)
+            bf16.wgrad(gs, hl, gwsig, None, ws, s)
             grads[2 * depth], grads[2 * depth + 1] = gwsig[:1].clone(), g_sig.sum(0)
             for i in range(depth - 1, -1, -1):
-                xp, ldx, kin = X[i]
-                gw, gb = torch.empty(W, kvalid[i], device=dev), torch.empty(W, device=dev)
-                wg(G[0].data_ptr(), W, xp, ldx, W, kin, gw, kvalid[i], gb)
+                gw, gb = torch.empty(wshapes[i], device=dev), torch.empty(W, device=dev)
+                bf16.wgrad(G[0], xs[i], gw, gb, ws, s)
                 grads[2 * i], grads[2 * i + 1] = gw, gb
                 if i in wft:        # dL/dz_i . W_i[:, feature columns] in fp32 (fp32 epilogue of the bf16 GEMM)
-                    L.check(lib.neo_tc_gemm_bf16(G[0].data_ptr(), W, wft[i].data_ptr(), W, None, g_in[i].data_ptr(), Kf, M, Kf, W, 2, s))
+                    bf16.gemm(G[0], wft[i], None, g_in[i], 2, s)
                 if i > 0:
-                    L.check(lib.neo_tc_dgrad_bf16(G[0].data_ptr(), W, WT[i - 1].data_ptr(), W, xp, ldx, None, None, G[1].data_ptr(), W, M, W, W, s))
+                    bf16.dgrad(G[0], WT[i - 1], xs[i][:, :W], None, None, G[1], s)
                     G.reverse()
         g_feats = None
         if g_in:
@@ -613,8 +572,8 @@ class _Distortion(torch.autograd.Function):
         wc, mc, ic = (t.detach().contiguous().float() for t in (w, m, interval))
         n, N = wc.shape
         out = torch.empty(n, device=wc.device)
-        with torch.cuda.device(wc.device):
-            L.check(lib.neo_distortion_loss(L.ptr(wc), L.ptr(mc), L.ptr(ic), 0.0, n, N, L.ptr(out), _stream()))
+        with L.on(wc) as s:
+            L.check(lib.neo_distortion_loss(L.ptr(wc), L.ptr(mc), L.ptr(ic), 0.0, n, N, L.ptr(out), s))
         ctx.save_for_backward(wc, mc, ic)
         return out
 
@@ -624,8 +583,8 @@ class _Distortion(torch.autograd.Function):
         wc, mc, ic = ctx.saved_tensors
         n, N = wc.shape
         d_w = torch.empty_like(wc)
-        with torch.cuda.device(wc.device):
-            L.check(lib.neo_distortion_loss_bwd(L.ptr(wc), L.ptr(mc), L.ptr(ic), 0.0, n, N, L.ptr(g.contiguous().float()), L.ptr(d_w), _stream()))
+        with L.on(wc) as s:
+            L.check(lib.neo_distortion_loss_bwd(L.ptr(wc), L.ptr(mc), L.ptr(ic), 0.0, n, N, L.ptr(g.contiguous().float()), L.ptr(d_w), s))
         return d_w, None, None
 
 

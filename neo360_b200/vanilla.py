@@ -95,8 +95,8 @@ class _VanillaEncode(torch.autograd.Function):
         o_c, vd_c, t_c = (x.detach().contiguous().float() for x in (o, vd, t))
         n, N = t_c.shape
         enc, denc = torch.empty(n * N, 63, device=o_c.device), torch.empty(n, 27, device=o_c.device)
-        with torch.cuda.device(o_c.device):
-            L.check(lib.neo_vanilla_encode(L.ptr(o_c), L.ptr(vd_c), L.ptr(t_c), n, N, L.ptr(enc), L.ptr(denc), torch.cuda.current_stream().cuda_stream))
+        with L.on(o_c) as s:
+            L.check(lib.neo_vanilla_encode(L.ptr(o_c), L.ptr(vd_c), L.ptr(t_c), n, N, L.ptr(enc), L.ptr(denc), s))
         ctx.save_for_backward(o_c, vd_c, t_c)
         return enc, denc
 
@@ -109,9 +109,9 @@ class _VanillaEncode(torch.autograd.Function):
         g_enc = torch.zeros(n * N, 63, device=dev) if g_enc is None else g_enc.contiguous().float()
         g_denc = torch.zeros(n, 27, device=dev) if g_denc is None else g_denc.contiguous().float()
         g_o, g_vd = torch.empty(n, 3, device=dev), torch.empty(n, 3, device=dev)
-        with torch.cuda.device(dev):
+        with L.on(dev) as s:
             L.check(lib.neo_vanilla_encode_bwd(L.ptr(o_c), L.ptr(vd_c), L.ptr(t_c), n, N, L.ptr(g_enc), L.ptr(g_denc), L.ptr(g_o), L.ptr(g_vd),
-                                               torch.cuda.current_stream().cuda_stream))
+                                               s))
         return g_o, g_vd, None
 
 
@@ -138,8 +138,8 @@ class NeRF(nn.Module):
             keep = []
             arr = (L.NeoVanillaMLPParams * 2)(self.coarse_mlp.to(dev).c_params(keep), self.fine_mlp.to(dev).c_params(keep))
             h = C.c_void_p()
-            with torch.cuda.device(dev):
-                L.check(lib.neo_vanilla_create(arr, C.byref(h), torch.cuda.current_stream().cuda_stream))
+            with L.on(dev) as s:
+                L.check(lib.neo_vanilla_create(arr, C.byref(h), s))
             self._handle, self._key = h, tuple((p.data_ptr(), p._version) for p in self.parameters())
         return self._handle
 
@@ -178,11 +178,7 @@ class NeRF(nn.Module):
         r = L.NeoRays()
         r.n_rays, r.chunk = n, 0
         r.rays_o, r.rays_d, r.viewdirs = L.ptr(o), L.ptr(d), L.ptr(vd)
-        need = lib.neo_vanilla_workspace_bytes(n, C.byref(cfg))
-        if need == 0:
-            raise RuntimeError("neo360_b200: " + lib.neo_last_error().decode())
-        if self._ws is None or self._ws.numel() < need or self._ws.device != dev:
-            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        self._ws = L.grow(self._ws, lib.neo_vanilla_workspace_bytes(n, C.byref(cfg)), dev)
         out = L.NeoVanillaOut()
         T = {k: [] for k in L.VANILLA_OUT_FIELDS}
         N = (nc + 1, nc + 1 + nf)
@@ -193,10 +189,9 @@ class NeRF(nn.Module):
             for k, shp in shapes.items():
                 t = torch.empty(*shp, device=dev)
                 T[k].append(t)
-                getattr(out, k)[lvl] = t.data_ptr()
-        with torch.cuda.device(dev):
-            L.check(lib.neo_vanilla_render_fwd(h, C.byref(r), C.byref(cfg), C.byref(out), self._ws.data_ptr(), self._ws.numel(),
-                                               torch.cuda.current_stream().cuda_stream))
+                getattr(out, k)[lvl] = L.ptr(t)
+        with L.on(dev) as s:
+            L.check(lib.neo_vanilla_render_fwd(h, C.byref(r), C.byref(cfg), C.byref(out), L.ptr(self._ws), self._ws.numel(), s))
         if debug:
             self.last_debug = T
         return [(T["comp_rgb"][lvl], T["acc"][lvl], T["depth"][lvl]) for lvl in range(2)]
@@ -219,15 +214,15 @@ class NeRF(nn.Module):
         h = self._ensure(dev)
         P = {"fp32": L.NEO_PREC_FP32, "tc": L.NEO_PREC_TC}[prec]
         need = lib.neo_vanilla_field_workspace_bytes(n * N, P)
-        if need and (self._ws is None or self._ws.numel() < need or self._ws.device != dev):
-            self._ws = torch.empty(need, dtype=torch.uint8, device=dev)
+        if need:            # 0: the fp32 field needs no workspace
+            self._ws = L.grow(self._ws, need, dev)
         r = L.NeoRays()
         r.n_rays, r.chunk = n, 0
         r.rays_o, r.rays_d, r.viewdirs = L.ptr(o), L.ptr(vd), L.ptr(vd)
         rgb, sigma = torch.empty(n, N, 3, device=dev), torch.empty(n, N, device=dev)
-        with torch.cuda.device(dev):
+        with L.on(dev) as s:
             L.check(lib.neo_vanilla_field_eval(h, C.byref(r), L.ptr(t), N, int(level), P, L.ptr(rgb), L.ptr(sigma),
-                                               self._ws.data_ptr() if need else None, need, torch.cuda.current_stream().cuda_stream))
+                                               L.ptr(self._ws) if need else None, need, s))
         return rgb, sigma
 
     def density_grid(self, resolution, bbox=((-1.0, -1.0, -1.0), (1.0, 1.0, 1.0)), level: int = 1, precision: Optional[str] = None,
@@ -253,27 +248,26 @@ class NeRF(nn.Module):
         if randomized:
             u = rays.get("_uniforms") or [torch.rand((n, nc + 1), device=dev), torch.rand((n, nf), device=dev)]   # helper.py:438, 587
             u = [x.contiguous().float() for x in u]
-        stream = torch.cuda.current_stream(dev).cuda_stream
         tc = check_train_precision(self.train_precision) == "tc"
         ray_grad = o.requires_grad or vd.requires_grad
         ret, t, w = [], None, None
         dbg = {"t": [], "weights": []}
         for lvl, mlp in enumerate((self.coarse_mlp, self.fine_mlp)):
-            with torch.cuda.device(dev):
+            with L.on(dev) as s:
                 if lvl == 0:
                     t = torch.empty(n, nc + 1, device=dev)
-                    L.check(lib.neo_vanilla_sample_along_rays(L.ptr(o.detach()), L.ptr(vd.detach()), n, nc, float(near), float(far), L.ptr(u[0]), L.ptr(t), stream))
+                    L.check(lib.neo_vanilla_sample_along_rays(L.ptr(o.detach()), L.ptr(vd.detach()), n, nc, float(near), float(far), L.ptr(u[0]), L.ptr(t), s))
                 else:       # bins = mids(t), weights[1:-1] of the DETACHED level-0 weights (helper.py:613)
                     t1 = torch.empty(n, t.shape[1] + nf, device=dev)
                     L.check(lib.neo_sample_pdf(L.ptr(o.detach()), L.ptr(vd.detach()), None, L.ptr(t), L.ptr(w.detach().contiguous()), n, t.shape[1], nf, 1, 0.0,
-                                               L.ptr(u[1]), L.ptr(t1), None, None, stream))
+                                               L.ptr(u[1]), L.ptr(t1), None, None, s))
                     t = t1
                 N = t.shape[1]
                 if ray_grad:
                     enc, denc = _VanillaEncode.apply(o, vd, t)
                 else:
                     enc, denc = torch.empty(n * N, 63, device=dev), torch.empty(n, 27, device=dev)
-                    L.check(lib.neo_vanilla_encode(L.ptr(o), L.ptr(vd), L.ptr(t), n, N, L.ptr(enc), L.ptr(denc), stream))
+                    L.check(lib.neo_vanilla_encode(L.ptr(o), L.ptr(vd), L.ptr(t), n, N, L.ptr(enc), L.ptr(denc), s))
             if tc:
                 raw_sigma, raw_rgb = mlp_train_tc(mlp, enc, denc, n, N)
                 raw_sigma = raw_sigma.reshape(n, N, 1)
